@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- FEAR-XS per-frame inference throughput on B200 (BASELINE.json metric).
+"""bench.py -- FEAR-XS per-frame inference throughput on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path (FEARNet.track + box decode) over one batch of synthetic
 crops: 256 search crops (3x256x256 fp32, ImageNet-normalised uniform uint8, seed 20260924) with
@@ -36,7 +36,7 @@ def load_peaks():
     if os.path.isfile(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 def load_state():
@@ -60,7 +60,7 @@ def synthetic_batch(batch, rank, with_u8=False):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -217,7 +217,7 @@ def read_video(path):
 
 def run_stream(net, dev, repeat=2):
     """BASELINE config 3: FEARTracker.update over the demo clip (tests/golden/test.mp4, 661 frames 480x256, init box
-    [163,53,45,174]); sequentially dependent frames, batch 1, one B200.  frames/s includes host crop/resize, H2D,
+    [163,53,45,174]); sequentially dependent frames, batch 1, one H100.  frames/s includes host crop/resize, H2D,
     kernels, D2H of the box record; also the device-only time of the per-frame step and the agreement with the
     reference's trajectory (golden fixture recorded from the reference's own source)."""
     import feartracker_b200 as fb
@@ -317,8 +317,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--batch", type=int, default=256, help="frames per GPU per step")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--corr", default=None, help="correlation kernel implementation: ffma | tcgen05")
-    ap.add_argument("--pw", default=None, help="1x1-conv implementation: ffma | tcgen05")
+    ap.add_argument("--corr", default=None, help="correlation kernel implementation: ffma | wgmma")
+    ap.add_argument("--pw", default=None, help="1x1-conv implementation: ffma | wgmma")
     ap.add_argument("--dw", default=None, help="depthwise implementation: pixel | strip | roll | auto")
     ap.add_argument("--dw-wide", type=int, default=None)
     ap.add_argument("--fuse", type=int, default=None, help="1 = fused pw-expand+dw kernels for the stride-2 blocks")
@@ -331,8 +331,14 @@ def main():
                     help="batch = BASELINE config 2/4 (default, the contract line); stream = config 3 only")
     ap.add_argument("--no-stream", action="store_true", help="skip the config-3 streaming measurement")
     ap.add_argument("--no-parity", action="store_true", help="skip the post-run oracle parity check")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the box records of the last timed step to DIR/boxes.npy (float64 [frames][8]: "
+                         "x, y, w, h, score, row, col, flat)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
+    if args.dump_outputs and (args.impl == "reference" or args.workload == "stream"):
+        ap.error("--dump-outputs writes the box records of the batched GPU workload; it does not apply to "
+                 "--impl reference or --workload stream")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -427,7 +433,7 @@ def main():
         sync_all()
         a.record(stream)
         for _ in range(steps):
-            fn()
+            timed.last = fn()
         b.record(stream)
         sync_all()
         ms = torch.tensor([a.elapsed_time(b)], device=dev)
@@ -451,6 +457,12 @@ def main():
     clocks.__exit__()
     launches = (net.launch_count() - l0) // (args.steps + (extra if ms_total < 400.0 else 0))
     fps = total * args.steps / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path received in its last step (inputs are a function of the seed alone)
+        rec = net.boxes_to_numpy(timed.last)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "boxes.npy"),
+                np.stack([rec[k].astype(np.float64) for k in ("x", "y", "w", "h", "score", "row", "col", "flat")], 1))
 
     for _ in range(args.warmup):
         step_e2e()
@@ -475,14 +487,9 @@ def main():
         per_launch_s = corr_ms * 1e-3 / corr_n
         bytes_per_launch = CORR_BYTES_PER_FRAME * B / (corr_n / args.steps)  # one launch covers both branches
         achieved = bytes_per_launch / per_launch_s / 1e9
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "corr_traffic.json")
-        if os.path.isfile(tpath):
-            with open(tpath) as f:
-                traffic = json.load(f).get("dram_bytes_per_launch")
         roofline = {
-            "kernel": "tc::corr_ts_kernel -- pixel-wise correlation, both head branches in one launch", "bound": "hbm",
-            "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "kernel": "tc::corr_tc_kernel -- pixel-wise correlation, both head branches in one launch", "bound": "hbm",
+            "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
             "peak_source": peak_src, "us_per_launch": per_launch_s * 1e6,
             "algorithmic_bytes_per_launch": int(bytes_per_launch),
             "how": "CUDA events around every correlation launch inside K extra steps (includes the launch latency the event "

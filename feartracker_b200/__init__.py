@@ -1,4 +1,4 @@
-"""feartracker_b200 -- B200-native (sm_100a) implementation of the FEAR-XS per-frame inference hot
+"""feartracker_b200 -- H100-native (sm_90a) implementation of the FEAR-XS per-frame inference hot
 path behind the reference's FEARNet / FEARTracker API.  See DESIGN.md."""
 from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY  # noqa: F401
 from .fear_net import FEARNet  # noqa: F401

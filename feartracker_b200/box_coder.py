@@ -36,7 +36,7 @@ class FEARBoxCoder:
                        use_sigmoid: bool = True) -> np.ndarray:
         """Structured array (x, y, w, h float64; score; row; col; flat) per frame."""
         if not (regression_map.is_cuda and classification_map.is_cuda):
-            raise RuntimeError("FEARBoxCoder.decode (B200) needs CUDA tensors: there is no CPU path")
+            raise RuntimeError("FEARBoxCoder.decode (H100) needs CUDA tensors: there is no CPU path")
         reg = regression_map.detach().float().contiguous()
         cls = classification_map.detach().float().contiguous()
         b = reg.shape[0]

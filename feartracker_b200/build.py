@@ -1,8 +1,8 @@
-"""Build libfear_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libfear_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m feartracker_b200.build [--force]
 
-The shared object is git-ignored but travels to the GPU box with the repo snapshot.
+The shared object is a build product and is not tracked by git.
 """
 import os
 import shutil
@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libfear_b200.so")
 SOURCES = ["fear_context.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

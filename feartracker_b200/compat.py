@@ -1,5 +1,5 @@
 """Config / CLI glue so the reference's ``demo_video.py`` (reference demo_video.py:1-62) and any script written against
-``model_training.*`` run UNMODIFIED on the B200 implementation, on a machine that has none of hydra / omegaconf /
+``model_training.*`` run UNMODIFIED on the H100 implementation, on a machine that has none of hydra / omegaconf /
 fire / imageio installed (this image) and no reference package on the path.
 
 Two pieces:
@@ -13,7 +13,7 @@ Two pieces:
   ``.tracker.fear_tracker`` / ``.dataset.box_coder`` / ``.utils.{torch,hydra,constants}`` mapped onto
   feartracker_b200, plus ``hydra.utils``, ``fire`` and ``imageio.v3`` (cv2-backed) -- each ONLY when the real module
   is not importable.  After that ``_target_: model_training.model.fear_net.FEARNet`` in the reference's own YAML tree
-  instantiates the B200 FEARNet.
+  instantiates the H100 FEARNet.
 
 Not a general Hydra: no config groups inside groups, no sweeps, no resolvers besides plain key interpolation (the
 ``hydra:`` node, whose ``${now:...}`` needs one, is dropped from the result exactly as ``compose()`` drops it).

@@ -1,4 +1,4 @@
-// libfear_b200.so -- executor + C ABI of the FEAR-XS hot path on B200 (sm_100a).
+// libfear_b200.so -- executor + C ABI of the FEAR-XS hot path on H100 (sm_90a).
 // See include/fear_b200.h for the contract and DESIGN.md for the data layout.
 #include <cuda_runtime.h>
 
@@ -61,18 +61,17 @@ enum Stage {
 static const char* kStageNames[ST_COUNT] = {"stem",    "backbone_pw", "backbone_dw", "neck",   "head_dw",
                                             "head_pw", "corr",        "pred",        "decode", "layout"};
 
-enum Impl { IMPL_FFMA = 0, IMPL_TC = 1 };  // CUDA cores (FFMA baseline / fallback shapes) | tcgen05
+enum Impl { IMPL_FFMA = 0, IMPL_TC = 1 };  // CUDA cores (FFMA baseline / fallback shapes) | wgmma
 
 struct Options {
-  int corr = -1;  // -1 = auto: tcgen05 when the tensor-core path initialised on this device, else CUDA cores
+  int corr = -1;  // -1 = auto: wgmma when the tensor-core path initialised on this device, else CUDA cores
   int pw = -1;
   int fuse_dwpw = 15; // bit mask: 1 = IRF blocks on 16x16 maps, 4 = also the IRF blocks on 32x32 maps, 2 = head SepConvs run
-                      // depthwise + 1x1 as one tcgen05 kernel (pw_tc_kernel<DWK, MW>): bit-identical to the unfused pair,
-                      // the depthwise maps are never written.  Round 2: 3.56 -> 3.40 ms / step, -2.3 GB DRAM traffic / step.
+                      // depthwise + 1x1 as one wgmma kernel (pw_tc_kernel<NT, DWK, MW>): bit-identical to the unfused pair,
+                      // the depthwise maps are never written.
                       // 8 = the expand-1 blocks (xif2_2, xif2_3: dw 3x3 -> 1x1 24 -> 24 -> + x) as one CUDA-core kernel
-  int pw_ts = 1;      // 1: plain 1x1 GEMMs take their A operand from tensor memory (pw_tc_kernel<0, 16, true>); 0: from shared memory
   int fuse_stem = 1;  // 1: stem + xif1_0 in one kernel (stem_xif1_fused_kernel) when the map tiles by 16x32
-  int fuse_irf = 1;   // 1: xif2_0 (expand -> depthwise s2 -> project) as ONE tcgen05 kernel (irf_s2_fused_kernel)
+  int fuse_irf = 1;   // 1: xif2_0 (expand -> depthwise s2 -> project) as ONE wgmma kernel (irf_s2_fused_kernel)
   int dw = 3;  // 3 = auto (default); 0 = one pixel per thread, 1 = register-strip kernel, 2 = rolling-window kernel,
                // 6 = TMA pipeline only where it applies (auto also uses it)
 };
@@ -81,7 +80,7 @@ static inline int effective(int impl) { return impl >= 0 ? impl : (tc::available
 
 struct PwW {
   const float* w = nullptr;  // [cout][cin]
-  const float* w_hi = nullptr;  // tf32 split of w for the tcgen05 path: w ~= w_hi + w_lo
+  const float* w_hi = nullptr;  // tf32 split of w for the tensor-core path: w ~= w_hi + w_lo
   const float* w_lo = nullptr;
   const float* b = nullptr;
   const float* h_w = nullptr;  // host copies (persistent): small layers pass their weights by value
@@ -117,7 +116,6 @@ struct FearContext {
   Options opt;
   float* d_weights = nullptr;
   float* d_irf_image = nullptr;  // packed shared-memory weights image of the fused xif2_0 kernel
-  unsigned long long* d_irf_dbg = nullptr;  // FEAR_IRF_TIMING builds only
   std::vector<float> h_weights;  // host mirror of d_weights (device layout)
   const float *stem_w = nullptr, *stem_b = nullptr;
   BlockW blocks[kNumBlocks];
@@ -224,8 +222,8 @@ static int launch_pw(FearContext* c, int stage, cudaStream_t s, const float* A, 
   }
   if (pw_impl == IMPL_TC && tc::pw_supported(w.cin, w.cout)) {
     LaunchScope scope(c, stage, s);
-    int r = tc::launch_pw(s, A, lda, w.w_hi, w.w_lo, w.b, R, ldr, C, ldc, M, w.cout, w.cin, relu, c->opt.pw_ts != 0);
-    if (r) return set_err(r, "tcgen05 pw launch failed (%d)", r);
+    int r = tc::launch_pw(s, A, lda, w.w_hi, w.w_lo, w.b, R, ldr, C, ldc, M, w.cout, w.cin, relu);
+    if (r) return set_err(r, "wgmma pw launch failed (%d)", r);
     return check_launch("tc::pw");
   }
   return launch_gemm_ffma(c, stage, s, A, lda, 0, w.w, w.cin, 0, w.b, R, ldr, C, ldc, 0, M, w.cout, w.cin, relu, 1);
@@ -345,7 +343,7 @@ static int launch_corr(FearContext* c, const Options& opt, cudaStream_t s, const
   if (corr_impl == IMPL_TC) {
     LaunchScope scope(c, ST_CORR, s);
     int r = tc::launch_corr(s, zt, Bz, cat, B, groups);
-    if (r) return set_err(r, "tcgen05 corr launch failed (%d)", r);
+    if (r) return set_err(r, "wgmma corr launch failed (%d)", r);
     return check_launch("tc::corr");
   }
   for (int g = 0; g < groups; ++g) {
@@ -371,7 +369,7 @@ static int run_blocks(FearContext* c, cudaStream_t s, float* X, int B, int& h, i
     if (i == 1 && c->opt.fuse_irf && tc::available() && effective(c->opt.pw) == IMPL_TC && c->d_irf_image) {
       // xif2_0: expand 1x1 -> depthwise 3x3 s2 -> project 1x1 in ONE kernel; the expanded tensor stays on the SM
       LaunchScope scope(c, ST_BACKBONE_PW, s);
-      int r = tc::launch_irf_s2(s, X, Y, c->d_irf_image, B, h, w, c->d_irf_dbg);
+      int r = tc::launch_irf_s2(s, X, Y, c->d_irf_image, B, h, w);
       if (r < 0) return set_err(FEAR_EINVAL, "fused IRF block launch failed (%d)", r);
       if (r == 0) {
         FEAR_TRY(check_launch("tc::irf_s2_fused_kernel"));
@@ -409,7 +407,7 @@ static int run_blocks(FearContext* c, cudaStream_t s, float* X, int B, int& h, i
     if ((c->opt.fuse_dwpw & 1) && tc::available() && sp.stride == 1 && sp.has_pw() && w == h &&
         (h == 16 || (h == 32 && (c->opt.fuse_dwpw & 4))) &&
         effective(c->opt.pw) == IMPL_TC) {
-      // depthwise + project 1x1 in one tcgen05 kernel (the depthwise map is never written)
+      // depthwise + project 1x1 in one wgmma kernel (the depthwise map is never written)
       LaunchScope scope(c, ST_BACKBONE_PW, s);
       int r = tc::launch_pw_dw(s, E, B, sp.k, bw.dw.w, bw.dw.b, 1, bw.pwl.w_hi, bw.pwl.w_lo, bw.pwl.b,
                                sp.residual() ? X : nullptr, sp.cout, Y, sp.cout, sp.cout, sp.mid(), 0, h);
@@ -503,7 +501,7 @@ static int run_features(FearContext* c, cudaStream_t s, const void* img, int B, 
 
 // F: NHWC search features [B][256][256]; zt: [Bz][64][256]; outputs NCHW maps.
 // SepConv of the head (blocks.py:45-72): depthwise 3x3 (no bias, no activation) then 1x1 (+bias, ReLU).
-// With the experimental "fuse_dwpw" bit 2 the pair runs as one tcgen05 kernel (the depthwise map is not written).
+// With the experimental "fuse_dwpw" bit 2 the pair runs as one wgmma kernel (the depthwise map is not written).
 static int launch_sepconv(FearContext* c, cudaStream_t s, const float* X, const DwW& dw, const PwW& pw, float* out,
                           int ldc, int B) {
   const int M = B * kScorePix;
@@ -594,8 +592,8 @@ extern "C" int fear_init(int device) {
   if (device < 0 || device >= n) return set_err(FEAR_EINVAL, "device %d out of range (%d devices)", device, n);
   cudaDeviceProp p;
   CUDA_TRY(cudaGetDeviceProperties(&p, device));
-  if (p.major != 10)
-    return set_err(FEAR_ENODEV, "device %d is sm_%d%d; libfear_b200 is built for sm_100a only", device, p.major, p.minor);
+  if (p.major != 9)
+    return set_err(FEAR_ENODEV, "device %d is sm_%d%d; libfear_b200 is built for sm_90a only", device, p.major, p.minor);
   CUDA_TRY(cudaSetDevice(device));
   if (tc::dev_state().inited) return 0;
   return tc::init();
@@ -1042,7 +1040,7 @@ extern "C" size_t fear_corr_concat_workspace_bytes(int B, int Bz) {
   return ((size_t)B * kScorePix * kCatC + (size_t)Bz * kCorrC * kFeatC) * sizeof(float);
 }
 
-// NCHW in / NCHW out through the hot path's channels-last tcgen05 kernel; the two layout changes use the
+// NCHW in / NCHW out through the hot path's channels-last wgmma kernel; the two layout changes use the
 // caller's workspace (nothing is allocated, the stream is never synchronised).
 extern "C" int fear_corr_concat_ws_f32(const float* d_z, int Bz, const float* d_x, int B, float* d_out, void* d_workspace,
                                        size_t workspace_bytes, void* stream) {
@@ -1067,7 +1065,7 @@ extern "C" int fear_corr_concat_ws_f32(const float* d_z, int Bz, const float* d_
 }
 
 // Workspace-free form with the signature SURVEY.md 8(b) lists: a direct CUDA-core kernel on the reference's own
-// layouts (compatibility entry point -- the hot path and the _ws form above use the tcgen05 kernel).
+// layouts (compatibility entry point -- the hot path and the _ws form above use the wgmma kernel).
 extern "C" int fear_corr_concat_f32(const float* d_z, int Bz, const float* d_x, int B, float* d_out, void* stream) {
   if (!d_z || !d_x || !d_out || B < 1) return set_err(FEAR_EINVAL, "bad argument");
   if (Bz != 1 && Bz != B) return set_err(FEAR_EINVAL, "template batch must be 1 or B (got %d vs %d)", Bz, B);
@@ -1123,16 +1121,12 @@ extern "C" int fear_set_option(FearContext* c, const char* key, const char* valu
   if (!key || !value) return set_err(FEAR_EINVAL, "null option");
   Options& o = c ? c->opt : g_default_options;
   if (c) c->generation++;
-  if (!strcmp(key, "pdl")) {  // process-wide: programmatic dependent launch for the TMA / tcgen05 kernels
+  if (!strcmp(key, "pdl")) {  // process-wide: programmatic dependent launch for the TMA / wgmma kernels
     tc::pdl_enabled() = atoi(value) != 0;
     return 0;
   }
   if (!strcmp(key, "fuse_dwpw")) {
     o.fuse_dwpw = atoi(value) & 15;  // bit 0: 16x16-stage backbone blocks, bit 1: the head's SepConvs, bit 2: also the 32x32-stage blocks, bit 3: expand-1 blocks
-    return 0;
-  }
-  if (!strcmp(key, "pw_ts")) {
-    o.pw_ts = atoi(value) != 0;
     return 0;
   }
   if (!strcmp(key, "fuse_stem")) {
@@ -1154,64 +1148,15 @@ extern "C" int fear_set_option(FearContext* c, const char* key, const char* valu
   }
   int impl;
   if (!strcmp(value, "ffma")) impl = IMPL_FFMA;
-  else if (!strcmp(value, "tcgen05")) impl = IMPL_TC;
+  else if (!strcmp(value, "wgmma")) impl = IMPL_TC;
   else if (!strcmp(value, "auto")) impl = -1;
-  else return set_err(FEAR_EINVAL, "unknown implementation '%s' (auto | ffma | tcgen05)", value);
-  if (impl > IMPL_FFMA && !tc::available()) return set_err(FEAR_EINVAL, "tcgen05 kernels not available in this build");
+  else return set_err(FEAR_EINVAL, "unknown implementation '%s' (auto | ffma | wgmma)", value);
+  if (impl > IMPL_FFMA && !tc::available()) return set_err(FEAR_EINVAL, "wgmma kernels not available on this device");
   if (!strcmp(key, "corr")) o.corr = impl;
   else if (!strcmp(key, "pw")) o.pw = impl;
   else return set_err(FEAR_EINVAL, "unknown option '%s' (corr | pw)", key);
   return 0;
 }
-
-#ifdef FEAR_IRF_TIMING
-// Profiling build only (python -m feartracker_b200.build with FEAR_NVCC_FLAGS=-DFEAR_IRF_TIMING; not declared in the
-// public header): per-warp cycle counters of the last irf_s2_fused_kernel launch, [148][8 warps][8] uint64.
-extern "C" int fear_debug_irf_timing(FearContext* c, unsigned long long* host_out, int n) {
-  if (!c || !host_out) return FEAR_EINVAL;
-  DeviceGuard guard(c->device);
-  if (!c->d_irf_dbg) {
-    CUDA_TRY(cudaMalloc(&c->d_irf_dbg, 148 * 128 * sizeof(unsigned long long)));
-    CUDA_TRY(cudaMemset(c->d_irf_dbg, 0, 148 * 128 * sizeof(unsigned long long)));
-    return 1;  // armed: run a step, then call again
-  }
-  CUDA_TRY(cudaDeviceSynchronize());
-  CUDA_TRY(cudaMemcpy(host_out, c->d_irf_dbg, sizeof(unsigned long long) * (n < 148 * 128 ? n : 148 * 128), cudaMemcpyDeviceToHost));
-  return 0;
-}
-#endif
-
-#ifdef FEAR_CORR_ABLATE
-// Profiling build only (FEAR_NVCC_FLAGS=-DFEAR_CORR_ABLATE; not in the public header): roles of corr_ts_kernel that skip
-// their work.  1 = MMAs, 2 = convert, 4 = epilogue, 8 = x tiles re-read from L2 (no HBM stream).  Results are garbage.
-extern "C" int fear_debug_corr_ablate(int mask) {
-  CUDA_TRY(cudaMemcpyToSymbol(tc::g_corr_ablate, &mask, sizeof(int)));
-  return 0;
-}
-#endif
-
-#ifdef FEAR_PW_ABLATE
-// Profiling build only (FEAR_NVCC_FLAGS=-DFEAR_PW_ABLATE): see kernels_tc.cuh / tools/pw_ablate.py.
-extern "C" int fear_debug_pw_ablate(int mask) {
-  CUDA_TRY(cudaMemcpyToSymbol(tc::g_pw_ablate, &mask, sizeof(int)));
-  return 0;
-}
-#endif
-
-#ifdef FEAR_PW_TIMING
-// Profiling build only (FEAR_NVCC_FLAGS=-DFEAR_PW_TIMING): per-launch role cycle counters of pw_tc_kernel since the last
-// call (launch ordinal modulo 64); counters [64][32] u64, info [64][8] int.  Resets both.  tools/pw_timing.py
-extern "C" int fear_debug_pw_timing(unsigned long long* counters, int* info) {
-  CUDA_TRY(cudaDeviceSynchronize());
-  if (counters) CUDA_TRY(cudaMemcpyFromSymbol(counters, tc::g_pw_timing, sizeof(unsigned long long) * 64 * 32));
-  if (info) memcpy(info, tc::pw_timing_info(), sizeof(tc::PwTimingInfo) * 64);
-  static unsigned long long zeros[64 * 32];
-  CUDA_TRY(cudaMemcpyToSymbol(tc::g_pw_timing, zeros, sizeof(zeros)));
-  int n = tc::pw_timing_next();
-  tc::pw_timing_next() = 0;
-  return n;
-}
-#endif
 
 extern "C" int64_t fear_launch_count(const FearContext* c) { return c ? c->launches : 0; }
 extern "C" int64_t fear_generation(const FearContext* c) { return c ? c->generation : -1; }

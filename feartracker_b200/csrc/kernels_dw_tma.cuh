@@ -1,4 +1,4 @@
-// TMA-fed depthwise convolution (channels-last fp32), sm_100a.
+// TMA-fed depthwise convolution (channels-last fp32), sm_90a.
 //
 // The register-strip kernels in kernels_ffma.cuh fetch every input pixel straight from global memory; ncu shows
 // them latency-bound on the 5x5 layers (2 TB/s of DRAM traffic, ~50 % L1 hit rate, 4x the algorithmic bytes
@@ -49,9 +49,8 @@ constexpr int dw_tma_smem_bytes() {
   return STAGES * DwTile<K, S, TH, TW>::kStageBytes + 2 * STAGES * 8 + 128;
 }
 
-// GW = consumer warps working on one tile (per group).  Measured on B200 (round 2): 8 warps x (2 x 4)-pixel blocks
-// are 3 % SLOWER than 4 warps x (2 x 8)-pixel blocks -- the extra shared-memory loads per output cost more than the
-// extra resident warps hide, i.e. this kernel is bound by LDS / FFMA2 issue, not by latency.
+// GW = consumer warps working on one tile (per group); the default of 4 warps x (2 x 8)-pixel blocks has not been compared
+// against other splits on the H100.
 template <int K, int S, int TH, int TW, int TX, int TY, int STAGES, int GROUPS, bool RELU, bool BIAS, int GW = 4>
 __global__ void __launch_bounds__(GROUPS * GW * 32, 1)
 dw_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant__ CUtensorMap tmW,

@@ -1,6 +1,6 @@
 // CUDA-core (FFMA) kernels of the FEAR-XS hot path, channels-last (NHWC) fp32.
 //
-// These are the always-correct implementations every stage can run on; the tcgen05 kernels in
+// These are the always-correct implementations every stage can run on; the wgmma kernels in
 // kernels_tc.cuh replace the dense contractions (1x1 convs, correlation) where they apply.
 // Layout: activations [B][H][W][C] fp32, C a multiple of 4 (float4 over channels); 1x1 weights
 // torch-native [Cout][Cin] ("K-major"); depthwise weights [k*k][C]; stem weights [27][16].

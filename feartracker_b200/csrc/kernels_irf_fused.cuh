@@ -1,42 +1,30 @@
-// irf_s2_fused_kernel -- the inverted-residual block xif2_0 of fbnet_c as ONE kernel (sm_100a):
+// irf_s2_fused_kernel -- the inverted-residual block xif2_0 of fbnet_c as ONE kernel (sm_90a):
 //
 //     Y = W2 * relu(dw3x3_s2(relu(W1 * X + b1)) + bd) + b2          16 -> 96 -> 96 -> 24 channels, 2x down
 //
 // (mobile_cv IRF block pw -> dw -> pwl as restated in oracle/fbnet_c.py:95-110; call site reference
 // model_training/model/blocks.py:27-35).  Unfused this block is three kernels that write and re-read the 6x
-// expanded tensor E = relu(W1 X + b1) and the depthwise map: 4.3 GB of HBM traffic per 256-frame step for 0.37 GB
-// of block input + output.  Here E and the depthwise output never leave the SM.
+// expanded tensor E = relu(W1 X + b1) and the depthwise map; here E and the depthwise output never leave the SM.
 //
-// One persistent CTA per SM walks 8 x 16 output-pixel tiles (= one M = 128 tile of the project GEMM).  Per tile:
+// One CTA (two warpgroups) per 8 x 16 output-pixel tile (= one M = 128 tile of the project GEMM):
 //
-//   loader warps (4)   read the 17 x 33 input pixels the tile needs (halo of the stride-2 3x3 window; 561 pixels,
-//                      64 B each) straight from global memory one tile AHEAD, split them into tf32 (hi, lo) and park
-//                      them in TENSOR MEMORY as the A operand of the expand GEMM (5 M-tiles x (16 + 16) columns):
-//                      X never touches shared memory.  They also run the project epilogue (+b2, store Y).
-//   MMA threads (4)    warps 0-2 -- expand, one issuer per 32-channel slab c: per M-tile i, D[128 x 32] = A_i * W1[c]^T
-//                      as 3xTF32 with the A operand in TMEM ("TS" form) into a ring of eight 32-column TMEM
-//                      accumulators;  warp 3 -- project: acc2[128 x 24] += dw_c * W2[:, c]^T (A = depthwise output
-//                      tile in smem, hi/lo).  Several issuers because ONE thread's instruction latency (waits +
-//                      descriptors + 6 MMAs per unit), not the tensor pipe, bounded the first version.
-//   worker groups (2x4 warps)  take alternate slabs: (1) expand epilogue TMEM -> +b1, ReLU, zero outside the image
-//                      (the depthwise conv zero-pads E, and E(0) = relu(b1) != 0) -> 561 x 32-channel fp32 slab in
-//                      shared memory; (2) depthwise 3x3 stride 2 out of that slab (packed FFMA2, same FMA order
-//                      as the stand-alone depthwise kernels) -> +bd, ReLU -> (hi, lo) A tile of the project GEMM in
-//                      the SWIZZLE_128B K-major layout.  Group A's TMEM reads overlap group B's FMAs.
+//   load      the 17 x 33 input pixels the tile needs (halo of the stride-2 3x3 window; 561 pixels, 64 B each) go to
+//             shared memory with coalesced 16-byte loads (zero outside the image), the packed weights image likewise.
+//   per 32-channel slab c of the expanded tensor:
+//     expand     nine 64-row blocks of the box, alternating between the warpgroups: D[64 x 32] = A * W1[c]^T as 3xTF32
+//                wgmma with the A fragments split in registers; + b1, ReLU, zero outside the image (the depthwise conv
+//                zero-pads E, and E(0) = relu(b1) != 0) -> 561 x 32-channel fp32 slab in shared memory.
+//     depthwise  3x3 stride 2 out of that slab (same FMA order as the stand-alone depthwise kernels) -> + bd, ReLU ->
+//                A tile of the project GEMM in the SWIZZLE_128B layout.
+//     project    acc2[128 x 32] += dw_c * W2[:, c]^T, accumulators kept in registers across the slabs.
+//   store     Y = acc2 + b2.
 //
-// All MMA orders / operand splits / epilogue additions replicate pw_tc_kernel, so the block is bit-identical to the
-// three-kernel path (tests/test_gpu_parity.py::test_fused_irf_block_is_bit_identical).
+// All MMA orders / operand splits / epilogue additions replicate pw_tc_kernel (both go through tc::mma3), so the block
+// is bit-identical to the three-kernel path (tests/test_gpu_tcgen05.py::test_fused_irf_block).
 //
-// TMEM (512 columns): [0,160) A operand (5 x (16 hi + 16 lo)); [160,448) 3 slabs x 3-deep ring of 32-column expand
-// accumulators (a ring per issuer: mbarrier parity waits are only safe when producer and consumer of a slot can be
-// at most one phase apart, which in-order use by ONE issuer guarantees); [448,480) project main, [480,512) project
-// correction accumulator.
-// (tile order and barrier protocol: DESIGN.md section 4.4)
-// smem: A2 (hi, lo) 32 KB | weights image 40.25 KB (W1 [hi|lo] rows, W2 [hi;lo] x 3 chunks, dw, biases) | barriers |
-// 2 x 70.1 KB slabs = 214 KB.
+// smem: A2 16 KB | weights image 40.25 KB (W1 [hi|lo] rows, W2 [hi;lo] x 3 chunks, dw, biases) | input box 45 KB |
+// slab 70.1 KB.
 #pragma once
-#include <type_traits>
-
 #include "tc_common.cuh"
 
 namespace fear {
@@ -46,11 +34,10 @@ constexpr int kIrfCin = 16, kIrfMid = 96, kIrfCout = 24, kIrfCoutPad = 32;
 constexpr int kIrfTH = 8, kIrfTW = 16;                          // output tile
 constexpr int kIrfIH = 2 * kIrfTH + 1, kIrfIW = 2 * kIrfTW + 1;  // 17 x 33 input pixels
 constexpr int kIrfPix = kIrfIH * kIrfIW;                        // 561
-constexpr int kIrfMT = (kIrfPix + 127) / 128;                   // 5 M-tiles of the expand GEMM
+constexpr int kIrfMB = (kIrfPix + 63) / 64;                     // 9 64-row blocks of the expand GEMM
 constexpr int kIrfSlabs = kIrfMid / 32;                         // 3
-constexpr int kIrfUnitsPerTile = kIrfSlabs * kIrfMT;            // 15
-constexpr int kIrfRing = 3;                                     // expand accumulator ring PER SLAB ISSUER (TMEM): 9 slots
-constexpr int kIrfThreads = 512;                                // 16 warps: 4 MMA issuers, 4 loader, 2 x 4 workers
+constexpr int kIrfThreads = 256;                                // two warpgroups
+constexpr int kIrfXPitch = 20;                                  // floats per input-box row (16 + 4: conflict-free fragment loads)
 
 // weights image (floats), copied verbatim into shared memory
 constexpr int kIrfW1Floats = kIrfMid * 32;                        // [96 rows][hi 16 | lo 16], SWIZZLE_128B
@@ -58,23 +45,20 @@ constexpr int kIrfW2Floats = kIrfSlabs * 2 * kIrfCoutPad * 32;    // per chunk: 
 constexpr int kIrfDwFloats = 9 * kIrfMid;
 constexpr int kIrfImageFloats = kIrfW1Floats + kIrfW2Floats + kIrfDwFloats + kIrfMid + kIrfMid + kIrfCoutPad;
 
-constexpr int kIrfOffA2 = 0;                                       // hi 16 KB, lo 16 KB
-constexpr int kIrfOffImg = 32768;
+constexpr int kIrfOffA2 = 0;                                       // raw fp32 A tile of the project GEMM
+constexpr int kIrfOffImg = 16384;
 constexpr int kIrfOffW1 = kIrfOffImg;
 constexpr int kIrfOffW2 = kIrfOffW1 + kIrfW1Floats * 4;
 constexpr int kIrfOffDw = kIrfOffW2 + kIrfW2Floats * 4;
 constexpr int kIrfOffB1 = kIrfOffDw + kIrfDwFloats * 4;
 constexpr int kIrfOffBd = kIrfOffB1 + kIrfMid * 4;
 constexpr int kIrfOffB2 = kIrfOffBd + kIrfMid * 4;
-constexpr int kIrfOffBars = ((kIrfOffB2 + kIrfCoutPad * 4 + 255) / 256) * 256;
-constexpr int kIrfOffSlab = kIrfOffBars + 512;  // 33 mbarriers + the TMEM base slot
+constexpr int kIrfOffX = ((kIrfOffB2 + kIrfCoutPad * 4 + 255) / 256) * 256;
+constexpr int kIrfOffSlab = kIrfOffX + kIrfMB * 64 * kIrfXPitch * 4;
 constexpr int kIrfSlabBytes = kIrfPix * 128;
-constexpr int kIrfSmemBytes = kIrfOffSlab + 2 * kIrfSlabBytes + 1024 /*alignment slack*/;
+constexpr int kIrfSmemBytes = kIrfOffSlab + kIrfSlabBytes + 1024 /*alignment slack*/;
 static_assert(kIrfSmemBytes <= 232448, "fused IRF kernel exceeds the 227 KB shared-memory limit");
-static_assert(kIrfOffW1 % 1024 == 0 && kIrfOffW2 % 1024 == 0, "UMMA tiles must be 1024-byte aligned");
-
-constexpr int kIrfColA = 0, kIrfColAcc = 160, kIrfColP = 448;  // TMEM column map
-constexpr int kIrfTmemCols = 512;
+static_assert(kIrfOffW1 % 1024 == 0 && kIrfOffW2 % 1024 == 0, "swizzled weight tiles must be 1024-byte aligned");
 
 struct IrfParams {
   const float* X;      // [B][H][W][16]
@@ -82,16 +66,7 @@ struct IrfParams {
   const float* image;  // kIrfImageFloats packed weights (device)
   int B, H, W;         // input map
   int tiles_x, tiles_y, num_tiles;
-  unsigned long long* dbg;  // FEAR_IRF_TIMING builds only: [grid][8 worker warps][8] cycle counters, else null
 };
-
-#ifdef FEAR_IRF_TIMING
-#define IRF_T(var) const long long var = clock64()
-#define IRF_ACC(slot, a, b) tacc[slot] += (b) - (a)
-#else
-#define IRF_T(var)
-#define IRF_ACC(slot, a, b)
-#endif
 
 // Host: build the shared-memory weights image.  w1_hi/w1_lo [96][16], w2_hi/w2_lo [24][96] (tf32-split copies the
 // tensor-core path already keeps), dw [9][96] (tap-major), biases.
@@ -124,422 +99,175 @@ inline void irf_build_image(float* img, const float* w1_hi, const float* w1_lo, 
   for (int i = 0; i < kIrfCout; ++i) p[i] = b2[i];
 }
 
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-
 __global__ void __launch_bounds__(kIrfThreads, 1) irf_s2_fused_kernel(const IrfParams p) {
   extern __shared__ uint8_t irf_smem_raw[];
   uint8_t* smem = irf_smem_raw + ((1024u - (smem_u32(irf_smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kIrfOffBars);
-  uint64_t* a_full = bars;                 // [5] M-tile i of the tile's A operand is in TMEM   (4 loader warps)
-  uint64_t* a_empty = bars + 5;            // [5] the expand MMAs of the tile have read it      (commit)
-  uint64_t* acc_full = bars + 10;          // [9] expand accumulator complete           (commit)
-  uint64_t* acc_empty = bars + 19;         // [9] drained by the worker group           (4 warps)
-  uint64_t* a2_full = bars + 28;           // depthwise (hi, lo) tile written           (4 warps)
-  uint64_t* a2_empty = bars + 29;          // project MMAs have read it                 (commit)
-  uint64_t* acc2_full = bars + 30;         // project accumulator complete              (commit)
-  uint64_t* acc2_empty = bars + 31;        // drained by the loader warps               (4 warps)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 32);
-
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 4) {
-    tmem_alloc(tmem_slot, kIrfTmemCols);
-    tmem_relinquish();
-  }
-  if (threadIdx.x == 160) {
-    for (int i = 0; i < kIrfMT; ++i) {
-      mbar_init(&a_full[i], 4);
-      mbar_init(&a_empty[i], kIrfSlabs);
-    }
-    for (int s = 0; s < kIrfSlabs * kIrfRing; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], 4);
-    }
-    mbar_init(a2_full, 4);
-    mbar_init(a2_empty, 1);
-    mbar_init(acc2_full, 1);
-    mbar_init(acc2_empty, 4);
-    fence_mbar_init();
-  }
   {  // weights image -> shared memory (constant data: may be read before the previous kernel has finished)
     const float4* src = reinterpret_cast<const float4*>(p.image);
     float4* dst = reinterpret_cast<float4*>(smem + kIrfOffImg);
     for (int i = threadIdx.x; i < kIrfImageFloats / 4; i += kIrfThreads) dst[i] = __ldg(src + i);
-    fence_proxy_async_smem();  // the tensor core reads W1 / W2 through the async proxy
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_trigger();
   pdl_wait();  // X is written by the previous kernel in the stream
 
   const int Ho = p.H >> 1, Wo = p.W >> 1;
-  const int my_tiles = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles of this CTA
-  auto tile_coords = [&](int tl, int& b, int& oy0, int& ox0) {
-    const int tile = blockIdx.x + tl * gridDim.x;
-    const int tx = tile % p.tiles_x;
-    const int rest = tile / p.tiles_x;
-    const int ty = rest % p.tiles_y;
-    b = rest / p.tiles_y;
-    oy0 = ty * kIrfTH;
-    ox0 = tx * kIrfTW;
-  };
+  const int tx = blockIdx.x % p.tiles_x, rest = blockIdx.x / p.tiles_x;
+  const int b = rest / p.tiles_y, oy0 = (rest % p.tiles_y) * kIrfTH, ox0 = tx * kIrfTW;
+  float* xs = reinterpret_cast<float*>(smem + kIrfOffX);
+  for (int i = threadIdx.x; i < kIrfMB * 64 * 4; i += kIrfThreads) {  // (box pixel, 16-byte quarter)
+    const int pb = i >> 2, j = i & 3;
+    const int by = pb / kIrfIW, bx = pb - by * kIrfIW;
+    const int iy = 2 * oy0 - 1 + by, ix = 2 * ox0 - 1 + bx;
+    const bool ok = pb < kIrfPix && iy >= 0 && ix >= 0;
+    const float4 v = ok ? __ldg(reinterpret_cast<const float4*>(p.X + (((long long)b * p.H + iy) * p.W + ix) * kIrfCin) + j)
+                        : make_float4(0.f, 0.f, 0.f, 0.f);
+    *reinterpret_cast<float4*>(xs + pb * kIrfXPitch + 4 * j) = v;
+  }
+  fence_proxy_async_smem();  // the tensor core reads W1 / W2 through the async proxy
+  __syncthreads();
 
-  if (warp < kIrfSlabs) {
-    // ===================================== expand MMA issuers =====================================
-    // One issuing thread per 32-channel slab c = warp (a single thread's instruction latency, not the tensor pipe,
-    // bounded a one-issuer version): its W1 descriptors are loop invariants, it walks the tile's five M-tiles.
-    if (lane == 0 && my_tiles > 0) {
-      constexpr uint32_t idesc_e = umma_idesc_tf32(128, 32);  // N = 32-channel slab
-      const int c = warp;
-      const uint32_t brow = smem_u32(smem + kIrfOffW1) + c * 4096;  // rows [32c, 32c + 32) of W1: [hi 64 B | lo 64 B]
-      const uint64_t dbh0 = umma_desc_k_sw128(brow), dbh1 = umma_desc_k_sw128(brow + 32);
-      const uint64_t dbl0 = umma_desc_k_sw128(brow + 64), dbl1 = umma_desc_k_sw128(brow + 96);
-      int n = 0;  // this issuer's unit counter: unit n uses slot c * 3 + n % 3 for the (n / 3)-th time
-      for (int tl = 0; tl < my_tiles; ++tl) {
-        for (int i = 0; i < kIrfMT; ++i, ++n) {
-          mbar_wait_backoff(&a_full[i], (uint32_t)(tl & 1));
-          const int slot = c * kIrfRing + n % kIrfRing;
-          mbar_wait_backoff(&acc_empty[slot], (uint32_t)(((n / kIrfRing) & 1) ^ 1));
-          tc_fence_after();
-          const uint32_t d = tmem_base + kIrfColAcc + slot * 32;
-          const uint32_t a_hi = tmem_base + kIrfColA + i * 32, a_lo = a_hi + 16;
-          // K = 16 = 2 K-steps x (hi*hi, lo*hi, hi*lo): same product order as pw_tc_kernel's single-accumulator path
-          asm volatile(
-              "{\n\t"
-              ".reg .pred p0, p1;\n\t"
-              "setp.ne.b32 p0, 0, 0;\n\t"
-              "setp.eq.b32 p1, 0, 0;\n\t"
-              "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %3, %7, p0;\n\t"
-              "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%2], %3, %7, p1;\n\t"
-              "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %5, %7, p1;\n\t"
-              "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%8], %4, %7, p1;\n\t"
-              "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%9], %4, %7, p1;\n\t"
-              "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%8], %6, %7, p1;\n\t"
-              "}\n" ::"r"(d),
-              "r"(a_hi), "r"(a_lo), "l"(dbh0), "l"(dbh1), "l"(dbl0), "l"(dbl1), "r"(idesc_e), "r"(a_hi + 8), "r"(a_lo + 8)
-              : "memory");
-          tc_commit(&acc_full[slot]);
-          tc_commit(&a_empty[i]);  // (count 3: one commit per slab issuer) this M-tile's A columns may be refilled
-        }
-      }
-    }
-  } else if (warp == 3) {
-    // ===================================== project MMA issuer =====================================
-    if (lane == 0 && my_tiles > 0) {
-      constexpr uint32_t idesc_p = umma_idesc_tf32(128, 32);   // a_lo x w_hi
-      constexpr uint32_t idesc_p2 = umma_idesc_tf32(128, 64);  // a_hi x [w_hi ; w_lo] -> main | corr
-      const uint32_t w2 = smem_u32(smem + kIrfOffW2);
-      const uint32_t a2h = smem_u32(smem + kIrfOffA2), a2l = a2h + 16384;
-      const int projects = my_tiles * kIrfSlabs;
-      int tl = 0, c = 0;
-      for (int pj = 0; pj < projects; ++pj) {
-        if (c == 0) {
-          mbar_wait_backoff(acc2_empty, (uint32_t)((tl & 1) ^ 1));
-          tc_fence_after();
-        }
-        mbar_wait_backoff(a2_full, (uint32_t)(pj & 1));
-        tc_fence_after();
-        const uint32_t d = tmem_base + kIrfColP;
-        const uint32_t bh = w2 + c * 8192;  // [hi 32 rows ; lo 32 rows] x 128 B
+  const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
+  const int rw = (warp & 3) * 16 + g;  // this thread's first row inside a 64-row block (second: + 8)
+  const bool border = (oy0 == 0) || (ox0 == 0);  // only these tiles have box pixels outside the image
+  float acc2m[16], acc2c[16];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint64_t dah = umma_desc_k_sw128(a2h + j * 32), dal = umma_desc_k_sw128(a2l + j * 32);
-          const uint64_t dbh = umma_desc_k_sw128(bh + j * 32);
-          mma_tf32_ss(d, dah, dbh, idesc_p2, (c | j) != 0);  // main += a_hi w_hi ; corr (+)= a_hi w_lo
-          mma_tf32_ss(d + 32, dal, dbh, idesc_p, 1);         // corr += a_lo w_hi
-        }
-        tc_commit(a2_empty);
-        if (c == kIrfSlabs - 1) tc_commit(acc2_full);
-        if (++c == kIrfSlabs) {
-          c = 0;
-          ++tl;
-        }
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================================== loader + project epilogue =====================================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;  // TMEM lane = row inside every M-tile
-    float4 xr[kIrfMT][4];
-    auto prefetch = [&](int tl) {
-      int b, oy0, ox0;
-      tile_coords(tl, b, oy0, ox0);
-#pragma unroll
-      for (int i = 0; i < kIrfMT; ++i) {
-        const int pb = i * 128 + row;
-        const int by = pb / kIrfIW, bx = pb - by * kIrfIW;
-        const int iy = 2 * oy0 - 1 + by, ix = 2 * ox0 - 1 + bx;
-        const bool ok = pb < kIrfPix && iy >= 0 && ix >= 0;
-        const float4* src = reinterpret_cast<const float4*>(p.X + (((long long)b * p.H + iy) * p.W + ix) * kIrfCin);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) xr[i][j] = ok ? __ldg(src + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    };
-    auto project_epilogue = [&](int tl) {
-      int b, oy0, ox0;
-      tile_coords(tl, b, oy0, ox0);
-      mbar_wait_backoff(acc2_full, (uint32_t)(tl & 1));
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + kIrfColP + ((uint32_t)(q * 32) << 16);
-      const int oy = oy0 + (row >> 4), ox = ox0 + (row & 15);
-      float4* dst = reinterpret_cast<float4*>(p.Y + (((long long)b * Ho + oy) * Wo + ox) * kIrfCout);
-      const float4* b2 = reinterpret_cast<const float4*>(smem + kIrfOffB2);
-#pragma unroll
-      for (int g = 0; g < kIrfCout; g += 8) {
-        uint32_t m[8], s[8];
-        tmem_ld_32x8(taddr + g, m);
-        tmem_ld_32x8(taddr + 32 + g, s);
-        tmem_ld_wait();
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const float4 bb = b2[g / 4 + h];
-          float4 o;
-          o.x = __uint_as_float(m[4 * h]) + __uint_as_float(s[4 * h]) + bb.x;
-          o.y = __uint_as_float(m[4 * h + 1]) + __uint_as_float(s[4 * h + 1]) + bb.y;
-          o.z = __uint_as_float(m[4 * h + 2]) + __uint_as_float(s[4 * h + 2]) + bb.z;
-          o.w = __uint_as_float(m[4 * h + 3]) + __uint_as_float(s[4 * h + 3]) + bb.w;
-          dst[g / 4 + h] = o;
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc2_empty);
-    };
-    if (my_tiles > 0) prefetch(0);
-    for (int tl = 0; tl < my_tiles; ++tl) {
-#pragma unroll
-      for (int i = 0; i < kIrfMT; ++i) {
-        mbar_wait_backoff(&a_empty[i], (uint32_t)((tl & 1) ^ 1));  // the previous tile's MMAs no longer read these columns
-        tc_fence_after();
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float v[4] = {xr[i][j].x, xr[i][j].y, xr[i][j].z, xr[i][j].w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const uint32_t h = __float_as_uint(v[e]) & 0xFFFFE000u;  // = what kind::tf32 reads from the raw word
-            hi[4 * j + e] = h;
-            lo[4 * j + e] = __float_as_uint(v[e] - __uint_as_float(h));
-          }
-        }
-        const uint32_t tdst = tmem_base + kIrfColA + i * 32 + ((uint32_t)(q * 32) << 16);
-        tmem_st_32x16(tdst, hi);
-        tmem_st_32x16(tdst + 16, lo);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_full[i]);
-      }
-      if (tl + 1 < my_tiles) prefetch(tl + 1);
-      if (tl > 0) project_epilogue(tl - 1);
-    }
-    if (my_tiles > 0) project_epilogue(my_tiles - 1);
-  } else if (warp >= 8) {
-    // ===================================== worker groups =====================================
-    const int group = (warp - 8) >> 2, gw = warp & 3;  // gw = TMEM lane quadrant of this warp
-    uint8_t* slab = smem + kIrfOffSlab + group * kIrfSlabBytes;
-    const int bar_id = 1 + group;
-    const int total_slabs = my_tiles * kIrfSlabs;
-    const int cg = lane & 7;
-    const uint32_t lane_base = tmem_base + kIrfColAcc + ((uint32_t)(gw * 32) << 16);
+  for (int i = 0; i < 16; ++i) acc2m[i] = acc2c[i] = 0.f;
+  uint8_t* slab = smem + kIrfOffSlab;
+  uint8_t* a2 = smem + kIrfOffA2;
+
+  for (int c = 0; c < kIrfSlabs; ++c) {
+    // ---- (1) expand: relu(X W1[c]^T + b1), zero outside the image -> slab ----
     // Slab layout: pixel pb = by * 33 + bx of the 17 x 33 box at byte pb * 128; the 16-byte chunk of channel group j
-    // sits at position j ^ (bx & 7): consecutive pixels of a row (= consecutive lanes of the writer) hit different
-    // banks, and a reader's chunk offset depends only on the box column -> five per-thread constants.
-    // Per-thread geometry of the two 2 x 2 output blocks this thread computes (it = 0 / 1):
-    //   block id = it * 16 + gw * 4 + (lane >> 3):  oy_l = (blk >> 3) * 2 (it adds 4), ox_l = (blk & 7) * 2
-    const int blk0 = gw * 4 + (lane >> 3);
-    const int oy_l0 = (blk0 >> 3) * 2, ox_l = (blk0 & 7) * 2;
-    uint32_t col_off[5];  // byte offset of input column 2 * ox_l + i inside a slab row (incl. the channel-group swizzle)
+    // sits at position j ^ (bx & 7): a reader's chunk offset depends only on the box column.
+    const uint32_t brow = smem_u32(smem + kIrfOffW1) + c * 4096;  // rows [32c, 32c + 32) of W1: [hi 64 B | lo 64 B]
+    const float* b1 = reinterpret_cast<const float*>(smem + kIrfOffB1) + c * 32;
+    for (int mb = wg; mb < kIrfMB; mb += 2) {
+      uint32_t hi[2][4], lo[2][4];
 #pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const int bx = 2 * ox_l + i;
-      col_off[i] = (uint32_t)(bx * 128 + ((cg ^ (bx & 7)) << 4));
-    }
-    // expand-epilogue geometry per M-tile: box coordinates of this thread's row
-#ifdef FEAR_IRF_TIMING
-    long long tacc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};  // 8 arrive part, 9 prefetch issue, 10 processing, 11 bias loads
-    long long tacc_unused[1] = {0};  // 0 wait acc_full, 1 epilogue, 2 bar (slab done), 3 wait a2_empty,
-                                                   // 4 depthwise, 5 bar (slab free), 6 total
-    const long long t_begin = clock64();
-#endif
-    for (int sc = group; sc < total_slabs; sc += 2) {
-      const int tl = sc / kIrfSlabs, c = sc - tl * kIrfSlabs;
-      int b, oy0, ox0;
-      tile_coords(tl, b, oy0, ox0);
-      const bool border = (oy0 == 0) || (ox0 == 0);  // only these tiles have box pixels outside the image
-      // ---- (1) expand epilogue: TMEM -> +b1, ReLU, zero outside the image -> slab ----
-      // Software pipeline over 10 half-M-tiles (16 accumulator columns each): the TMEM load of half k + 1 is in
-      // flight while half k is biased / clamped / stored; the slab's 32 biases live in registers.
-      float4 bb[8];
+      for (int j = 0; j < 2; ++j)
 #pragma unroll
-      for (int j = 0; j < 8; ++j) bb[j] = reinterpret_cast<const float4*>(smem + kIrfOffB1 + c * 128)[j];
-      const int n0 = tl * kIrfMT;  // slab issuer c's unit counter at M-tile 0 of this tile (slot c * 3 + n % 3)
-      uint32_t r[2][16];
-      IRF_T(t0);
-      mbar_wait(&acc_full[c * kIrfRing + n0 % kIrfRing], (uint32_t)((n0 / kIrfRing) & 1));
-      IRF_T(t0b);
-      IRF_ACC(0, t0, t0b);
-      tc_fence_after();
-      tmem_ld_32x16(lane_base + (c * kIrfRing + n0 % kIrfRing) * 32, r[0]);
-#pragma unroll 1
-      for (int i = 0; i < kIrfMT; ++i) {  // (runtime loop: the fully unrolled version thrashed the instruction cache)
-        const int n = n0 + i;
-        const int pb = i * 128 + gw * 32 + lane;
+        for (int e = 0; e < 4; ++e) {
+          const float v = xs[(mb * 64 + rw + (e & 1) * 8) * kIrfXPitch + 8 * j + 4 * (e >> 1) + t];
+          const uint32_t h = __float_as_uint(v) & 0xFFFFE000u;
+          hi[j][e] = h;
+          lo[j][e] = __float_as_uint(v - __uint_as_float(h));
+        }
+      float em[16], ec[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) em[i] = ec[i] = 0.f;
+      wg_fence();
+#pragma unroll
+      for (int j = 0; j < 2; ++j) mma3<32>(em, ec, hi[j], lo[j], brow + j * 32, brow + 64 + j * 32);
+      wg_commit();
+      wg_wait();
+#pragma unroll
+      for (int hrow = 0; hrow < 2; ++hrow) {
+        const int pb = mb * 64 + rw + hrow * 8;
+        if (pb >= kIrfPix) continue;
         const int by = pb / kIrfIW, bx = pb - by * kIrfIW;
-        const int sw = bx & 7;
         const bool outside = border && ((2 * oy0 - 1 + by) < 0 || (2 * ox0 - 1 + bx) < 0);
-        const uint32_t dst = smem_u32(slab + pb * 128);
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          tmem_ld_wait();  // half (i, hh) has landed in r[hh]
-          if (hh == 1) {   // both halves of M-tile i are out of TMEM: hand the accumulator slot back at once
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[c * kIrfRing + n % kIrfRing]);
-          }
-          // prefetch the next half (rows >= 561 of the last M-tile are padding: quadrants 2 and 3 skip it)
-          if (hh == 0) {
-            if (i * 128 + gw * 32 < kIrfPix) tmem_ld_32x16(lane_base + (c * kIrfRing + n % kIrfRing) * 32 + 16, r[1]);
-          } else if (i + 1 < kIrfMT) {
-            const int sl = c * kIrfRing + (n + 1) % kIrfRing;
-            IRF_T(tw0);
-            mbar_wait(&acc_full[sl], (uint32_t)(((n + 1) / kIrfRing) & 1));
-            IRF_T(tw1);
-            IRF_ACC(0, tw0, tw1);
-            IRF_ACC(1, tw1, tw0);  // (keeps the wait out of the epilogue time accumulated below)
-            tc_fence_after();
-            if ((i + 1) * 128 + gw * 32 < kIrfPix) tmem_ld_32x16(lane_base + sl * 32, r[0]);
-          }
-          if (pb < kIrfPix) {
-            // (instruction diet: this loop is bound by the FMA / ALU issue rate, so the bias add is packed -- FADD2 --
-            // and the "pixel outside the image" select only runs for the few warps that hold such a pixel)
-            const bool any_outside = border && __any_sync(__activemask(), outside);
-            auto emit = [&](auto with_select) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const F4 bj = reinterpret_cast<const F4*>(bb)[4 * hh + j];
-                const unsigned long long s0 = fadd2(pack2(r[hh][4 * j], r[hh][4 * j + 1]), bj.lo);
-                const unsigned long long s1 = fadd2(pack2(r[hh][4 * j + 2], r[hh][4 * j + 3]), bj.hi);
-                float4 o;
-                o.x = fmaxf(__uint_as_float((uint32_t)s0), 0.f);
-                o.y = fmaxf(__uint_as_float((uint32_t)(s0 >> 32)), 0.f);
-                o.z = fmaxf(__uint_as_float((uint32_t)s1), 0.f);
-                o.w = fmaxf(__uint_as_float((uint32_t)(s1 >> 32)), 0.f);
-                if (decltype(with_select)::value && outside) o = make_float4(0.f, 0.f, 0.f, 0.f);
-                // volatile: keeps this store after the prefetch of the next half in program order
-                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + (((4 * hh + j) ^ sw) << 4)), "f"(o.x),
-                             "f"(o.y), "f"(o.z), "f"(o.w)
-                             : "memory");
-              }
-            };
-            if (any_outside) emit(std::true_type{});
-            else emit(std::false_type{});
-          }
+        for (int i = 0; i < 4; ++i) {
+          const int col = 8 * i + 2 * t;
+          float2 o;
+          o.x = fmaxf((em[4 * i + 2 * hrow] + ec[4 * i + 2 * hrow]) + b1[col], 0.f);
+          o.y = fmaxf((em[4 * i + 2 * hrow + 1] + ec[4 * i + 2 * hrow + 1]) + b1[col + 1], 0.f);
+          if (outside) o = make_float2(0.f, 0.f);
+          *reinterpret_cast<float2*>(slab + pb * 128 + ((((col >> 2) ^ (bx & 7))) << 4) + (col & 3) * 4) = o;
         }
       }
-      IRF_T(t1);
-      IRF_ACC(1, t0b, t1);
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");  // the slab is complete
-      IRF_T(t2);
-      IRF_ACC(2, t1, t2);
-      // ---- (2) depthwise 3x3 stride 2 + bd + ReLU -> (hi, lo) A tile of the project GEMM ----
-      {
-        const F4* w4 = reinterpret_cast<const F4*>(smem + kIrfOffDw) + c * 8 + cg;  // tap t at + t * 24
-        const F4 bias4 = reinterpret_cast<const F4*>(smem + kIrfOffBd)[c * 8 + cg];
-        F4 wk[3][3];
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx) wk[ky][kx] = w4[(ky * 3 + kx) * (kIrfMid / 4)];
-        uint8_t* ah = smem + kIrfOffA2;
-        uint8_t* al = ah + 16384;
-        IRF_T(t3);
-        mbar_wait(a2_empty, (uint32_t)((sc & 1) ^ 1));  // the previous slab's project MMAs have read the A tile
-        IRF_T(t4);
-        IRF_ACC(3, t3, t4);
-#pragma unroll
-        for (int it = 0; it < 2; ++it) {
-          const int oy_l = oy_l0 + 4 * it;
-          const uint8_t* rows = slab + (2 * oy_l) * (kIrfIW * 128);
-          F4 acc[2][2];
-#pragma unroll
-          for (int y = 0; y < 2; ++y)
-#pragma unroll
-            for (int x = 0; x < 2; ++x) acc[y][x] = bias4;
-#pragma unroll
-          for (int rr = 0; rr < 5; ++rr) {
-            F4 v[5];
-#pragma unroll
-            for (int i = 0; i < 5; ++i) v[i] = *reinterpret_cast<const F4*>(rows + rr * (kIrfIW * 128) + col_off[i]);
-#pragma unroll
-            for (int y = 0; y < 2; ++y) {
-              const int ky = rr - 2 * y;
-              if (ky >= 0 && ky < 3) {
-#pragma unroll
-                for (int kx = 0; kx < 3; ++kx) {
-                  const F4 k = wk[(ky >= 0 && ky < 3) ? ky : 0][kx];
-#pragma unroll
-                  for (int x = 0; x < 2; ++x) ffma2(acc[y][x].lo, v[2 * x + kx].lo, k.lo);
-#pragma unroll
-                  for (int x = 0; x < 2; ++x) ffma2(acc[y][x].hi, v[2 * x + kx].hi, k.hi);
-                }
-              }
-            }
-          }
-#pragma unroll
-          for (int y = 0; y < 2; ++y)
-#pragma unroll
-            for (int x = 0; x < 2; ++x) {
-              float4 v = f4_to_float4(acc[y][x]);
-              v.x = fmaxf(v.x, 0.f);
-              v.y = fmaxf(v.y, 0.f);
-              v.z = fmaxf(v.z, 0.f);
-              v.w = fmaxf(v.w, 0.f);
-              float4 h, l;
-              split_tf32_trunc(v.x, h.x, l.x);
-              split_tf32_trunc(v.y, h.y, l.y);
-              split_tf32_trunc(v.z, h.z, l.z);
-              split_tf32_trunc(v.w, h.w, l.w);
-              const int R = (oy_l + y) * kIrfTW + ox_l + x;           // A-tile row = pixel inside the 8 x 16 tile
-              const int off = R * 128 + ((cg ^ (R & 7)) << 4);       // SWIZZLE_128B
-              *reinterpret_cast<float4*>(ah + off) = v;              // raw fp32 = hi operand (hardware truncation)
-              *reinterpret_cast<float4*>(al + off) = l;
-            }
-        }
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a2_full);
-      IRF_T(t5);
-      IRF_ACC(4, t2, t5);
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");  // everyone has left the slab before it is rewritten
-      IRF_T(t6);
-      IRF_ACC(5, t5, t6);
     }
-#ifdef FEAR_IRF_TIMING
-    tacc[6] = clock64() - t_begin;
-    if (p.dbg && lane == 0)
-      for (int k = 0; k < 12; ++k) p.dbg[((long long)blockIdx.x * 8 + (warp - 8)) * 16 + k] = (unsigned long long)tacc[k];
-#endif
+    __syncthreads();  // the slab is complete
+    // ---- (2) depthwise 3x3 stride 2 + bd + ReLU -> A tile of the project GEMM: thread = (4-channel group, 2 x 2 pixels) ----
+    {
+      const int cg = threadIdx.x & 7, blk = threadIdx.x >> 3;
+      const int oy_l = (blk >> 3) * 2, ox_l = (blk & 7) * 2;
+      const float4* w4 = reinterpret_cast<const float4*>(smem + kIrfOffDw) + c * 8 + cg;  // tap t at + t * 24
+      const float4 bias4 = reinterpret_cast<const float4*>(smem + kIrfOffBd)[c * 8 + cg];
+      float4 wk[3][3];
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) wk[ky][kx] = w4[(ky * 3 + kx) * (kIrfMid / 4)];
+      const uint8_t* rows = slab + (2 * oy_l) * (kIrfIW * 128);
+      float4 acc[2][2];
+#pragma unroll
+      for (int y = 0; y < 2; ++y)
+#pragma unroll
+        for (int x = 0; x < 2; ++x) acc[y][x] = bias4;
+#pragma unroll
+      for (int rr = 0; rr < 5; ++rr) {
+        float4 v[5];
+#pragma unroll
+        for (int i = 0; i < 5; ++i) {
+          const int bx = 2 * ox_l + i;
+          v[i] = *reinterpret_cast<const float4*>(rows + rr * (kIrfIW * 128) + bx * 128 + ((cg ^ (bx & 7)) << 4));
+        }
+#pragma unroll
+        for (int y = 0; y < 2; ++y) {
+          const int ky = rr - 2 * y;
+          if (ky >= 0 && ky < 3) {
+#pragma unroll
+            for (int kx = 0; kx < 3; ++kx) {
+              const float4 k = wk[(ky >= 0 && ky < 3) ? ky : 0][kx];
+#pragma unroll
+              for (int x = 0; x < 2; ++x) {
+                const float4 u = v[2 * x + kx];
+                acc[y][x].x = fmaf(u.x, k.x, acc[y][x].x);
+                acc[y][x].y = fmaf(u.y, k.y, acc[y][x].y);
+                acc[y][x].z = fmaf(u.z, k.z, acc[y][x].z);
+                acc[y][x].w = fmaf(u.w, k.w, acc[y][x].w);
+              }
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int y = 0; y < 2; ++y)
+#pragma unroll
+        for (int x = 0; x < 2; ++x) {
+          float4 v = acc[y][x];
+          v.x = fmaxf(v.x, 0.f);
+          v.y = fmaxf(v.y, 0.f);
+          v.z = fmaxf(v.z, 0.f);
+          v.w = fmaxf(v.w, 0.f);
+          const int R = (oy_l + y) * kIrfTW + ox_l + x;  // A-tile row = pixel inside the 8 x 16 tile
+          *reinterpret_cast<float4*>(a2 + R * 128 + ((cg ^ (R & 7)) << 4)) = v;
+        }
+    }
+    __syncthreads();  // the A tile is complete; everyone has left the slab
+    // ---- (3) project: acc2 += dw_c * W2[:, c]^T ----
+    {
+      uint32_t hi[4][4], lo[4][4];
+      load_a_frags(a2, wg * 64 + rw, t, hi, lo);
+      const uint32_t bh = smem_u32(smem + kIrfOffW2) + c * 8192;  // [hi 32 rows ; lo 32 rows] x 128 B
+      wg_fence();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) mma3<32>(acc2m, acc2c, hi[j], lo[j], bh + j * 32, bh + 4096 + j * 32);
+      wg_commit();
+      wg_wait();
+    }
+    __syncthreads();  // the A tile has been read by every warp before the next slab rewrites it
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kIrfTmemCols);
+  const float* b2 = reinterpret_cast<const float*>(smem + kIrfOffB2);
+#pragma unroll
+  for (int hrow = 0; hrow < 2; ++hrow) {
+    const int row = wg * 64 + rw + hrow * 8;
+    const int oy = oy0 + (row >> 4), ox = ox0 + (row & 15);
+    float* dst = p.Y + (((long long)b * Ho + oy) * Wo + ox) * kIrfCout;
+#pragma unroll
+    for (int i = 0; i < kIrfCout / 8; ++i) {
+      const int col = 8 * i + 2 * t;
+      *reinterpret_cast<float2*>(dst + col) = make_float2((acc2m[4 * i + 2 * hrow] + acc2c[4 * i + 2 * hrow]) + b2[col],
+                                                          (acc2m[4 * i + 2 * hrow + 1] + acc2c[4 * i + 2 * hrow + 1]) + b2[col + 1]);
+    }
   }
 }
 
 // X [B][H][W][16] -> Y [B][H/2][W/2][24].  Returns 0 on launch, 1 when the shape is not covered, < 0 on error.
-inline int launch_irf_s2(cudaStream_t s, const float* X, float* Y, const float* image, int B, int H, int W,
-                         unsigned long long* dbg = nullptr) {
+inline int launch_irf_s2(cudaStream_t s, const float* X, float* Y, const float* image, int B, int H, int W) {
   if (!available()) return 1;
   const int Ho = H / 2, Wo = W / 2;
   if (H % 2 || W % 2 || Ho % kIrfTH || Wo % kIrfTW) return 1;
@@ -551,15 +279,13 @@ inline int launch_irf_s2(cudaStream_t s, const float* X, float* Y, const float* 
   p.X = X;
   p.Y = Y;
   p.image = image;
-  p.dbg = dbg;
   p.B = B;
   p.H = H;
   p.W = W;
   p.tiles_x = Wo / kIrfTW;
   p.tiles_y = Ho / kIrfTH;
   p.num_tiles = B * p.tiles_x * p.tiles_y;
-  const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
-  if (launch_pdl(irf_s2_fused_kernel, dim3(grid), dim3(kIrfThreads), (size_t)kIrfSmemBytes, s, p) != cudaSuccess) return -31;
+  if (launch_pdl(irf_s2_fused_kernel, dim3(p.num_tiles), dim3(kIrfThreads), (size_t)kIrfSmemBytes, s, p) != cudaSuccess) return -31;
   return 0;
 }
 

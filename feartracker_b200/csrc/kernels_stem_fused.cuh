@@ -1,4 +1,4 @@
-// Fused stem + xif1_0 kernel (CUDA cores, weights in the constant bank, input patch by TMA).  sm_100a.
+// Fused stem + xif1_0 kernel (CUDA cores, weights in the constant bank, input patch by TMA).  sm_90a.
 #pragma once
 #include "kernels_ffma.cuh"
 #include "tc_common.cuh"

@@ -1,7 +1,7 @@
-// tcgen05 / TMEM / TMA kernels of the FEAR-XS hot path (sm_100a only).
+// wgmma / TMA kernels of the FEAR-XS hot path (sm_90a only).
 //
-// corr_ts_kernel -- the pixel-wise template (x) search correlation (MobileCorrelation.forward's matmul,
-// reference model_training/model/blocks.py:123) on the 5th-generation tensor cores:
+// corr_tc_kernel -- the pixel-wise template (x) search correlation (MobileCorrelation.forward's matmul,
+// reference model_training/model/blocks.py:123) on the Hopper tensor cores:
 //
 //     s[b, p, k] = sum_c x[b, p, c] * z[b, k, c]        p in 256 search cells, k in 64 template cells, c in 256
 //
@@ -10,15 +10,23 @@
 // The result goes straight into channels [256,320) of the same buffer, so the "torch.cat" of the
 // reference costs nothing and the kernel moves exactly the algorithmic bytes (z + x in, s out).
 //
-// fp32 fidelity: kind::tf32 keeps 11 significand bits, which fails the 1e-3 parity bar (SURVEY.md
+// fp32 fidelity: tf32 keeps 11 significand bits, which fails the 1e-3 parity bar (SURVEY.md
 // section 7.4), so each operand is split on the fly into tf32 (hi, lo) pairs and three products
-// (hi*hi + hi*lo + lo*hi) accumulate in TMEM in fp32 -- error ~1e-6, still far above the FFMA rate.
+// (hi*hi + hi*lo + lo*hi) accumulate in fp32 registers -- error ~1e-6, still far above the FFMA rate.
 //
 // pw_tc_kernel -- every 1x1 convolution as a 3xTF32 GEMM on the same pipeline (optionally with the preceding
-// depthwise conv computed by its producer warps).
+// depthwise conv computed by its consumer warps).
+//
+// Common shape of the kernels: one CTA per 128-row tile = two consumer warpgroups of 64 rows each plus one TMA
+// producer warp; K streamed in 32-channel chunks (one 128-byte swizzled row) through an mbarrier ring.  The A
+// operand of every wgmma comes from REGISTERS: a consumer thread reads its fragment of the raw fp32 tile from
+// shared memory once, splits it into (hi, lo) in registers and issues the three products against the weight tiles
+// in shared memory, so no lo tile of the activations is ever written.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdlib.h>
+
+#include <initializer_list>
 
 #include "tc_common.cuh"
 
@@ -28,266 +36,99 @@ namespace tc {
 constexpr int kCorrChunk = 32;                 // channels per stage = one 128-byte swizzled row
 constexpr int kCorrABytes = 128 * 128;         // [128 pixels][32 ch] fp32
 constexpr int kCorrBBytes = 64 * 128;          // [64 template cells][32 ch] fp32
+constexpr int kTcThreads = 288;                // 2 consumer warpgroups + the TMA producer warp
+constexpr int kTcConsumers = 256;
+
+// named barrier over the consumer warps (the producer warp never joins)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
-// corr_ts_kernel -- the same correlation with the search-feature operand in TENSOR MEMORY ("TS" form) and TWO MMA issuers.
-//
-// Two measured facts shape it (tools/microbench/mma_rate.cu, profiles/r2_mma_issue_rate.txt):
-//  * one warp gets a tcgen05.mma accepted only every ~105-115 clk whatever its size (N <= 128): 12 small MMAs per 24 KB
-//    chunk from ONE issuer (the first round-2 version) cost ~1300 clk of issue time against the ~900 clk the chunk takes to
-//    arrive from HBM at the SM's share of the bandwidth.  Issuers in different warps overlap, so the products are divided between two warps, each
-//    owning its accumulators (the accumulation order inside every accumulator stays fixed => deterministic results);
-//  * with both operands in shared memory a chunk moves ~144 KB through the SM's 128 B/clk shared-memory port (TMA write,
-//    split read + lo write, three MMAs re-reading the 16 KB x tile) -- 1150 clk.  Here the convert warps read the raw x
-//    tile ONCE, split it in registers and park (hi, lo) in TMEM with tcgen05.st; only the template tiles are MMA operands
-//    in shared memory: ~80 KB per chunk.
-//
-// Per K-step (8 channels):  issuer A:  [main | c1] += x_hi * [z_hi ; z_lo]^T   (one N = 128 MMA: z_lo is written right
-//                                                                              behind the raw z tile of the stage)
-//                           issuer B:  c2 += x_lo * z_hi^T                     (N = 64)
-// and the epilogue writes main + (c1 + c2).  TMEM (512 columns): two accumulator sets of 192 columns, then two A slots of
-// (32 hi + 32 lo) columns.
+// corr_tc_kernel: tile = half a frame (128 search cells) x 64 template cells, K = 256 in 8 chunks.  The template
+// tile is an MMA operand in shared memory and is not pre-split: the consumers rewrite each landed tile as hi
+// (low mantissa bits cleared, in place) and write lo right behind it.
 // ------------------------------------------------------------------------------------------
-constexpr int kCtsStages = 6;
-constexpr int kCtsSlots = 2;
-constexpr int kCtsStageBytes = kCorrABytes + 2 * kCorrBBytes;  // x raw | z raw | z lo
-constexpr int kCtsThreads = 15 * 32;  // producer, issuer A, 8 convert warps, 4 epilogue warps, issuer B
-constexpr int kCtsSmemBytes = kCtsStages * kCtsStageBytes + 1024 /*align*/ + 256 /*barriers*/ + 8192 /*epilogue*/;
-#ifdef FEAR_CORR_ABLATE
-// profiling build only: bit mask of pipeline roles that skip their work (barrier traffic kept) -- tools/corr_ablate.py
-__device__ int g_corr_ablate = 0;
-#define CORR_ABL(bit) (abl & (bit))
-#else
-#define CORR_ABL(bit) false
-#endif
+constexpr int kCorrStages = 3;
+constexpr int kCorrStageBytes = kCorrABytes + 2 * kCorrBBytes;  // x raw | z hi | z lo
+constexpr int kCorrSmemBytes = kCorrStages * kCorrStageBytes + 1024 /*align*/ + 256 /*barriers*/;
 
-__global__ void __launch_bounds__(kCtsThreads, 1)
-corr_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               float* __restrict__ cat, int num_frames, int z_mod) {
+__global__ void __launch_bounds__(kTcThreads, 1)
+corr_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               float* __restrict__ cat, int z_mod) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kCtsStages * kCtsStageBytes);
-  uint64_t* full = bars;                          // [stages] TMA landed
-  uint64_t* empty = bars + kCtsStages;            // [stages] x tile read by the 8 convert warps + z tiles read by both issuers' MMAs
-  uint64_t* slot_full = bars + 2 * kCtsStages;    // [slots] (hi, lo) of x in TMEM and z_lo in smem written (8 warps)
-  uint64_t* slot_empty = slot_full + kCtsSlots;   // [slots] both issuers' MMAs reading the slot have completed
-  uint64_t* acc_full = slot_empty + kCtsSlots;    // [2] (both issuers)
-  uint64_t* acc_empty = acc_full + 2;             // [2] (4 epilogue warps)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  uint8_t* epi_stage = reinterpret_cast<uint8_t*>(bars) + 256;  // 4 warps x 2 KB
-
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kCorrStages * kCorrStageBytes);  // [stages] TMA landed
+  uint64_t* empty = full + kCorrStages;                                                // [stages] 8 consumer warps done
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_tiles = num_frames * 2;
   constexpr int kChunks = 256 / kCorrChunk;
-  constexpr uint32_t kColSlots = 384;
-#ifdef FEAR_CORR_ABLATE
-  const int abl = g_corr_ablate;
-#endif
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  if (threadIdx.x == 64) {
-    for (int s = 0; s < kCtsStages; ++s) {
+    for (int s = 0; s < kCorrStages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 10);
-    }
-    for (int a = 0; a < kCtsSlots; ++a) {
-      mbar_init(&slot_full[a], 8);
-      mbar_init(&slot_empty[a], 2);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&acc_full[a], 2);
-      mbar_init(&acc_empty[a], 4);
+      mbar_init(&empty[s], 8);
     }
     fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_trigger();
   pdl_wait();
+  const int frame = blockIdx.x >> 1, half = blockIdx.x & 1;
+  const int arow = frame * 256 + half * 128;
+  auto st_x = [&](int s) { return smem + s * kCorrStageBytes; };
+  auto st_z = [&](int s) { return smem + s * kCorrStageBytes + kCorrABytes; };
 
-  auto st_x = [&](int s) { return smem + s * kCtsStageBytes; };
-  auto st_z = [&](int s) { return smem + s * kCtsStageBytes + kCorrABytes; };  // raw (= hi) tile, lo tile right behind it
-
-  if (warp == 0) {
-    // ===================================== TMA producer =====================================
+  if (warp == 8) {
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int frame = t >> 1, half = t & 1;
-        const int arow = frame * 256 + half * 128;
-        const int brow = z_mod ? (frame % z_mod) * 64 : 0;
-        for (int c = 0; c < kChunks; ++c) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full[stage], kCorrABytes + kCorrBBytes);
-          tma_load_2d(st_x(stage), &tmA, &full[stage], c * kCorrChunk, CORR_ABL(8) ? (int)(blockIdx.x & 1) * 128 : arow);
-          tma_load_2d(st_z(stage), &tmB, &full[stage], c * kCorrChunk, brow);
-          if (++stage == kCtsStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
+      const int brow = z_mod ? (frame % z_mod) * 64 : 0;
+      for (int c = 0; c < kChunks; ++c) {
+        const int stage = c % kCorrStages;
+        mbar_wait_backoff(&empty[stage], (uint32_t)(((c / kCorrStages) & 1) ^ 1));
+        mbar_arrive_expect_tx(&full[stage], kCorrABytes + kCorrBBytes);
+        tma_load_2d(st_x(stage), &tmA, &full[stage], c * kCorrChunk, arow);
+        tma_load_2d(st_z(stage), &tmB, &full[stage], c * kCorrChunk, brow);
       }
     }
-  } else if (warp == 1 || warp == 14) {
-    // ============================ MMA issuers: A (warp 1) = x_hi products, B (warp 14) = x_lo product ============================
-    if (lane == 0) {
-      const bool issuer_b = warp == 14;
-      const uint32_t idesc = issuer_b ? umma_idesc_tf32(128, 64) : umma_idesc_tf32(128, 128);
-      int stage = 0, acc = 0, q = 0;
-      uint32_t acc_phase = 0, phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + acc * 192 + (issuer_b ? 128 : 0);  // A: [main | c1] (128 columns); B: c2 (64)
-        for (int c = 0; c < kChunks; ++c, ++q) {
-          const int slot = q % kCtsSlots;
-          mbar_wait(&full[stage], phase);  // z tile (raw = hi) landed
-          mbar_wait(&slot_full[slot], (uint32_t)((q / kCtsSlots) & 1));
-          tc_fence_after();
-          const uint32_t a = tmem_base + kColSlots + slot * 64 + (issuer_b ? 32 : 0);
-          const uint32_t bz = smem_u32(st_z(stage));
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (CORR_ABL(1)) break;
-            mma_tf32_ts(d, a + j * 8, umma_desc_k_sw128(bz + j * 32), idesc, (c | j) != 0);
-          }
-          tc_commit(&empty[stage]);      // this issuer's reads of the stage's z tiles
-          tc_commit(&slot_empty[slot]);  // ... and of the TMEM A slot
-          if (++stage == kCtsStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        tc_commit(&acc_full[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp < 10) {
-    // ============================ convert: smem fp32 -> TMEM (hi, lo), z -> z_lo ============================
-    // 8 warps: two per TMEM lane quadrant, each converting 16 of the 32 channels of its 32 rows
-    const int qd = warp & 3;            // TMEM lane quadrant of this warp
-    const int hh = (warp - 2) >> 2;     // which 16-channel half of the chunk
-    const int row = qd * 32 + lane;     // x-tile row handled by this thread (= TMEM lane)
-    const int ts = threadIdx.x - 64;    // 0..255
-    int stage = 0, q = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      for (int c = 0; c < kChunks; ++c, ++q) {
-        const int slot = q % kCtsSlots;
-        mbar_wait(&full[stage], phase);
-        mbar_wait(&slot_empty[slot], (uint32_t)(((q / kCtsSlots) & 1) ^ 1));
-        tc_fence_after();
-        if (!CORR_ABL(2)) {
-          const float4* xrow = reinterpret_cast<const float4*>(st_x(stage) + row * 128);
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float4 v = xrow[(hh * 4 + j) ^ (row & 7)];  // SWIZZLE_128B: 16-byte chunk index ^ (row % 8)
-            const float f[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const uint32_t h = __float_as_uint(f[e]) & 0xFFFFE000u;  // what kind::tf32 reads from the raw word
-              hi[4 * j + e] = h;
-              lo[4 * j + e] = __float_as_uint(f[e] - __uint_as_float(h));
-            }
-          }
-          const uint32_t tdst = tmem_base + kColSlots + slot * 64 + ((uint32_t)(qd * 32) << 16);
-          tmem_st_32x16(tdst + hh * 16, hi);
-          tmem_st_32x16(tdst + 32 + hh * 16, lo);
-          // template tile: lo = v - trunc(v) at the same swizzled positions (index-identical copy)
-          const float4* zsrc = reinterpret_cast<const float4*>(st_z(stage));
-          float4* zdst = reinterpret_cast<float4*>(st_z(stage) + kCorrBBytes);
-#pragma unroll
-          for (int i = 0; i < kCorrBBytes / 16 / 256; ++i) {
-            const float4 v = zsrc[ts + i * 256];
-            float4 h, l;
-            split_tf32_trunc(v.x, h.x, l.x);
-            split_tf32_trunc(v.y, h.y, l.y);
-            split_tf32_trunc(v.z, h.z, l.z);
-            split_tf32_trunc(v.w, h.w, l.w);
-            zdst[ts + i * 256] = l;
-          }
-        }
-        tmem_st_wait();
-        tc_fence_before();
-        fence_proxy_async_smem();  // z_lo: generic-proxy writes -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&empty[stage]);  // this warp has read the stage's x tile
-          mbar_arrive(&slot_full[slot]);
-        }
-        if (++stage == kCtsStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ===================================== epilogue (warps 10..13) =====================================
-    // TMEM -> registers -> per-warp smem staging (2 KB) -> 16-byte coalesced stores into cat[:, 256 + k]
-    const int qd = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    float4* stg = reinterpret_cast<float4*>(epi_stage + qd * 2048);
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int frame = t >> 1, half = t & 1;
-      mbar_wait(&acc_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + acc * 192 + ((uint32_t)(qd * 32) << 16);
-      const long long row0 = (long long)frame * 256 + half * 128 + qd * 32;
-#pragma unroll
-      for (int g = 0; g < 64; g += 16) {
-        uint32_t m[16], c1[16], c2[16];
-        if (CORR_ABL(4)) {
-          if (g == 48) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[acc]);
-          }
-          continue;
-        }
-        tmem_ld_32x16(taddr + g, m);
-        tmem_ld_32x16(taddr + 64 + g, c1);
-        tmem_ld_32x16(taddr + 128 + g, c2);
-        tmem_ld_wait();
-        if (g == 48) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[acc]);  // accumulators free for tile t+2
-        }
-        auto sum = [&](int i) { return __uint_as_float(m[i]) + (__uint_as_float(c1[i]) + __uint_as_float(c2[i])); };
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          stg[lane * 4 + (j ^ ((lane >> 1) & 3))] = make_float4(sum(4 * j), sum(4 * j + 1), sum(4 * j + 2), sum(4 * j + 3));
-        __syncwarp();
-        const int j = lane & 3;
-#pragma unroll
-        for (int rb = 0; rb < 4; ++rb) {
-          const int rl = rb * 8 + (lane >> 2);
-          *reinterpret_cast<float4*>(cat + (row0 + rl) * 320 + 256 + g + j * 4) = stg[rl * 4 + (j ^ ((rl >> 1) & 3))];
-        }
-        __syncwarp();
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    return;
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  const int wg = warp >> 2, r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), t = lane & 3;
+  float accm[32], accc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) accm[i] = accc[i] = 0.f;
+  for (int c = 0; c < kChunks; ++c) {
+    const int stage = c % kCorrStages;
+    mbar_wait(&full[stage], (uint32_t)((c / kCorrStages) & 1));
+    float4* zh = reinterpret_cast<float4*>(st_z(stage));
+    float4* zl = reinterpret_cast<float4*>(st_z(stage) + kCorrBBytes);
+#pragma unroll
+    for (int i = 0; i < kCorrBBytes / 16 / kTcConsumers; ++i) {  // index-identical copy: the swizzle carries over
+      const float4 v = zh[threadIdx.x + i * kTcConsumers];
+      float4 h, l;
+      split_tf32_trunc(v.x, h.x, l.x);
+      split_tf32_trunc(v.y, h.y, l.y);
+      split_tf32_trunc(v.z, h.z, l.z);
+      split_tf32_trunc(v.w, h.w, l.w);
+      zh[threadIdx.x + i * kTcConsumers] = h;
+      zl[threadIdx.x + i * kTcConsumers] = l;
+    }
+    fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
+    consumer_sync();
+    uint32_t hi[4][4], lo[4][4];
+    load_a_frags(st_x(stage), r0, t, hi, lo);
+    const uint32_t bh = smem_u32(zh), bl = smem_u32(zl);
+    wg_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) mma3<64>(accm, accc, hi[j], lo[j], bh + j * 32, bl + j * 32);
+    wg_commit();
+    wg_wait();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);
+  }
+  float* out = cat + (long long)(arow + r0) * 320 + 256 + 2 * t;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    *reinterpret_cast<float2*>(out + 8 * i) = make_float2(accm[4 * i] + accc[4 * i], accm[4 * i + 1] + accc[4 * i + 1]);
+    *reinterpret_cast<float2*>(out + 8 * 320 + 8 * i) =
+        make_float2(accm[4 * i + 2] + accc[4 * i + 2], accm[4 * i + 3] + accc[4 * i + 3]);
   }
 }
 
@@ -305,8 +146,8 @@ inline int init() {
   DeviceState& st = dev_state();
   st.num_sms = p.multiProcessorCount;
   st.inited = true;
-  if (resolve_driver()) return 0;  // tcgen05 path stays unavailable; the FFMA path still works
-  if (cudaFuncSetAttribute(corr_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCtsSmemBytes) != cudaSuccess) {
+  if (resolve_driver()) return 0;  // tensor-core / TMA path stays unavailable; the FFMA path still works
+  if (cudaFuncSetAttribute(corr_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCorrSmemBytes) != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
@@ -316,8 +157,7 @@ inline int init() {
 }
 
 // cat holds `groups` consecutive [B][256][320] buffers (the cls and reg branches of the head): frame f of
-// every group correlates with template f (or template 0 when Bz == 1).  One launch for all groups keeps
-// the persistent grid busy for ~7 tile rounds instead of 3.46, i.e. almost no tail.
+// every group correlates with template f (or template 0 when Bz == 1).  One launch covers all groups.
 inline int launch_corr(cudaStream_t s, const float* zt, int Bz, float* cat, int B, int groups) {
   if (!available()) return -20;
   CUtensorMap tmA, tmB;
@@ -327,734 +167,208 @@ inline int launch_corr(cudaStream_t s, const float* zt, int Bz, float* cat, int 
   if (r) return r;
   r = make_tmap_2d(&tmB, zt, (uint64_t)Bz * 64, 256, 256, 64, kCorrChunk);
   if (r) return r;
-  const int tiles = frames * 2;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  if (launch_pdl(corr_ts_kernel, dim3(grid), dim3(kCtsThreads), kCtsSmemBytes, s, tmA, tmB, cat, frames, Bz == 1 ? 0 : B) !=
+  if (launch_pdl(corr_tc_kernel, dim3(frames * 2), dim3(kTcThreads), kCorrSmemBytes, s, tmA, tmB, cat, Bz == 1 ? 0 : B) !=
       cudaSuccess)
     return -23;
   return 0;
 }
 
 // ------------------------------------------------------------------------------------------
-// pw_tc_kernel -- 1x1 convolution as a GEMM on tcgen05:  C[M][N] = act(A[M][K] * W[N][K]^T + bias (+ R))
+// pw_tc_kernel -- 1x1 convolution as a GEMM on wgmma:  C[M][N] = act(A[M][K] * W[N][K]^T + bias (+ R))
 // A = channels-last activations (rows = pixels), W = BN-folded torch-native [Cout][Cin] weights,
-// pre-split on the host into tf32 (hi, lo) copies; A is split on the fly exactly like in the
-// correlation kernel.  Persistent CTAs walk (m_tile, n_tile) pairs, n fastest; tile = 128 pixels x NT
-// output channels (NT multiple of 16, <= 256), K streamed in 32-channel chunks through an S-stage ring
-// (S chosen from the stage size).  TMA zero-fills the K tail (Cin not a multiple of 32), rows >= M
-// and weight rows >= N.  Two TMEM accumulators of NT columns each overlap epilogue and MMA.
+// pre-split on the host into tf32 (hi, lo) copies; A is split in registers.  One CTA per (m_tile, n_tile) pair,
+// n fastest; tile = 128 pixels x NT output channels.  TMA zero-fills the K tail (Cin not a multiple of 32),
+// rows >= M and weight rows >= N; the epilogue clips the M / N tails.
 // ------------------------------------------------------------------------------------------
-#ifdef FEAR_PW_ABLATE
-// profiling build only: roles of pw_tc_kernel that skip their work (barrier traffic kept; results are garbage) --
-// tools/pw_ablate.py.  1 = MMAs, 2 = operand split / depthwise compute + A-tile writes, 4 = epilogue, 8 = weight loads,
-// 16 = activation (A tile / depthwise input box) loads
-__device__ int g_pw_ablate = 0;
-#define PW_ABL(bit) (pw_abl & (bit))
-#else
-#define PW_ABL(bit) false
-#endif
-
-#ifdef FEAR_PW_TIMING
-// profiling build only: per-launch, per-role cycle counters (summed over CTAs) -- tools/pw_timing.py
-__device__ unsigned long long g_pw_timing[64][32];
-inline int& pw_timing_next() {
-  static int n = 0;
-  return n;
-}
-struct PwTimingInfo { int M, N, K, dwk, map_w, grid, tiles, chunks; };
-inline PwTimingInfo* pw_timing_info() {
-  static PwTimingInfo info[64];
-  return info;
-}
-#define PWT(v) const long long v = clock64()
-#define PWT_ACC(slot, a, b) pwt[slot] += (unsigned long long)((b) - (a))
-#define PWT_FLUSH(lo, hi)                                                                              \
-  if (lane == 0)                                                                                       \
-    for (int k_ = (lo); k_ < (hi); ++k_) atomicAdd(&g_pw_timing[p.timing_id & 63][k_], pwt[k_])
-#else
-#define PWT(v)
-#define PWT_ACC(slot, a, b)
-#define PWT_FLUSH(lo, hi)
-#endif
-
 struct PwParams {
   const float* bias;  // [N] or null
   const float* R;     // residual [M][ldr] or null
   float* C;
   int ldr, ldc;
-  int M, N, NT, num_n_tiles, num_chunks, last_ksteps, relu, stages, stage_bytes, tmem_cols;
-  int split_acc;  // 1: hi*hi and the cross terms accumulate separately (long K); 0: one accumulator (K <= 64)
-  int acc_stride; // TMEM columns per accumulator stage: 2*NT (main + correction) or NT
-  // --- fused depthwise producer (pw_tc_kernel<DWK>, DWK = 3 | 5): the A operand is dw(X) computed on the fly ---
+  int M, N, num_n_tiles, num_chunks, last_ksteps, relu, stages, stage_bytes;
+  // --- fused depthwise producer (DWK = 3 | 5): the A operand is dw(X) computed on the fly ---
   int dw_relu, dw_bias;  // ReLU / bias of the depthwise stage
   int box_bytes;         // bytes of one (tile rows + DWK - 1) x (map width + DWK - 1) x 32-channel input box
-  int map_w;             // fused depthwise: square map side, 16 (tile = 8 rows x 16) or 32 (tile = 4 rows x 32)
-#ifdef FEAR_PW_TIMING
-  int timing_id;
-#endif
-  int w_region;   // > 0: the (hi, lo) weight tile is loaded ONCE into the first w_region bytes of smem (layers with one
-                  // N tile and one K chunk) and the ring stages hold activations only
 };
 
-constexpr int kPwTsSlotCol = 384;  // TS form: two 64-column (32 hi + 32 lo) A slots behind <= 384 accumulator columns
-constexpr int kPwThreads = 608;  // producer, MMA, 8 split / depthwise warps, 8 epilogue warps, depthwise-box producer
-
-// DWK = 0: plain 1x1 conv.  DWK = 3 | 5 (option "fuse_dwpw", on by default; 16x16 and 32x32 maps, stride 1): the layer's input is
-// the output of a DWK x DWK depthwise conv that is never materialised -- the producer TMA-loads the depthwise INPUT
-// box of each (128-pixel tile, 32-channel chunk) with its zero-filled halo (tmA is then the 4-D NHWC map of X), two
-// groups of four "split" warps take alternate chunks, run the depthwise conv out of shared memory (same FMA order as
-// dw_tma_kernel => same fp32 values as the unfused pair of kernels) and write the (hi, lo) A tiles directly in the
-// SWIZZLE_128B K-major layout the MMA descriptors expect.  Everything downstream is unchanged.
-//
-// TS = true (plain 1x1 convs whose accumulators leave 128 TMEM columns free): the A operand goes to TENSOR MEMORY.  The eight
-// operand-split warps read the raw tile once (row per lane, swizzle-aware LDS.128), split it in registers and store
-// (hi, lo) with tcgen05.st into one of two 64-column slots; the MMAs take A from TMEM.  No lo tile is written to and no A
-// tile is read back from shared memory (40 % less shared-memory traffic per chunk; measured +0.5 % on the step only, because the
-// K >= 64 GEMMs turned out to be bound by the MMA issue rate, DESIGN.md 4.1), the two
-// 16 KB lo buffers become ring stages, and the N = 2 NT stacked MMA runs at the TS rate.  Same products in the same order as
-// the shared-memory form: bit-identical results.
-template <int DWK, int MW = 16, bool TS = false>
-__global__ void __launch_bounds__(kPwThreads, 1)
+// DWK = 0: plain 1x1 conv.  DWK = 3 | 5 (option "fuse_dwpw", on by default; MW x MW maps with MW = 16 | 32, stride 1): the
+// layer's input is the output of a DWK x DWK depthwise conv that is never materialised -- the producer TMA-loads the
+// depthwise INPUT box of each (128-pixel tile, 32-channel chunk) with its zero-filled halo (tmA is then the 4-D NHWC
+// map of X), the consumer warps run the depthwise conv out of shared memory (same FMA order as dw_tma_kernel => same
+// fp32 values as the unfused pair of kernels) and write the A tile in the SWIZZLE_128B layout the fragment loads expect.
+template <int NT, int DWK, int MW = 16>
+__global__ void __launch_bounds__(kTcThreads, 1)
 pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWh,
-             const __grid_constant__ CUtensorMap tmWl, const __grid_constant__ CUtensorMap tmC,
-             const __grid_constant__ CUtensorMap tmDW, const __grid_constant__ CUtensorMap tmDB, const PwParams p) {
+             const __grid_constant__ CUtensorMap tmWl, const __grid_constant__ CUtensorMap tmDW,
+             const __grid_constant__ CUtensorMap tmDB, const PwParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // offset arithmetic keeps LDS/STS
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int S = p.stages;
-  // DWK == 0: the lo halves of the A operand live in TWO dedicated 16 KB buffers, not in the TMA ring: a ring stage is
-  // then pure landing space (raw A tile + weight tiles), i.e. every byte of it can be "in flight" -- these GEMMs are
-  // bound by bytes in flight / loaded latency (Little's law: 3 x 44 KB per SM gave 22 B/clk), not by the tensor pipe.
-  uint8_t* lo_buf = smem + p.w_region;
-  static_assert(!TS || DWK == 0, "the tensor-memory A operand is for the plain 1x1 convs");
-  uint8_t* ring = lo_buf + ((DWK == 0 && !TS) ? 2 * kCorrABytes : 0);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + S * p.stage_bytes);
-  uint64_t* full = bars;
-  uint64_t* split = bars + S;  // DWK == 0: split[0..1] = lo buffer written; DWK > 0: per stage
-  uint64_t* empty = bars + 2 * S;
-  uint64_t* acc_full = bars + 3 * S;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* w_full = acc_empty + 2;
-  uint64_t* lo_empty = w_full + 1;  // [2] DWK == 0: the MMAs that read the lo buffer have completed
-  uint64_t* wfl = lo_empty + 2;     // [2] DWK > 0: the stage's weight tiles have landed (TMA producer warp)
-  uint64_t* box_empty = wfl + 2;    // [2] DWK > 0: the 4 depthwise warps of the owning group have read the input box
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(box_empty + 2);
-  uint8_t* epi_stage = reinterpret_cast<uint8_t*>(bars) + 1024;      // 8 warps x 2 buffers x 2 KB, 512-B aligned
-  float* sbias = reinterpret_cast<float*>(epi_stage + 8 * 2 * 2048);  // [2][256] per accumulator stage
-
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * p.stage_bytes);
+  uint64_t* empty = full + S;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#ifdef FEAR_PW_ABLATE
-  const int pw_abl = g_pw_ablate;
-#endif
-#ifdef FEAR_PW_TIMING
-  unsigned long long pwt[32];
-#pragma unroll
-  for (int k_ = 0; k_ < 32; ++k_) pwt[k_] = 0;
-#endif
-  const int num_m_tiles = (p.M + 127) >> 7;
-  const int num_tiles = num_m_tiles * p.num_n_tiles;
-  const int w_bytes = p.NT * 128;
-
-  if (warp == 0 && lane == 0) {
+  constexpr int w_bytes = NT * 128;
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmWh);
     prefetch_tmap(&tmWl);
-    prefetch_tmap(&tmC);
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  if (threadIdx.x == 64) {
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&split[s], DWK ? 4 : 8);
-      mbar_init(&empty[s], TS ? 9 : 1);  // TS: the 8 split warps read the A tile, the MMAs only the weight tiles
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&acc_full[a], 1);
-      mbar_init(&acc_empty[a], 8);
-    }
-    mbar_init(w_full, 1);
-    mbar_init(&lo_empty[0], 1);
-    mbar_init(&lo_empty[1], 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&wfl[a], 1);
-      mbar_init(&box_empty[a], 4);
+      mbar_init(&empty[s], 8);
     }
     fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const bool resident_w = p.w_region != 0;
   pdl_trigger();  // the next kernel may start its prologue on SMs we have left
   pdl_wait();     // everything above overlapped the previous kernel's tail; its results are visible from here on
 
-  constexpr int kAStage = DWK == 0 ? kCorrABytes : 2 * kCorrABytes;  // A part of a ring stage: raw tile (+ lo tile when fused)
-  auto a_hi = [&](int s) { return ring + s * p.stage_bytes; };
-  auto a_lo = [&](int s) { return ring + s * p.stage_bytes + kCorrABytes; };  // (DWK > 0 only)
-  auto w_hi = [&](int s) { return resident_w ? smem : ring + s * p.stage_bytes + kAStage; };
-  auto w_lo = [&](int s) { return resident_w ? smem + w_bytes : ring + s * p.stage_bytes + kAStage + w_bytes; };
-  // fused-depthwise stages: [a_hi][a_lo][w_hi][w_lo][input box][dw weights DWK*DWK x 32][dw bias 32]
-  auto dw_box = [&](int s) { return ring + s * p.stage_bytes + 2 * kCorrABytes + 2 * w_bytes; };
+  const int mt = blockIdx.x / p.num_n_tiles, nt = blockIdx.x - mt * p.num_n_tiles;
+  // stage: [A tile 16 KB][w_hi][w_lo] (+ fused depthwise: [input box][dw weights DWK*DWK x 32][dw bias 32])
+  auto a_tile = [&](int s) { return smem + s * p.stage_bytes; };
+  auto w_hi = [&](int s) { return smem + s * p.stage_bytes + kCorrABytes; };
+  auto w_lo = [&](int s) { return w_hi(s) + w_bytes; };
+  auto dw_box = [&](int s) { return w_lo(s) + w_bytes; };
   auto dw_wts = [&](int s) { return dw_box(s) + p.box_bytes; };
   auto dw_bia = [&](int s) { return dw_wts(s) + DWK * DWK * 128; };
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      if (resident_w) {  // one N tile, one K chunk: the weights never change -- fetch them once
-        mbar_arrive_expect_tx(w_full, 2 * w_bytes);
-        tma_load_2d(w_hi(0), &tmWh, w_full, 0, 0);
-        tma_load_2d(w_lo(0), &tmWl, w_full, 0, 0);
-      }
-      PWT(tp0);
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int mt = t / p.num_n_tiles, nt = t - mt * p.num_n_tiles;
-        for (int c = 0; c < p.num_chunks; ++c) {
-          PWT(tp1);
-          mbar_wait(&empty[stage], phase ^ 1);
-          PWT(tp2);
-          PWT_ACC(0, tp1, tp2);
-          if constexpr (DWK > 0) {
-            // weight tiles only: the input box of a stage is re-filled by the depthwise group that owns the stage as soon
-            // as it has read it (well before the MMAs release the stage), see below
-            mbar_arrive_expect_tx(&wfl[stage], PW_ABL(8) ? 0 : 2 * w_bytes);
-            if (!PW_ABL(8)) {
-              tma_load_2d(w_hi(stage), &tmWh, &wfl[stage], c * 32, nt * p.NT);
-              tma_load_2d(w_lo(stage), &tmWl, &wfl[stage], c * 32, nt * p.NT);
-            }
-            if (++stage == S) {
-              stage = 0;
-              phase ^= 1;
-            }
-            continue;
-          }
-          mbar_arrive_expect_tx(&full[stage], (PW_ABL(16) ? 0 : kCorrABytes) + ((resident_w || PW_ABL(8)) ? 0 : 2 * w_bytes));
-          if (!PW_ABL(16)) tma_load_2d(a_hi(stage), &tmA, &full[stage], c * 32, mt * 128);
-          if (!resident_w && !PW_ABL(8)) {
-            tma_load_2d(w_hi(stage), &tmWh, &full[stage], c * 32, nt * p.NT);
-            tma_load_2d(w_lo(stage), &tmWl, &full[stage], c * 32, nt * p.NT);
-          }
-          if (++stage == S) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-      PWT(tp3);
-      PWT_ACC(1, tp0, tp3);
-      PWT_FLUSH(0, 2);
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_tf32(128, p.NT);
-      const uint32_t idesc2 = umma_idesc_tf32(128, 2 * p.NT);  // stacked [W_hi ; W_lo] (NT <= 128)
-      int stage = 0, acc = 0, q = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      if (resident_w) mbar_wait(w_full, 0);
-      PWT(tm0);
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        PWT(tm1);
-        mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-        PWT(tm2);
-        PWT_ACC(2, tm1, tm2);
-        tc_fence_after();
-        const uint32_t d = tmem_base + acc * p.acc_stride;  // main; + NT = correction accumulator (split_acc)
-        for (int c = 0; c < p.num_chunks; ++c, ++q) {
-          PWT(tm3);
-          if constexpr (DWK == 0) {
-            mbar_wait(&split[q & 1], (uint32_t)((q >> 1) & 1));  // lo buffer written (=> stage landed)
-          } else {
-            mbar_wait(&split[stage], phase);  // depthwise output (hi, lo) written
-            PWT(tm3b);
-            PWT_ACC(21, tm3, tm3b);
-            mbar_wait(&wfl[stage], phase);    // weight tiles landed
-          }
-          PWT(tm4);
-          PWT_ACC(3, tm3, tm4);
-          tc_fence_after();
-          const uint32_t ah = smem_u32(a_hi(stage));
-          const uint32_t al = DWK == 0 ? smem_u32(lo_buf + (q & 1) * kCorrABytes) : smem_u32(a_lo(stage));
-          const uint32_t bh = smem_u32(w_hi(stage)), bl = smem_u32(w_lo(stage));
-          const int ksteps = (c == p.num_chunks - 1) ? p.last_ksteps : 4;  // K tail: skip all-zero K-steps
-          for (int j = 0; j < ksteps; ++j) {
-            if (PW_ABL(1)) break;
-            const uint64_t dah = umma_desc_k_sw128(ah + j * 32), dal = umma_desc_k_sw128(al + j * 32);
-            const uint64_t dbh = umma_desc_k_sw128(bh + j * 32), dbl = umma_desc_k_sw128(bl + j * 32);
-            if constexpr (TS) {
-              const uint32_t tah = tmem_base + kPwTsSlotCol + (q & 1) * 64 + j * 8, tal = tah + 32;
-              if (p.split_acc) {
-                mma_tf32_ts(d, tah, dbh, idesc2, (c | j) != 0);
-                mma_tf32_ts(d + p.NT, tal, dbh, idesc, 1);
-              } else {
-                mma_tf32_ts(d, tah, dbh, idesc, (c | j) != 0);
-                mma_tf32_ts(d, tal, dbh, idesc, 1);
-                mma_tf32_ts(d, tah, dbl, idesc, 1);
-              }
-              continue;
-            }
-            // short K (<= 2 chunks): a handful of accumulations, the truncating adder is harmless and a single
-            // accumulator halves the TMEM read (64 B/clk/SM) that dominates the epilogue of the wide layers
-            if (p.split_acc) {
-              // W_hi and W_lo tiles are adjacent in smem: one N = 2*NT MMA gives [a_hi*w_hi | a_hi*w_lo] in the adjacent
-              // (main | correction) accumulators, so the A_hi tile is read from shared memory once instead of twice
-              mma_tf32_ss(d, dah, dbh, idesc2, (c | j) != 0);
-              mma_tf32_ss(d + p.NT, dal, dbh, idesc, 1);
-            } else {
-              mma_tf32_ss(d, dah, dbh, idesc, (c | j) != 0);
-              mma_tf32_ss(d, dal, dbh, idesc, 1);
-              mma_tf32_ss(d, dah, dbl, idesc, 1);
-            }
-          }
-          tc_commit(&empty[stage]);
-          if constexpr (DWK == 0) tc_commit(&lo_empty[q & 1]);
-          PWT(tm5);
-          PWT_ACC(4, tm4, tm5);
-          if (++stage == S) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        tc_commit(&acc_full[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-      PWT(tm6);
-      PWT_ACC(5, tm0, tm6);
-      PWT_FLUSH(2, 6);
-      PWT_FLUSH(21, 22);
-    }
-  } else if (warp < 10) {
-    const int ts = threadIdx.x - 64;  // 0..255
-    int stage = 0;
-    uint32_t phase = 0;
-    if constexpr (DWK > 0) {
-      // ---- fused depthwise: group g (4 warps) owns stage g (S == 2); thread = (2-channel pair, 2 x 8 pixel block) ----
-      // These kernels are bound by the shared-memory port (tools/pw_timing.py: the depthwise pass is 60 % of the kernel and
-      // slows down with everything else that moves through smem).  A thread owning 2 channels x 16 pixels instead of
-      // 4 channels x 8 pixels issues the same FFMA2s but 1/3 fewer LDS wavefronts: the halo of a 2 x 8 block is smaller
-      // and a weight is fetched once per 16 pixels (5x5: 194 instead of 292 wavefronts per warp and chunk).
-      constexpr int K = DWK, TX = 8, TY = 2, NIN = TX + K - 1, NR = TY + K - 1;
-      constexpr int IW = MW + K - 1, PXN = MW / TX;  // 8 positions: 2 across x 4 down (16x16) | 4 x 2 (32x32)
-      const int group = (warp - 2) >> 2, gw = (warp - 2) & 3;
-      const int c2 = lane & 15, pos = gw * 2 + (lane >> 4);
-      const int x0 = (pos % PXN) * TX, r0 = (pos / PXN) * TY;
-      int chunk = 0;
-      PWT(td0);
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        for (int c = 0; c < p.num_chunks; ++c, ++chunk) {
-          if ((chunk & 1) == group) {
-            PWT(td1);
-            mbar_wait(&full[stage], phase);
-            PWT(td2);
-            PWT_ACC(6, td1, td2);
-            typedef unsigned long long U2;  // two packed fp32 channels
-            const U2* in2 = reinterpret_cast<const U2*>(dw_box(stage));
-            const U2* w2 = reinterpret_cast<const U2*>(dw_wts(stage));
-            U2 acc[TY][TX];
-            const U2 bias2 = p.dw_bias ? reinterpret_cast<const U2*>(dw_bia(stage))[c2] : 0ull;
-#pragma unroll
-            for (int y = 0; y < TY; ++y)
-#pragma unroll
-              for (int i = 0; i < TX; ++i) acc[y][i] = bias2;
-            U2 wk[K][K];
-            const U2* base = in2 + (r0 * IW + x0) * 16 + c2;
-#pragma unroll
-            for (int r = 0; r < NR; ++r) {
-              if (PW_ABL(2)) break;
-              U2 v[NIN];
-#pragma unroll
-              for (int i = 0; i < NIN; ++i) v[i] = base[(r * IW + i) * 16];
-              if (r < K) {
-#pragma unroll
-                for (int kx = 0; kx < K; ++kx) wk[r < K ? r : 0][kx] = w2[(r * K + kx) * 16 + c2];
-              }
-#pragma unroll
-              for (int y = 0; y < TY; ++y) {
-                const int ky = r - y;
-                if (ky >= 0 && ky < K) {
-#pragma unroll
-                  for (int kx = 0; kx < K; ++kx) {
-                    const U2 k = wk[(ky >= 0 && ky < K) ? ky : 0][kx];
-#pragma unroll
-                    for (int i = 0; i < TX; ++i) ffma2(acc[y][i], v[i + kx], k);
-                  }
-                }
-              }
-            }
-            __syncwarp();
-            PWT(td3);
-            PWT_ACC(7, td2, td3);
-            if (lane == 0) mbar_arrive(&box_empty[stage]);  // this warp has read the box (warp 18 refills it)
-            PWT(td4);
-            PWT_ACC(8, td3, td4);
-            mbar_wait(&empty[stage], phase ^ 1);  // the MMAs of this stage's previous chunk have read its A tiles
-            PWT(td5);
-            PWT_ACC(9, td4, td5);
-            uint8_t* ah = a_hi(stage);
-            uint8_t* al = a_lo(stage);
-#pragma unroll
-            for (int y = 0; y < TY; ++y)
-#pragma unroll
-              for (int i = 0; i < TX; ++i) {
-                if (PW_ABL(2)) break;
-                float2 v = make_float2(__uint_as_float((uint32_t)acc[y][i]), __uint_as_float((uint32_t)(acc[y][i] >> 32)));
-                if (p.dw_relu) {
-                  v.x = fmaxf(v.x, 0.f);
-                  v.y = fmaxf(v.y, 0.f);
-                }
-                float2 h, l;
-                split_tf32_trunc(v.x, h.x, l.x);
-                split_tf32_trunc(v.y, h.y, l.y);
-                const int R = (r0 + y) * MW + x0 + i;                                         // A-tile row = pixel inside the tile
-                const int off = R * 128 + (((c2 >> 1) ^ (R & 7)) << 4) + ((c2 & 1) << 3);     // SWIZZLE_128B: 16-byte chunk ^ (row % 8)
-                *reinterpret_cast<float2*>(ah + off) = v;                                     // raw fp32 = hi operand (hardware truncation)
-                *reinterpret_cast<float2*>(al + off) = l;
-              }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&split[stage]);
-            PWT(td6);
-            PWT_ACC(10, td5, td6);
-          }
-          if (++stage == S) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-      PWT(td7);
-      PWT_ACC(11, td0, td7);
-      if (gw == 0 && group == 0) { PWT_FLUSH(6, 12); }
-    } else {
-    int q = 0;
-    PWT(ts0);
-    const int qd = warp & 3, hh = (warp - 2) >> 2, row = qd * 32 + lane;  // (TS) TMEM lane quadrant, channel half, tile row
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      for (int c = 0; c < p.num_chunks; ++c, ++q) {
-        PWT(ts1);
-        mbar_wait(&full[stage], phase);
-        PWT(ts2);
-        PWT_ACC(6, ts1, ts2);
-        mbar_wait(&lo_empty[q & 1], (uint32_t)(((q >> 1) & 1) ^ 1));  // the MMAs of chunk q - 2 have read this lo buffer / slot
-        PWT(ts3);
-        PWT_ACC(9, ts2, ts3);
-        if constexpr (TS) {
-          tc_fence_after();
-          if (!PW_ABL(2)) {
-            const float4* xrow = reinterpret_cast<const float4*>(a_hi(stage) + row * 128);
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float4 v = xrow[(hh * 4 + j) ^ (row & 7)];  // SWIZZLE_128B: 16-byte chunk index ^ (row % 8)
-              const float f[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const uint32_t h = __float_as_uint(f[e]) & 0xFFFFE000u;  // what kind::tf32 reads from the raw word
-                hi[4 * j + e] = h;
-                lo[4 * j + e] = __float_as_uint(f[e] - __uint_as_float(h));
-              }
-            }
-            const uint32_t tdst = tmem_base + kPwTsSlotCol + (q & 1) * 64 + ((uint32_t)(qd * 32) << 16);
-            tmem_st_32x16(tdst + hh * 16, hi);
-            tmem_st_32x16(tdst + 32 + hh * 16, lo);
-          }
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(&empty[stage]);  // this warp has read the stage's A tile
-            mbar_arrive(&split[q & 1]);
-          }
-          PWT(ts4t);
-          PWT_ACC(10, ts3, ts4t);
-          if (++stage == S) {
-            stage = 0;
-            phase ^= 1;
-          }
-          continue;
-        }
-        float4* ah = reinterpret_cast<float4*>(a_hi(stage));
-        float4* al = reinterpret_cast<float4*>(lo_buf + (q & 1) * kCorrABytes);
-#pragma unroll
-        for (int i = 0; i < kCorrABytes / 16 / 256; ++i) {
-          if (PW_ABL(2)) break;
-          const float4 v = ah[ts + i * 256];  // the raw tile is the hi operand as it stands (hardware truncation)
-          float4 h, l;
-          split_tf32_trunc(v.x, h.x, l.x);
-          split_tf32_trunc(v.y, h.y, l.y);
-          split_tf32_trunc(v.z, h.z, l.z);
-          split_tf32_trunc(v.w, h.w, l.w);
-          al[ts + i * 256] = l;
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&split[q & 1]);
-        PWT(ts4);
-        PWT_ACC(10, ts3, ts4);
-        if (++stage == S) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-    PWT(ts5);
-    PWT_ACC(11, ts0, ts5);
-    if (warp == 2) { PWT_FLUSH(6, 12); }
-    }
-  } else if (warp == 18) {
-    // ---- depthwise-box producer (DWK > 0): group g = chunk & 1 owns box g; chunk i + 2 is loaded into it as soon as the four
-    // warps of the group have READ chunk i -- not when the MMAs release the stage (the box is ~1/3 of a stage and its load
-    // latency was fully exposed with two stages), and by this warp rather than by one of the depthwise warps: the warp
-    // that waited for its three siblings wrote its share of the A tile last and delayed every chunk by that wait.
-    if constexpr (DWK > 0) {
-      if (lane == 0) {
-        constexpr int th = 128 / MW, tpf = MW / th;
-        struct It {
-          int t, c;
-        };
-        auto advance = [&](It& it) {
-          if (++it.c == p.num_chunks) {
-            it.c = 0;
-            it.t += gridDim.x;
-          }
-        };
-        auto load_box = [&](const It& it, int st) {
-          const int mt2 = it.t / p.num_n_tiles;
-          mbar_arrive_expect_tx(&full[st], (PW_ABL(16) ? 0 : p.box_bytes) + DWK * DWK * 128 + (p.dw_bias ? 128 : 0));
-          if (!PW_ABL(16))
-            tma_load_4d(dw_box(st), &tmA, &full[st], it.c * 32, -(DWK / 2), (mt2 % tpf) * th - DWK / 2, mt2 / tpf);
-          tma_load_2d(dw_wts(st), &tmDW, &full[st], it.c * 32, 0);
-          if (p.dw_bias) tma_load_2d(dw_bia(st), &tmDB, &full[st], it.c * 32, 0);
-        };
-        auto prefetch_box = [&](const It& it) {  // HBM -> L2 leg of a later box, no shared memory needed
-          const int mt2 = it.t / p.num_n_tiles;
-          if (!PW_ABL(32)) tma_prefetch_4d(&tmA, it.c * 32, -(DWK / 2), (mt2 % tpf) * th - DWK / 2, mt2 / tpf);
-        };
-        It nx = {(int)blockIdx.x, 0};  // next chunk to load
-        for (int j = 0; j < 2 && nx.t < num_tiles; ++j, advance(nx)) load_box(nx, j);
-        It pf = nx;                    // next chunk to prefetch into L2 (two chunks ahead of the loads)
-        for (int j = 0; j < 2 && pf.t < num_tiles; ++j, advance(pf)) prefetch_box(pf);
-        for (int i = 0; nx.t < num_tiles; ++i, advance(nx)) {
-          mbar_wait(&box_empty[i & 1], (uint32_t)((i >> 1) & 1));  // chunk i has been read by its group
-          load_box(nx, i & 1);                                       // chunk i + 2
-          if (pf.t < num_tiles) {
-            prefetch_box(pf);                                        // chunk i + 4
-            advance(pf);
-          }
-        }
-      }
-    }
-  } else {
-    // 8 epilogue warps: two per TMEM lane quadrant, taking alternate 16-column groups.
-    // ncu showed these warps ~96 % busy on the wide layers (the kernel's critical path), so the common case
-    // (no residual) is kept lean: bias from shared memory, the finished 32 x 16 block is staged in the
-    // SWIZZLE_64B layout and handed to TMA (cp.async.bulk.tensor store), which also clips the M / N tails.
-    const int q = warp & 3;
-    const int ew = warp - 10;
-    const int hsel = ew >> 2;
-    const int etid = threadIdx.x - 320;  // 0..255 among the epilogue warps
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int buf = 0;
-    // Bias of a tile's columns lives in smem, one slot per accumulator stage.  The global load is issued one tile
-    // ahead (its L2 latency used to sit on the per-tile critical path); layers with a single N tile load it once.
-    const bool fixed_bias = p.num_n_tiles == 1;
-    auto load_bias = [&](int tile) -> float {
-      const int col = (tile % p.num_n_tiles) * p.NT + etid;
-      return (p.bias && etid < p.NT && col < p.N) ? __ldg(p.bias + col) : 0.f;
-    };
-    float bias_next = blockIdx.x < num_tiles ? load_bias(blockIdx.x) : 0.f;
-    if (fixed_bias) {
-      sbias[etid] = bias_next;
-      sbias[256 + etid] = bias_next;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int mt = t / p.num_n_tiles, nt = t - mt * p.num_n_tiles;
-      const int n0 = nt * p.NT;
-      if (!fixed_bias) {
-        sbias[acc * 256 + etid] = bias_next;
-        if (t + (int)gridDim.x < num_tiles) bias_next = load_bias(t + gridDim.x);
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // named barrier over the 8 epilogue warps
-      }
-      PWT(te1);
-      mbar_wait(&acc_full[acc], acc_phase);
-      PWT(te2);
-      PWT_ACC(18, te1, te2);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + acc * p.acc_stride + ((uint32_t)(q * 32) << 16);
-      const float* sb = sbias + acc * 256;
-      if (PW_ABL(4)) {
-      } else if (!p.R && !p.split_acc) {
-        // short-K layers (wide, epilogue-bound): 32 columns per TMEM round trip, single accumulator
-        for (int g = hsel * 32; g < p.NT; g += 64) {
-          uint32_t r32[32];
-          const bool second = g + 16 < p.NT;  // NT is a multiple of 16: the upper half may not exist
-          if (second) {
-            tmem_ld_32x32(taddr + g, r32);
-          } else {
-            uint32_t r16[16];
-            tmem_ld_32x16(taddr + g, r16);
-#pragma unroll
-            for (int e = 0; e < 16; ++e) r32[e] = r16[e];
-          }
-          tmem_ld_wait();
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            if (half == 1 && !second) break;
-            float4* stg = reinterpret_cast<float4*>(epi_stage + (ew * 2 + buf) * 2048);
-            tma_store_wait_read<1>();
-            __syncwarp();
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float4 b = *reinterpret_cast<const float4*>(sb + g + half * 16 + 4 * j);
-              float4 o = make_float4(__uint_as_float(r32[half * 16 + 4 * j]) + b.x,
-                                     __uint_as_float(r32[half * 16 + 4 * j + 1]) + b.y,
-                                     __uint_as_float(r32[half * 16 + 4 * j + 2]) + b.z,
-                                     __uint_as_float(r32[half * 16 + 4 * j + 3]) + b.w);
-              if (p.relu) {
-                o.x = fmaxf(o.x, 0.f);
-                o.y = fmaxf(o.y, 0.f);
-                o.z = fmaxf(o.z, 0.f);
-                o.w = fmaxf(o.w, 0.f);
-              }
-              stg[lane * 4 + (j ^ ((lane >> 1) & 3))] = o;
-            }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-              tma_store_2d(&tmC, stg, n0 + g + half * 16, mt * 128 + q * 32);
-              tma_store_commit();
-            }
-            buf ^= 1;
-          }
-        }
-      } else
-      for (int g = hsel * 16; g < p.NT; g += 32) {
-        uint32_t r[16], rs[16];
-        tmem_ld_32x16(taddr + g, r);
-        if (p.split_acc) {
-          tmem_ld_32x16(taddr + p.NT + g, rs);
+      constexpr int th = 128 / MW, tpf = MW / th;  // tile rows, tiles per frame
+      for (int c = 0; c < p.num_chunks; ++c) {
+        const int stage = c % S;
+        mbar_wait_backoff(&empty[stage], (uint32_t)(((c / S) & 1) ^ 1));
+        if constexpr (DWK > 0) {
+          mbar_arrive_expect_tx(&full[stage], 2 * w_bytes + p.box_bytes + DWK * DWK * 128 + (p.dw_bias ? 128 : 0));
+          tma_load_4d(dw_box(stage), &tmA, &full[stage], c * 32, -(DWK / 2), (mt % tpf) * th - DWK / 2, mt / tpf);
+          tma_load_2d(dw_wts(stage), &tmDW, &full[stage], c * 32, 0);
+          if (p.dw_bias) tma_load_2d(dw_bia(stage), &tmDB, &full[stage], c * 32, 0);
         } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) rs[e] = 0u;
+          mbar_arrive_expect_tx(&full[stage], kCorrABytes + 2 * w_bytes);
+          tma_load_2d(a_tile(stage), &tmA, &full[stage], c * 32, mt * 128);
         }
-        float4* stg = reinterpret_cast<float4*>(epi_stage + (ew * 2 + buf) * 2048);
-        if (!p.R) tma_store_wait_read<1>();  // the store issued two groups ago has finished reading this buffer
-        tmem_ld_wait();
-        if (!p.R) {
-          // ---- lean path: bias + ReLU in registers, swizzled staging, TMA store ----
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float4 b = *reinterpret_cast<const float4*>(sb + g + 4 * j);
-            float4 o = make_float4(__uint_as_float(r[4 * j]) + __uint_as_float(rs[4 * j]) + b.x,
-                                   __uint_as_float(r[4 * j + 1]) + __uint_as_float(rs[4 * j + 1]) + b.y,
-                                   __uint_as_float(r[4 * j + 2]) + __uint_as_float(rs[4 * j + 2]) + b.z,
-                                   __uint_as_float(r[4 * j + 3]) + __uint_as_float(rs[4 * j + 3]) + b.w);
-            if (p.relu) {
-              o.x = fmaxf(o.x, 0.f);
-              o.y = fmaxf(o.y, 0.f);
-              o.z = fmaxf(o.z, 0.f);
-              o.w = fmaxf(o.w, 0.f);
-            }
-            stg[lane * 4 + (j ^ ((lane >> 1) & 3))] = o;
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&tmC, stg, n0 + g, mt * 128 + q * 32);
-            tma_store_commit();
-          }
-          buf ^= 1;
-        } else {
-          // ---- residual path: transpose through smem, coalesced residual loads and stores ----
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            stg[lane * 4 + (j ^ ((lane >> 1) & 3))] =
-                make_float4(__uint_as_float(r[4 * j]) + __uint_as_float(rs[4 * j]),
-                            __uint_as_float(r[4 * j + 1]) + __uint_as_float(rs[4 * j + 1]),
-                            __uint_as_float(r[4 * j + 2]) + __uint_as_float(rs[4 * j + 2]),
-                            __uint_as_float(r[4 * j + 3]) + __uint_as_float(rs[4 * j + 3]));
-          __syncwarp();
-          const int j = lane & 3;
-          const int col = n0 + g + j * 4;
-          if (col < p.N) {
-            const float4 b = *reinterpret_cast<const float4*>(sb + g + 4 * j);
-#pragma unroll
-            for (int rb = 0; rb < 4; ++rb) {
-              const int rl = rb * 8 + (lane >> 2);
-              const long long grow = (long long)mt * 128 + q * 32 + rl;
-              if (grow < p.M) {
-                float4 o = stg[rl * 4 + (j ^ ((rl >> 1) & 3))];
-                const float4 rr = __ldg(reinterpret_cast<const float4*>(p.R + grow * p.ldr + col));
-                o.x += b.x + rr.x;
-                o.y += b.y + rr.y;
-                o.z += b.z + rr.z;
-                o.w += b.w + rr.w;
-                if (p.relu) {
-                  o.x = fmaxf(o.x, 0.f);
-                  o.y = fmaxf(o.y, 0.f);
-                  o.z = fmaxf(o.z, 0.f);
-                  o.w = fmaxf(o.w, 0.f);
-                }
-                *reinterpret_cast<float4*>(p.C + grow * p.ldc + col) = o;
-              }
-            }
-          }
-          __syncwarp();
-        }
+        tma_load_2d(w_hi(stage), &tmWh, &full[stage], c * 32, nt * NT);
+        tma_load_2d(w_lo(stage), &tmWl, &full[stage], c * 32, nt * NT);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[acc]);
-      PWT(te3);
-      PWT_ACC(19, te2, te3);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
-    if (!p.R) tma_store_wait<0>();  // all bulk stores of this warp have completed before the CTA exits
-    if (warp == 10) { PWT_FLUSH(18, 20); }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
+  const int wg = warp >> 2, r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), t = lane & 3;
+  float accm[NT / 2], accc[NT / 2];
+#pragma unroll
+  for (int i = 0; i < NT / 2; ++i) accm[i] = accc[i] = 0.f;
+  for (int c = 0; c < p.num_chunks; ++c) {
+    const int stage = c % S;
+    mbar_wait(&full[stage], (uint32_t)((c / S) & 1));
+    if constexpr (DWK > 0) {
+      // thread = (2-channel pair, 1 x 8 pixel strip); 16 strips cover the 128-pixel tile
+      constexpr int K = DWK, TX = 8, NIN = TX + K - 1, IW = MW + K - 1, PXN = MW / TX;
+      typedef unsigned long long U2;  // two packed fp32 channels
+      const int c2 = threadIdx.x & 15, pos = threadIdx.x >> 4;
+      const int x0 = (pos % PXN) * TX, y0 = pos / PXN;
+      const U2* in2 = reinterpret_cast<const U2*>(dw_box(stage)) + (y0 * IW + x0) * 16 + c2;
+      const U2* w2 = reinterpret_cast<const U2*>(dw_wts(stage)) + c2;
+      const U2 bias2 = p.dw_bias ? reinterpret_cast<const U2*>(dw_bia(stage))[c2] : 0ull;
+      U2 acc[TX];
+#pragma unroll
+      for (int i = 0; i < TX; ++i) acc[i] = bias2;
+#pragma unroll
+      for (int ky = 0; ky < K; ++ky) {
+        U2 v[NIN];
+#pragma unroll
+        for (int i = 0; i < NIN; ++i) v[i] = in2[(ky * IW + i) * 16];
+#pragma unroll
+        for (int kx = 0; kx < K; ++kx) {
+          const U2 k = w2[(ky * K + kx) * 16];
+#pragma unroll
+          for (int i = 0; i < TX; ++i) ffma2(acc[i], v[i + kx], k);
+        }
+      }
+      uint8_t* at = a_tile(stage);
+#pragma unroll
+      for (int i = 0; i < TX; ++i) {
+        float2 v = make_float2(__uint_as_float((uint32_t)acc[i]), __uint_as_float((uint32_t)(acc[i] >> 32)));
+        if (p.dw_relu) {
+          v.x = fmaxf(v.x, 0.f);
+          v.y = fmaxf(v.y, 0.f);
+        }
+        const int R = y0 * MW + x0 + i;  // A-tile row = pixel inside the tile
+        *reinterpret_cast<float2*>(at + R * 128 + (((c2 >> 1) ^ (R & 7)) << 4) + ((c2 & 1) << 3)) = v;
+      }
+      consumer_sync();  // the A tile of this chunk is complete (and every warp has left the previous chunk's)
+    }
+    uint32_t hi[4][4], lo[4][4];
+    load_a_frags(a_tile(stage), r0, t, hi, lo);
+    const uint32_t bh = smem_u32(w_hi(stage)), bl = smem_u32(w_lo(stage));
+    const int ksteps = (c == p.num_chunks - 1) ? p.last_ksteps : 4;  // K tail: skip all-zero K-steps
+    wg_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (j < ksteps) mma3<NT>(accm, accc, hi[j], lo[j], bh + j * 32, bl + j * 32);
+    wg_commit();
+    wg_wait();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);
+  }
+
+  // epilogue: (main + corr) + bias (+ residual), ReLU, 8-byte stores (4 lanes cover one 32-byte sector)
+  const int n0 = nt * NT + 2 * t;
+#pragma unroll
+  for (int hrow = 0; hrow < 2; ++hrow) {
+    const long long grow = (long long)mt * 128 + r0 + hrow * 8;
+    if (grow >= p.M) continue;
+#pragma unroll
+    for (int i = 0; i < NT / 8; ++i) {
+      const int col = n0 + 8 * i;
+      if (col >= p.N) continue;
+      float2 o = make_float2(accm[4 * i + 2 * hrow] + accc[4 * i + 2 * hrow], accm[4 * i + 2 * hrow + 1] + accc[4 * i + 2 * hrow + 1]);
+      float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+      if (p.R) {
+        const float2 rr = __ldg(reinterpret_cast<const float2*>(p.R + grow * p.ldr + col));
+        b.x += rr.x;
+        b.y += rr.y;
+      }
+      o.x += b.x;
+      o.y += b.y;
+      if (p.relu) {
+        o.x = fmaxf(o.x, 0.f);
+        o.y = fmaxf(o.y, 0.f);
+      }
+      *reinterpret_cast<float2*>(p.C + grow * p.ldc + col) = o;
+    }
   }
 }
 
 constexpr int kPwMaxSmem = 232448 - 1024;  // 227 KB opt-in limit minus static/driver slack
-constexpr int kPwTailBytes = 1024 /*barriers*/ + 8 * 2 * 2048 /*epilogue staging*/ + 2048 /*bias*/;
+constexpr int kPwMaxStages = 3;
 
-// Output-channel tile for a layer: largest divisor-style tile <= 256 that is a multiple of 16.
-// wide = single-chunk layers (K <= 32, one accumulator per stage): tiles up to 256 columns.  Those layers are
-// bound by the per-tile round trips (TMA -> split -> MMA -> epilogue), so fewer, wider tiles win.
-inline int pw_tile_n(int N, bool wide = false) {
-  // <= 128 so that 2 buffers x (main + correction) accumulators fit the 512 TMEM columns
-  const int limit = wide ? 256 : 128;
-  const int Np = (N + 15) & ~15;  // N = 24 -> 32 (weight rows >= N are zero-filled by TMA)
-  if (Np <= limit) return Np;
-  for (int parts = 2; parts <= 8; ++parts)
-    if (Np % parts == 0 && (Np / parts) % 16 == 0 && Np / parts <= limit) return Np / parts;
+// Output-channel tile for a layer: the layer is cut into the fewest tiles of <= 128 columns (two accumulators of
+// NT / 2 registers per thread), each the narrowest instantiated width that covers its share; the last tile may hang
+// over N (weight rows >= N are zero-filled by TMA, the store is clipped).
+inline int pw_tile_n(int N) {
+  const int Np = (N + 15) & ~15;
+  const int tiles = (Np + 127) / 128;
+  const int need = (Np + tiles - 1) / tiles;
+  for (int nt : {16, 32, 48, 64, 96, 112, 128})
+    if (nt >= need) return nt;
   return 0;
 }
 
-inline bool pw_supported(int cin, int cout) {
-  return available() && cin % 8 == 0 && cout % 8 == 0 && pw_tile_n(cout) != 0;
-}
+inline bool pw_supported(int cin, int cout) { return available() && cin % 8 == 0 && cout % 8 == 0; }
+
+#define FEAR_PW_FOR_NT(X) X(16) X(32) X(48) X(64) X(96) X(112) X(128)
 
 inline int init_pw() {
-  if (cudaFuncSetAttribute(pw_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(pw_tc_kernel<0, 16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(pw_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(pw_tc_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(pw_tc_kernel<3, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(pw_tc_kernel<5, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem) != cudaSuccess) {
+  cudaError_t e = cudaSuccess;
+#define FEAR_PW_ATTR(NT_)                                                                                                  \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_kernel<NT_, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem);     \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_kernel<NT_, 3, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem); \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_kernel<NT_, 5, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem); \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_kernel<NT_, 3, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem); \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_kernel<NT_, 5, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem);
+  FEAR_PW_FOR_NT(FEAR_PW_ATTR)
+#undef FEAR_PW_ATTR
+  if (e != cudaSuccess) {
     cudaGetLastError();
     return -1;
   }
@@ -1062,18 +376,8 @@ inline int init_pw() {
 }
 
 // w_hi / w_lo: tf32-split copies of the [N][K] weights (device).
-// Tile width for the tensor-memory (TS) form: the accumulators may use 384 TMEM columns (2 sets x (main + correction) x NT or
-// 2 sets x NT), i.e. NT <= 96 with split accumulators and <= 192 without; the layer is cut into the fewest such tiles, the last
-// one may hang over N (weight rows >= N are zero-filled by TMA, the store is clipped).
-inline int pw_tile_n_ts(int N, bool split_acc) {
-  const int limit = split_acc ? 96 : 192;
-  const int Np = (N + 15) & ~15;
-  const int tiles = (Np + limit - 1) / limit;
-  return (((Np + tiles - 1) / tiles) + 15) & ~15;
-}
-
 inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi, const float* w_lo, const float* bias,
-                     const float* R, int ldr, float* C, int ldc, int M, int N, int K, int relu, bool ts_form = true) {
+                     const float* R, int ldr, float* C, int ldc, int M, int N, int K, int relu) {
   if (!available()) return -20;
   PwParams p;
   p.bias = bias;
@@ -1084,59 +388,37 @@ inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi,
   p.M = M;
   p.N = N;
   p.num_chunks = (K + 31) / 32;
-  p.split_acc = p.num_chunks > 2;
-  if (ts_form) {
-    // only where the narrower TS tiles cut the layer without waste (N = 256 / 336 with split accumulators would pad to 288 /
-    // 384 columns: measured slower than the shared-memory form with NT = 128 / 112)
-    const int nt = pw_tile_n_ts(N, p.split_acc);
-    if (((N + 15) & ~15) % nt) ts_form = false;
-  }
-  p.NT = ts_form ? pw_tile_n_ts(N, p.split_acc) : pw_tile_n(N, p.num_chunks == 1);
-  if (!p.NT) return -21;
-  p.num_n_tiles = (((N + 15) & ~15) + p.NT - 1) / p.NT;
+  const int NT = pw_tile_n(N);
+  if (!NT) return -21;
+  p.num_n_tiles = (((N + 15) & ~15) + NT - 1) / NT;
   p.last_ksteps = ((K - 32 * (p.num_chunks - 1)) + 7) / 8;
-  p.acc_stride = p.split_acc ? 2 * p.NT : p.NT;
   p.relu = relu;
   p.dw_relu = p.dw_bias = p.box_bytes = 0;
-  p.map_w = 16;
-  const bool resident = p.num_n_tiles == 1 && p.num_chunks == 1;
-  p.w_region = resident ? 2 * p.NT * 128 : 0;
-  p.stage_bytes = resident ? kCorrABytes : kCorrABytes + 2 * p.NT * 128;  // landing space only
-  const int lo_bytes = ts_form ? 0 : 2 * kCorrABytes;                      // (shared-memory form: two lo tiles beside the ring)
-  p.stages = (kPwMaxSmem - 1024 - kPwTailBytes - p.w_region - lo_bytes) / p.stage_bytes;
-  if (p.stages > 8) p.stages = 8;
-  if (p.stages < 2) return -22;
-  int cols = 32;
-  while (cols < 2 * p.acc_stride) cols <<= 1;
-  p.tmem_cols = ts_form ? 512 : cols;
-  if (ts_form && 2 * p.acc_stride > kPwTsSlotCol) return -21;
+  p.stage_bytes = kCorrABytes + 2 * NT * 128;
+  p.stages = p.num_chunks < kPwMaxStages ? p.num_chunks : kPwMaxStages;
   CUtensorMap tmA, tmWh, tmWl;
   int r = make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 128, 32);
   if (r) return r;
-  r = make_tmap_2d(&tmWh, w_hi, (uint64_t)N, (uint64_t)K, (uint64_t)K, p.NT, 32);
+  r = make_tmap_2d(&tmWh, w_hi, (uint64_t)N, (uint64_t)K, (uint64_t)K, NT, 32);
   if (r) return r;
-  r = make_tmap_2d(&tmWl, w_lo, (uint64_t)N, (uint64_t)K, (uint64_t)K, p.NT, 32);
+  r = make_tmap_2d(&tmWl, w_lo, (uint64_t)N, (uint64_t)K, (uint64_t)K, NT, 32);
   if (r) return r;
   const int tiles = ((M + 127) / 128) * p.num_n_tiles;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  CUtensorMap tmC;  // output: [M][N] window of C (pitch ldc); 32 x 16 boxes, SWIZZLE_64B staging; clips the tails
-  r = make_tmap_2d(&tmC, C, (uint64_t)M, (uint64_t)N, (uint64_t)ldc, 32, 16);
-  if (r) return r;
-  const int smem_bytes = p.w_region + lo_bytes + p.stages * p.stage_bytes + 1024 + kPwTailBytes;
-#ifdef FEAR_PW_TIMING
-  p.timing_id = pw_timing_next()++;
-  pw_timing_info()[p.timing_id & 63] = {M, N, K, 0, 0, grid, tiles, p.num_chunks};
-#endif
-  const cudaError_t e =
-      ts_form ? launch_pdl(pw_tc_kernel<0, 16, true>, dim3(grid), dim3(kPwThreads), (size_t)smem_bytes, s, tmA, tmWh, tmWl, tmC, tmA,
-                           tmA, p)
-              : launch_pdl(pw_tc_kernel<0>, dim3(grid), dim3(kPwThreads), (size_t)smem_bytes, s, tmA, tmWh, tmWl, tmC, tmA, tmA, p);
-  if (e != cudaSuccess) return -23;
-  return 0;
+  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 1024 + 256;
+  cudaError_t e = cudaErrorInvalidValue;
+  switch (NT) {
+#define FEAR_PW_CASE(NT_)                                                                                                     \
+  case NT_:                                                                                                                   \
+    e = launch_pdl(pw_tc_kernel<NT_, 0>, dim3(tiles), dim3(kTcThreads), smem_bytes, s, tmA, tmWh, tmWl, tmA, tmA, p); \
+    break;
+    FEAR_PW_FOR_NT(FEAR_PW_CASE)
+#undef FEAR_PW_CASE
+  }
+  return e == cudaSuccess ? 0 : -23;
 }
 
 // Depthwise-fused GEMM (option "fuse_dwpw", default on; tests/test_gpu_parity.py): 1x1 conv whose input is dw_k x dw_k depthwise(X)
-// (+bias, ReLU), X = [B][16][16][K] channels-last, stride 1.  out = act(dw(X) * W^T + bias (+R)).
+// (+bias, ReLU), X = [B][map_w][map_w][K] channels-last, stride 1.  out = act(dw(X) * W^T + bias (+R)).
 // Returns 1 when the shape is not covered (caller runs the two kernels separately).
 inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const float* dw_w, const float* dw_b, int dw_relu,
                         const float* w_hi, const float* w_lo, const float* bias, const float* R, int ldr, float* C,
@@ -1145,7 +427,6 @@ inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const f
   if ((dw_k != 3 && dw_k != 5) || K % 4 || (map_w != 16 && map_w != 32)) return 1;
   PwParams p;
   const int M = B * map_w * map_w;
-  p.map_w = map_w;
   p.bias = bias;
   p.R = R;
   p.C = C;
@@ -1154,32 +435,25 @@ inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const f
   p.M = M;
   p.N = N;
   p.num_chunks = (K + 31) / 32;
-  p.NT = pw_tile_n(N, false);
-  if (!p.NT) return 1;
-  p.num_n_tiles = (((N + 15) & ~15) + p.NT - 1) / p.NT;
+  const int NT = pw_tile_n(N);
+  if (!NT) return 1;
+  p.num_n_tiles = (((N + 15) & ~15) + NT - 1) / NT;
   p.last_ksteps = ((K - 32 * (p.num_chunks - 1)) + 7) / 8;
-  p.split_acc = p.num_chunks > 2;
-  p.acc_stride = p.split_acc ? 2 * p.NT : p.NT;
   p.relu = relu;
   p.dw_relu = dw_relu;
   p.dw_bias = dw_b != nullptr;
   const int ih = 128 / map_w + dw_k - 1, iw = map_w + dw_k - 1;
   p.box_bytes = ih * iw * 128;
-  p.w_region = 0;
-  p.stage_bytes = (2 * kCorrABytes + 2 * p.NT * 128 + p.box_bytes + dw_k * dw_k * 128 + 128 + 1023) & ~1023;
-  p.stages = 2;  // stage s belongs to split group s
-  if (2 * p.stage_bytes + 1024 + kPwTailBytes > kPwMaxSmem) return 1;
-  int cols = 32;
-  while (cols < 2 * p.acc_stride) cols <<= 1;
-  p.tmem_cols = cols;
-  CUtensorMap tmX, tmWh, tmWl, tmC, tmDW, tmDB;
+  p.stage_bytes = (kCorrABytes + 2 * NT * 128 + p.box_bytes + dw_k * dw_k * 128 + 128 + 1023) & ~1023;
+  p.stages = p.num_chunks < 2 ? 1 : 2;
+  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 1024 + 256;
+  if ((int)smem_bytes > kPwMaxSmem) return 1;
+  CUtensorMap tmX, tmWh, tmWl, tmDW, tmDB;
   int r = make_tmap_nhwc(&tmX, X, (uint64_t)B, (uint64_t)map_w, (uint64_t)map_w, (uint64_t)K, 32, iw, ih);
   if (r) return r;
-  r = make_tmap_2d(&tmWh, w_hi, (uint64_t)N, (uint64_t)K, (uint64_t)K, p.NT, 32);
+  r = make_tmap_2d(&tmWh, w_hi, (uint64_t)N, (uint64_t)K, (uint64_t)K, NT, 32);
   if (r) return r;
-  r = make_tmap_2d(&tmWl, w_lo, (uint64_t)N, (uint64_t)K, (uint64_t)K, p.NT, 32);
-  if (r) return r;
-  r = make_tmap_2d(&tmC, C, (uint64_t)M, (uint64_t)N, (uint64_t)ldc, 32, 16);
+  r = make_tmap_2d(&tmWl, w_lo, (uint64_t)N, (uint64_t)K, (uint64_t)K, NT, 32);
   if (r) return r;
   r = make_tmap_2d_plain(&tmDW, dw_w, (uint64_t)dw_k * dw_k, (uint64_t)K, dw_k * dw_k, 32);
   if (r) return r;
@@ -1190,19 +464,24 @@ inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const f
     tmDB = tmDW;
   }
   const int tiles = (M / 128) * p.num_n_tiles;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  const size_t smem_bytes = (size_t)2 * p.stage_bytes + 1024 + kPwTailBytes;
-#ifdef FEAR_PW_TIMING
-  p.timing_id = pw_timing_next()++;
-  pw_timing_info()[p.timing_id & 63] = {M, N, K, dw_k, map_w, grid, tiles, p.num_chunks};
-#endif
-  cudaError_t e;
-  if (map_w == 16)
-    e = dw_k == 5 ? launch_pdl(pw_tc_kernel<5, 16>, dim3(grid), dim3(kPwThreads), smem_bytes, s, tmX, tmWh, tmWl, tmC, tmDW, tmDB, p)
-                  : launch_pdl(pw_tc_kernel<3, 16>, dim3(grid), dim3(kPwThreads), smem_bytes, s, tmX, tmWh, tmWl, tmC, tmDW, tmDB, p);
-  else
-    e = dw_k == 5 ? launch_pdl(pw_tc_kernel<5, 32>, dim3(grid), dim3(kPwThreads), smem_bytes, s, tmX, tmWh, tmWl, tmC, tmDW, tmDB, p)
-                  : launch_pdl(pw_tc_kernel<3, 32>, dim3(grid), dim3(kPwThreads), smem_bytes, s, tmX, tmWh, tmWl, tmC, tmDW, tmDB, p);
+  cudaError_t e = cudaErrorInvalidValue;
+#define FEAR_PW_DW_LAUNCH(NT_, K_, MW_) \
+  e = launch_pdl(pw_tc_kernel<NT_, K_, MW_>, dim3(tiles), dim3(kTcThreads), smem_bytes, s, tmX, tmWh, tmWl, tmDW, tmDB, p)
+  switch (NT) {
+#define FEAR_PW_CASE(NT_)                                \
+  case NT_:                                              \
+    if (map_w == 16) {                                   \
+      if (dw_k == 5) FEAR_PW_DW_LAUNCH(NT_, 5, 16);      \
+      else FEAR_PW_DW_LAUNCH(NT_, 3, 16);                \
+    } else {                                             \
+      if (dw_k == 5) FEAR_PW_DW_LAUNCH(NT_, 5, 32);      \
+      else FEAR_PW_DW_LAUNCH(NT_, 3, 32);                \
+    }                                                    \
+    break;
+    FEAR_PW_FOR_NT(FEAR_PW_CASE)
+#undef FEAR_PW_CASE
+  }
+#undef FEAR_PW_DW_LAUNCH
   return e == cudaSuccess ? 0 : -23;
 }
 

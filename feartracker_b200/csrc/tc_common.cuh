@@ -1,8 +1,8 @@
-// sm_100a primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma kind::tf32 / commit / ld), UMMA descriptors, tensor-map creation.
+// sm_90a primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (mma_async kind tf32 / commit / wait), shared-memory matrix descriptors, tensor-map creation.
 //
-// All inline PTX here is architecture-specific to Blackwell; the library is compiled for
-// compute_100a only.  Nothing links against libcuda: cuTensorMapEncodeTiled is resolved at run
+// All inline PTX here is architecture-specific to Hopper; the library is compiled for
+// compute_90a only.  Nothing links against libcuda: cuTensorMapEncodeTiled is resolved at run
 // time through cudaGetDriverEntryPoint so the .so still loads on a machine without a driver.
 #pragma once
 #include <cuda.h>
@@ -41,7 +41,7 @@ inline int resolve_driver() {
 }
 
 // ---- per-device library state -----------------------------------------------------------------
-// cudaFuncSetAttribute and the "is this an sm_100 with a working driver entry point" answer are PER DEVICE, so they
+// cudaFuncSetAttribute and the "is this an sm_90 with a working driver entry point" answer are PER DEVICE, so they
 // are keyed by the current device (every C entry point selects its handle's device before launching anything).
 struct DeviceState {
   bool inited = false;    // fear_init() ran for this device
@@ -293,22 +293,15 @@ __device__ __forceinline__ void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// Blackwell packed fp32 FMA (SASS FFMA2): two independent round-to-nearest FMAs on 64-bit register pairs per
-// issue slot.  A scalar 3-register FFMA issues every other cycle per SM sub-partition, so the packed form is what
-// reaches the fp32 peak; the results are bit-identical to two fmaf() calls.
+// Two independent round-to-nearest fp32 FMAs on the halves of 64-bit register pairs (the kernels keep two channels
+// per 64-bit shared-memory word); bit-identical to two fmaf() calls.
 struct __align__(16) F4 {
   unsigned long long lo, hi;  // (x, y), (z, w)
 };
-// volatile: keeps the issue order chosen below (runs of FFMA2 sharing one multiplier register, which the operand
-// reuse cache serves -- measured 67 TFLOP/s vs 31-55 TFLOP/s for FFMA2 streams with three fresh operands each).
 __device__ __forceinline__ void ffma2(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-  asm volatile("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
-}
-// packed fp32 add (two independent round-to-nearest adds per issue slot; bit-identical to two __fadd_rn)
-__device__ __forceinline__ unsigned long long fadd2(unsigned long long a, unsigned long long b) {
-  unsigned long long d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  const float x = fmaf(__uint_as_float((uint32_t)a), __uint_as_float((uint32_t)b), __uint_as_float((uint32_t)acc));
+  const float y = fmaf(__uint_as_float((uint32_t)(a >> 32)), __uint_as_float((uint32_t)(b >> 32)), __uint_as_float((uint32_t)(acc >> 32)));
+  acc = (unsigned long long)__float_as_uint(x) | ((unsigned long long)__float_as_uint(y) << 32);
 }
 __device__ __forceinline__ unsigned long long pack2(uint32_t lo, uint32_t hi) {
   return (unsigned long long)lo | ((unsigned long long)hi << 32);
@@ -324,112 +317,94 @@ __device__ __forceinline__ float4 f4_to_float4(const F4& v) {
 
 // ---- programmatic dependent launch (PDL) ---------------------------------------------------
 // A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while its predecessor in
-// the stream is still draining: its CTAs run their prologue (barrier init, TMEM allocation, descriptor prefetch)
+// the stream is still draining: its CTAs run their prologue (barrier init, descriptor prefetch)
 // on SMs the predecessor has already left, then block in pdl_wait() until the predecessor has completed and its
 // writes are visible.  pdl_trigger() lets the *next* kernel do the same with us.  Both are no-ops for a normal launch.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// ---- tcgen05 -----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// mbarrier arrives once all tcgen05 ops issued so far by this thread have completed.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, kind::tf32, single CTA.  One thread issues.
-__device__ __forceinline__ void mma_tf32_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// ---- wgmma (warpgroup MMA, tf32) ----------------------------------------------------------
+// D[64 x N] += A[64 x 8] * B[N x 8]^T with the A fragment in REGISTERS and B a shared-memory descriptor; fp32
+// accumulators in registers (thread (warp w, lane 4g + t) of the warpgroup holds rows 16w + g and 16w + g + 8,
+// columns 8i + 2t and 8i + 2t + 1 of every 8-column group i; A: a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4),
+// a3 = (g + 8, t + 4)).  Wider tiles are composed of N = 64 / 32 / 16 instructions on adjacent weight rows.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// 32 lanes x 32 consecutive columns: thread i of the warp receives columns [c, c+32) of TMEM lane
-// (quadrant base + i).  taddr = (lane << 16) | column.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
+#define FEAR_WG_D8(d, o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, const uint32_t (&a)[4], uint64_t bdesc);
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float* d, const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}\n"
+      : FEAR_WG_D8(d, 0)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
 }
-
-// 32 lanes x 16 consecutive columns.
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float* d, const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
+      : FEAR_WG_D8(d, 0), FEAR_WG_D8(d, 8)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
 }
-
-// registers -> TMEM: thread i of the warp writes 16 consecutive columns of TMEM lane (quadrant base + i).
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float* d, const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+      : FEAR_WG_D8(d, 0), FEAR_WG_D8(d, 8), FEAR_WG_D8(d, 16), FEAR_WG_D8(d, 24)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+#undef FEAR_WG_D8
 
-// D[tmem] (+)= A[tmem] * B[smem]^T, kind::tf32: the A operand (M = 128 rows = 128 TMEM lanes, one tf32
-// per 32-bit column, K = 8 columns per MMA) comes from tensor memory, B from a shared-memory descriptor.
-__device__ __forceinline__ void mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// ---- UMMA descriptors --------------------------------------------------------------------
-// Shared-memory operand, K-major, 128-byte swizzle (rows of 128 B, 8-row atoms of 1024 B, tile base
-// 1024-B aligned): start address >> 4 in bits [0,14), LBO (unused for swizzled K-major) = 1 in
-// [16,30), SBO = 1024 B >> 4 in [32,46), descriptor version 1 in [46,48), layout SWIZZLE_128B = 2 in
-// [61,64).   Advancing K by one MMA step (8 tf32 = 32 B) adds 32 B to the start address.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// Shared-memory B operand, K-major, 128-byte swizzle (rows of 128 B, 8-row atoms of 1024 B, tile base 1024-B
+// aligned): start address >> 4 in bits [0,14), LBO (unused for swizzled K-major) = 1 in [16,30), SBO = 1024 B >> 4
+// in [32,46), layout SWIZZLE_128B = 1 in [62,64).  Advancing K by one MMA step (8 tf32 = 32 B) adds 32 B to the
+// start address; advancing N by 16 rows adds 2048 B.
+__device__ __forceinline__ uint64_t wg_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor, kind::tf32: D fp32 (bits 4-5 = 1), A/B tf32 (bits 7-9, 10-12 = 2), both
-// K-major (bits 15, 16 = 0), N >> 3 at bits 17-22, M >> 4 at bits 24-28.
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// 3xTF32 product of one K step into a (main, correction) accumulator pair, NT columns wide:
+//   main += a_hi * w_hi ;  corr += a_hi * w_lo ;  corr += a_lo * w_hi          (result = main + corr)
+// bh / bl: shared-memory addresses of the K step inside the w_hi / w_lo tiles.  Every tensor-core kernel of the
+// library accumulates through this function in K order, so fused and unfused forms of a layer agree bit for bit.
+template <int NT>
+__device__ __forceinline__ void mma3(float* main, float* corr, const uint32_t (&ah)[4], const uint32_t (&al)[4],
+                                     uint32_t bh, uint32_t bl) {
+  static_assert(NT % 16 == 0 && NT <= 128, "tile width");
+  constexpr int n0 = NT >= 64 ? 64 : (NT >= 32 ? 32 : 16);
+  wgmma_tf32<n0>(main, ah, wg_desc_k_sw128(bh));
+  wgmma_tf32<n0>(corr, ah, wg_desc_k_sw128(bl));
+  wgmma_tf32<n0>(corr, al, wg_desc_k_sw128(bh));
+  if constexpr (NT > n0) mma3<NT - n0>(main + n0 / 2, corr + n0 / 2, ah, al, bh + n0 * 128, bl + n0 * 128);
+}
+
+// A fragments of one 32-channel chunk (4 K steps) for this thread's rows r0 and r0 + 8 of a [rows][32] fp32 tile in
+// the SWIZZLE_128B layout (16-byte chunk index ^ (row % 8)), split into tf32 hi (13 low mantissa bits cleared) and
+// lo = v - hi (exact in fp32; the tensor core drops lo's own low bits: |err| <= 2^-21 |v|).
+__device__ __forceinline__ void load_a_frags(const uint8_t* tile, int r0, int t, uint32_t (&hi)[4][4], uint32_t (&lo)[4][4]) {
+  const int g = r0 & 7;
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int row = r0 + (e & 1) * 8, ch = 2 * j + (e >> 1);
+      const float v = *reinterpret_cast<const float*>(tile + row * 128 + ((ch ^ g) << 4) + t * 4);
+      const uint32_t h = __float_as_uint(v) & 0xFFFFE000u;
+      hi[j][e] = h;
+      lo[j][e] = __float_as_uint(v - __uint_as_float(h));
+    }
 }
 
 // Host mirror of cvt.rna.tf32.f32 (round to nearest, ties away from zero; finite inputs).
@@ -452,8 +427,7 @@ __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
   lo = __uint_as_float(l);
 }
 
-// Truncation split: hi = v with the 13 low mantissa bits cleared (exactly what kind::tf32 reads from a raw
-// fp32 word), lo = v - hi (exact in fp32; the tensor core then drops lo's own low bits: |err| <= 2^-21 |v|).
+// Truncation split: hi = v with the 13 low mantissa bits cleared, lo = v - hi (exact in fp32; the tensor core then drops lo's own low bits: |err| <= 2^-21 |v|).
 __device__ __forceinline__ void split_tf32_trunc(float v, float& hi, float& lo) {
   hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
   lo = v - hi;

@@ -1,4 +1,4 @@
-"""FEARNet with the reference's Python API, executed by libfear_b200 (sm_100a CUDA kernels).
+"""FEARNet with the reference's Python API, executed by libfear_b200 (sm_90a CUDA kernels).
 
 Drop-in for ``model_training.model.fear_net.FEARNet`` (reference fear_net.py:14-96): same
 constructor keywords (extras swallowed by ``**kwargs`` because hydra passes every YAML key),
@@ -42,7 +42,7 @@ class _Params(nn.Module):
 
     def forward(self, *args, **kwargs):
         raise RuntimeError(
-            f"{type(self).__name__} is a parameter container of the B200 FEARNet; call FEARNet.forward / "
+            f"{type(self).__name__} is a parameter container of the H100 FEARNet; call FEARNet.forward / "
             "track / get_features (executed by libfear_b200) instead"
         )
 
@@ -464,7 +464,7 @@ class FEARNet(nn.Module):
         if self.training:
             raise RuntimeError("internal: the library path was entered in train() mode")
         if not x.is_cuda:
-            raise RuntimeError("FEARNet (B200) has no CPU path: inputs must be CUDA tensors on a B200 (sm_100)")
+            raise RuntimeError("FEARNet (H100) has no CPU path: inputs must be CUDA tensors on an H100 (sm_90)")
         x = x.detach().contiguous() if keep_dtype else self._as_input(x, x.device)
         h, lib = self._ensure_handle(x.device)
         if x.shape[0] > self._reserved:
@@ -473,7 +473,7 @@ class FEARNet(nn.Module):
 
     def _ensure_handle(self, device: torch.device):
         if device.type != "cuda":
-            raise RuntimeError("FEARNet (B200) needs a CUDA device")
+            raise RuntimeError("FEARNet (H100) needs a CUDA device")
         index = device.index if device.index is not None else torch.cuda.current_device()
         if self._handle is not None and self._handle_device == index:
             return self._handle, _lib.load()

@@ -1,4 +1,4 @@
-"""FEARTracker: stateful single-object tracker around the B200 FEARNet.
+"""FEARTracker: stateful single-object tracker around the H100 FEARNet.
 
 API mirror of reference model_training/tracker/base_tracker.py:28-124 and fear_tracker.py:13-86:
 ``FEARTracker(model, cuda_id=0, **tracking_config)``, ``initialize(image, rect)``,
@@ -59,12 +59,12 @@ class Tracker:
 
     def _device(self) -> torch.device:
         if not torch.cuda.is_available():
-            raise RuntimeError("FEARTracker (B200) needs a CUDA device: there is no CPU path")
+            raise RuntimeError("FEARTracker (H100) needs a CUDA device: there is no CPU path")
         if isinstance(self.cuda_id, int):
             return torch.device("cuda", self.cuda_id)
         dev = torch.device(self.cuda_id)  # the reference also takes device strings ("cuda:1")
         if dev.type != "cuda":
-            raise RuntimeError(f"FEARTracker (B200) needs a CUDA device, got {self.cuda_id!r}: there is no CPU path")
+            raise RuntimeError(f"FEARTracker (H100) needs a CUDA device, got {self.cuda_id!r}: there is no CPU path")
         return torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
 
     def _preprocess_image(self, image: np.ndarray, transform=None) -> torch.Tensor:

@@ -1,4 +1,4 @@
-/* fear_b200.h -- C ABI of libfear_b200.so: the B200-native (sm_100a) FEAR-XS per-frame
+/* fear_b200.h -- C ABI of libfear_b200.so: the H100-native (sm_90a) FEAR-XS per-frame
  * inference hot path (backbone -> pixel-wise correlation -> cls/reg heads -> box decode).
  *
  * The reference (PinataFarms/FEARTracker) is pure Python/PyTorch and has no FFI; these entry
@@ -45,7 +45,7 @@ extern "C" {
 #define FEAR_EINVAL (-1)    /* bad argument (shape, null pointer, alignment)            */
 #define FEAR_ESTATE (-2)    /* handle not initialised / weights not packed              */
 #define FEAR_ENOMEM (-3)    /* workspace reservation failed                             */
-#define FEAR_ENODEV (-4)    /* no sm_100 device                                         */
+#define FEAR_ENODEV (-4)    /* no sm_90 device                                          */
 
 #define FEAR_FEAT_CH 256        /* AdjustLayer output channels                          */
 #define FEAR_SCORE 16           /* score map side (256 / 16)                            */
@@ -63,7 +63,7 @@ typedef struct FearBox {
 
 typedef struct FearContext FearContext;
 
-/* Verify `device` is sm_100, initialise the library's per-device state and make it the current device
+/* Verify `device` is sm_90, initialise the library's per-device state and make it the current device
  * (like torch's .cuda(id)).  Call once per device before packing weights on it; repeated calls are cheap. */
 int fear_init(int device);
 int fear_abi_version(void);
@@ -140,7 +140,7 @@ int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoi
  * out[:, :256] = x ; out[b, 256+k, p] = sum_c z[b,c,k] * x[b,c,p].   (blocks.py:121-124)
  * Workspace-free compatibility form: a direct CUDA-core kernel on the reference layouts (one D2D copy + one launch). */
 int fear_corr_concat_f32(const float* d_z, int Bz, const float* d_x, int B, float* d_out, void* stream);
-/* Same result through the hot path's tcgen05 kernel (layout changes in the caller's scratch: d_workspace must be
+/* Same result through the hot path's wgmma kernel (layout changes in the caller's scratch: d_workspace must be
  * 1024-byte aligned and hold fear_corr_concat_workspace_bytes(B, Bz) bytes). */
 size_t fear_corr_concat_workspace_bytes(int B, int Bz);
 int fear_corr_concat_ws_f32(const float* d_z, int Bz, const float* d_x, int B, float* d_out, void* d_workspace,
@@ -154,17 +154,15 @@ int fear_corr_nhwc_f32(const float* d_zt, int Bz, float* d_cat, int B, void* str
 /* ---- introspection (tests / bench) ---------------------------------------------------*/
 /* Select a kernel implementation for a stage by name.  Returns FEAR_EINVAL for unknown names.
  * Default = best validated implementation; every alternative is parity-tested against it.
- *   "corr", "pw"   : "auto" | "ffma" | "tcgen05"                  (correlation / 1x1 convs; ffma = CUDA-core baseline)
+ *   "corr", "pw"   : "auto" | "ffma" | "wgmma"                  (correlation / 1x1 convs; ffma = CUDA-core baseline)
  *   "dw"           : "auto" | "pixel" | "strip" | "roll" | "tma"  (depthwise)
  *   "fuse_stem"    : "1" (default) stem + xif1_0 in one kernel | "0" four separate kernels
- *   "fuse_irf"     : "1" (default) xif2_0 (expand 1x1 -> depthwise 3x3 s2 -> project 1x1) in ONE tcgen05 kernel, the
+ *   "fuse_irf"     : "1" (default) xif2_0 (expand 1x1 -> depthwise 3x3 s2 -> project 1x1) in ONE wgmma kernel, the
  *                    6x expanded tensor never leaves the SM | "0" three kernels
  *   "fuse_dwpw"    : bit mask (default 15): 1 = IRF blocks on 16x16 maps, 4 = also those on 32x32 maps, 2 = head SepConvs run
  *                    their depthwise conv inside the 1x1 GEMM kernel, 8 = the expand-1 blocks (depthwise 3x3 -> 1x1 24 -> 24
  *                    -> + x) run as one CUDA-core kernel; all bit-identical to the two-kernel paths (the depthwise maps are
  *                    never written)
- *   "pw_ts"        : "1" (default) plain 1x1 GEMMs take the activation operand from tensor memory (TS-form MMA) where their
- *                    accumulators leave room for it | "0" both operands in shared memory; bit-identical
  *   "pdl"          : "1" (default) programmatic dependent launch (process-wide) */
 int fear_set_option(FearContext* h, const char* key, const char* value);
 /* Number of kernels launched by this handle since creation (for bench's gpu_launches). */

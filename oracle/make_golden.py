@@ -50,6 +50,17 @@ def main() -> None:
     all_keys = {k: [list(v.shape), str(v.dtype).replace("torch.", "")] for k, v in sd32.items()}
     with open(os.path.join(OUT, "state_dict_keys.json"), "w") as f:
         json.dump(all_keys, f, indent=0, sort_keys=True)
+    # the reference's own outputs and checkpoint bytes, for tests/test_oracle_cpu.py::test_restatement_equals_reference_source
+    h = hashlib.sha256()
+    for k in sorted(keys):
+        h.update(k.encode())
+        h.update(sd32[k].contiguous().numpy().tobytes())
+    with open(os.path.join(OUT, "reference_state_sha256.json"), "w") as f:
+        json.dump({"tensors": len(keys), "sha256": h.hexdigest()}, f)
+    zt7, xt7, _, _ = fo.synthetic_crops(2, seed=7)
+    with torch.no_grad():
+        ref7 = net((zt7, xt7))
+    np.savez_compressed(os.path.join(OUT, "reference_forward_seed7.npz"), reg=ref7[R].numpy(), cls=ref7[C].numpy())
 
     # ---- fixture 1 (C1): seed-0 randn pair ----------------------------------------------
     torch.manual_seed(0)

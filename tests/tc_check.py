@@ -1,4 +1,4 @@
-"""Stand-alone checker for the tcgen05 kernels (run in its own process: a device-side trap would
+"""Stand-alone checker for the wgmma kernels (run in its own process: a device-side trap would
 poison the CUDA context of the main pytest process).  Prints one JSON object.
 
     python tests/tc_check.py corr [B] [Bz]
@@ -148,9 +148,9 @@ def main():
     if mode == "corr":
         B = int(sys.argv[2]) if len(sys.argv) > 2 else 3
         Bz = int(sys.argv[3]) if len(sys.argv) > 3 else B
-        impl = sys.argv[4] if len(sys.argv) > 4 else "tcgen05"
+        impl = sys.argv[4] if len(sys.argv) > 4 else "wgmma"
         res["ffma"] = corr_case(lib, B, Bz, "ffma")
-        res["tcgen05"] = corr_case(lib, B, Bz, impl)
+        res["wgmma"] = corr_case(lib, B, Bz, impl)
     elif mode == "corrperf":
         res["perf"] = [corr_perf(lib, impl) for impl in sys.argv[2:]]
     elif mode == "net":

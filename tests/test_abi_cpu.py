@@ -11,7 +11,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 @pytest.fixture(scope="module")
 def lib():
-    build.build()  # cross-compiles for sm_100a without a GPU
+    build.build()  # cross-compiles for sm_90a without a GPU
     return _lib.load()
 
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Config 3 (BASELINE.json): streaming single-object tracking over the demo clip (tests/golden/test.mp4,
-661 frames 480x256, init box [163,53,45,174]) with FEARTracker on one B200; sequentially dependent frames
+661 frames 480x256, init box [163,53,45,174]) with FEARTracker on one H100; sequentially dependent frames
 (batch 1).  Prints one JSON line: frames/s incl. host crop/resize + H2D + kernels + D2H of the box record,
 the split between host pre/post-processing and the device call, and agreement with the reference trajectory.
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""B200 counterpart of the reference's demo_video.py (reference demo_video.py:14-62): track one object through a
+"""H100 counterpart of the reference's demo_video.py (reference demo_video.py:14-62): track one object through a
 video with FEARTracker and write the annotated clip.  hydra / fire / imageio are not needed: the two YAML files the
 demo composes (model/fear.yaml, tracker/siam_tracker.yaml) are read directly when a reference config tree is given,
 otherwise the same values built into feartracker_b200 are used; video IO goes through cv2.

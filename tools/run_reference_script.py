@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""Run a script written against the reference package (e.g. the reference's demo_video.py) UNMODIFIED on the B200
+"""Run a script written against the reference package (e.g. the reference's demo_video.py) UNMODIFIED on the H100
 implementation: installs feartracker_b200.compat's stand-ins for ``model_training.*`` / hydra / fire / imageio (each
 only if the real module is missing), then executes the script as ``__main__``.
 
     cd <dir containing model_training/config and the video/checkpoint paths the script expects>
-    python /root/repo/tools/run_reference_script.py <reference>/demo_video.py --output_path=/tmp/out.mp4
+    python tools/run_reference_script.py <reference>/demo_video.py --output_path=/tmp/out.mp4
 """
 import os
 import runpy
