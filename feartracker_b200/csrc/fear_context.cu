@@ -151,9 +151,10 @@ static constexpr int64_t kActD = 64 * 64 * 96;    // largest depthwise output (x
 // RAII bracket around one kernel launch: counts it and, when profiling, records events.
 struct LaunchScope {
   FearContext* c;
+  int stage;
   cudaStream_t s;
   EventPair* ev = nullptr;
-  LaunchScope(FearContext* c_, int stage, cudaStream_t s_) : c(c_), s(s_) {
+  LaunchScope(FearContext* c_, int stage_, cudaStream_t s_) : c(c_), stage(stage_), s(s_) {
     if (!c) return;
     c->launches++;
     c->stage_launches[stage]++;
@@ -162,6 +163,16 @@ struct LaunchScope {
       ev->stage = stage;
       cudaEventRecord(ev->a, s);
     }
+  }
+  // The launcher declined the shape and launched nothing (the caller falls back to other kernels, which count
+  // themselves): take the launch back, and the event slot, which is the last one handed out.
+  void cancel() {
+    if (!c) return;
+    c->launches--;
+    c->stage_launches[stage]--;
+    if (ev) c->events_used--;
+    ev = nullptr;
+    c = nullptr;
   }
   ~LaunchScope() {
     if (ev) cudaEventRecord(ev->b, s);
@@ -371,6 +382,7 @@ static int run_blocks(FearContext* c, cudaStream_t s, float* X, int B, int& h, i
       LaunchScope scope(c, ST_BACKBONE_PW, s);
       int r = tc::launch_irf_s2(s, X, Y, c->d_irf_image, B, h, w);
       if (r < 0) return set_err(FEAR_EINVAL, "fused IRF block launch failed (%d)", r);
+      if (r == 1) scope.cancel();
       if (r == 0) {
         FEAR_TRY(check_launch("tc::irf_s2_fused_kernel"));
         h /= 2;
@@ -391,6 +403,7 @@ static int run_blocks(FearContext* c, cudaStream_t s, float* X, int B, int& h, i
       memcpy(pw.b, bw.pwl.h_b, sizeof(pw.b));
       int r = tc::launch_dw3_pw24(s, X, bw.dw.w, bw.dw.b, pw, Y, B, h, w, tc::num_sms());
       if (r < 0) return set_err(FEAR_EINVAL, "fused depthwise + 24x24 block launch failed (%d)", r);
+      if (r == 1) scope.cancel();
       if (r == 0) {
         FEAR_TRY(check_launch("tc::dw3_pw24_fused_kernel"));
         float* t = X;
@@ -412,6 +425,7 @@ static int run_blocks(FearContext* c, cudaStream_t s, float* X, int B, int& h, i
       int r = tc::launch_pw_dw(s, E, B, sp.k, bw.dw.w, bw.dw.b, 1, bw.pwl.w_hi, bw.pwl.w_lo, bw.pwl.b,
                                sp.residual() ? X : nullptr, sp.cout, Y, sp.cout, sp.cout, sp.mid(), 0, h);
       if (r < 0) return set_err(FEAR_EINVAL, "fused depthwise + 1x1 launch failed (%d)", r);
+      if (r == 1) scope.cancel();
       if (r == 0) {
         FEAR_TRY(check_launch("tc::pw_tc_kernel<DWK>"));
         float* t = X;
@@ -510,6 +524,7 @@ static int launch_sepconv(FearContext* c, cudaStream_t s, const float* X, const 
     int r = tc::launch_pw_dw(s, X, B, dw.k, dw.w, dw.b, 0, pw.w_hi, pw.w_lo, pw.b, nullptr, 0, out, ldc, pw.cout, pw.cin, 1);
     if (r < 0) return set_err(FEAR_EINVAL, "fused SepConv launch failed (%d)", r);
     if (r == 0) return check_launch("tc::pw_tc_kernel<3>");
+    scope.cancel();
   }
   FEAR_TRY(launch_dw(c, ST_HEAD_DW, s, X, dw, c->hT, B, kScore, kScore, 1, false));
   return launch_pw(c, ST_HEAD_PW, s, c->hT, pw.cin, pw, nullptr, 0, out, ldc, M, 1);
@@ -1083,6 +1098,9 @@ extern "C" int fear_debug_backbone_prefix(FearContext* c, const float* d_img, in
   DeviceGuard guard(c->device);
   if (!d_img || !d_out || B < 1 || B > c->reserved || nblocks < 0 || nblocks > kNumBlocks)
     return set_err(FEAR_EINVAL, "bad argument (B must be <= reserved batch)");
+  // the workspace holds 256 x 256 frames (kActX): larger sizes would write past bufX
+  if (H % 16 || W % 16 || H < 16 || W < 16 || H > 256 || W > 256)
+    return set_err(FEAR_EINVAL, "H, W must be multiples of 16 in [16, 256] (got %dx%d)", H, W);
   cudaStream_t s = (cudaStream_t)stream;
   {
     LaunchScope scope(c, ST_STEM, s);

@@ -165,7 +165,9 @@ int fear_corr_nhwc_f32(const float* d_zt, int Bz, float* d_cat, int B, void* str
  *                    never written)
  *   "pdl"          : "1" (default) programmatic dependent launch (process-wide) */
 int fear_set_option(FearContext* h, const char* key, const char* value);
-/* Number of kernels launched by this handle since creation (for bench's gpu_launches). */
+/* Number of kernels launched by this handle since creation (for bench's gpu_launches).  A fused kernel that declines
+ * a shape launches nothing and is not counted; only the kernels that run in its place are (the same holds for the
+ * per-stage launch counts and event brackets of fear_profile / fear_stage_ms). */
 int64_t fear_launch_count(const FearContext* h);
 /* Changes whenever the handle's workspace pointers or options change (fear_reserve growth, fear_set_option):
  * a CUDA graph captured from calls on this handle is stale once the value differs from the one seen at capture. */
@@ -178,7 +180,8 @@ const char* fear_stage_name(int i);
 int fear_stage_ms(FearContext* h, int i, float* ms, int64_t* launches);
 
 /* Debug: run the stem + the first `nblocks` backbone blocks (0..16) on img (B,3,H,W) and return
- * that activation as NCHW; B must not exceed the reserved batch. */
+ * that activation as NCHW; B must not exceed the reserved batch; H, W multiples of 16 in [16, 256]
+ * (as fear_get_features). */
 int fear_debug_backbone_prefix(FearContext* h, const float* d_img, int B, int H, int W, int nblocks,
                                float* d_out, void* stream);
 /* Debug: copy a head intermediate of the last fear_head / fear_track / fear_forward call as NCHW

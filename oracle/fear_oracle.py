@@ -447,3 +447,13 @@ def synthetic_crops(batch: int, seed: int = 20260924, with_template: bool = True
         return torch.from_numpy(np.stack([normalize_image(i) for i in hwc])).permute(0, 3, 1, 2).contiguous()
 
     return (norm(zu) if with_template else None), norm(xu), zu, xu
+
+
+def shape_crops(h: int, w: int, batch: int, seed: int = 11):
+    """Seeded uniform uint8 crops of any size (H, W), ImageNet-normalised as in synthetic_crops.
+    Returns (float32 NCHW, uint8 NCHW)."""
+    g = torch.Generator().manual_seed(seed * 100003 + h * 1009 + w)
+    u = torch.randint(0, 256, (batch, 3, h, w), generator=g, dtype=torch.uint8)
+    hwc = u.permute(0, 2, 3, 1).numpy()
+    x = torch.from_numpy(np.stack([normalize_image(i) for i in hwc])).permute(0, 3, 1, 2).contiguous()
+    return x, u

@@ -13,7 +13,10 @@ What it does
      synthetic_b4.npz            C2-style uint8-derived crops (seed 20260924), 4 frames, fp64 maps
      video_teacher.npz           C3: reference trajectory (660 int boxes) + 9 teacher-forced frames
      block_stats.json            per-block activation statistics of the reference (fp32, seed0)
+     features_shapes.npz         fp32 get_features of seeded crops at sizes other than 128 / 256 (square and not)
      test.mp4                    the demo clip (data asset, MIT) so config 3 can run on the GPU box
+
+``python -m oracle.make_golden shapes`` writes features_shapes.npz alone.
 """
 import hashlib
 import json
@@ -29,11 +32,27 @@ from oracle import ref_shims
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 R, C = fo.TARGET_REGRESSION_LABEL_KEY, fo.TARGET_CLASSIFICATION_KEY
 TEACHER_FRAMES = [1, 2, 3, 11, 51, 120, 200, 400, 660]
+FEATURE_SHAPES = [(16, 16), (48, 48), (128, 256)]  # (H, W): get_features is fully convolutional
 
 
 def _eq(a: torch.Tensor, b: torch.Tensor, what: str) -> None:
     assert a.shape == b.shape and a.dtype == b.dtype, (what, a.shape, b.shape, a.dtype, b.dtype)
     assert torch.equal(a, b), f"restatement differs from reference: {what} max|d|={(a - b).abs().max().item():.3e}"
+
+
+def record_feature_shapes(net=None) -> None:
+    """The reference's fp32 FEARNet.get_features at non-default crop sizes (tests/test_oracle_cpu.py)."""
+    net = net if net is not None else ref_shims.build_reference_net()
+    sd32 = fo.load_lightning_state(ref_shims.REF_CKPT)
+    out = {}
+    for h, w in FEATURE_SHAPES:
+        x, _ = fo.shape_crops(h, w, 2)
+        with torch.no_grad():
+            ref = net.get_features(x)
+        assert ref.shape == (2, 256, h // 16, w // 16), ref.shape
+        _eq(ref, fo.get_features(sd32, x), f"get_features fp32 {h}x{w}")
+        out[f"feat_{h}x{w}"] = ref.numpy()
+    np.savez_compressed(os.path.join(OUT, "features_shapes.npz"), **out)
 
 
 def main() -> None:
@@ -61,6 +80,7 @@ def main() -> None:
     with torch.no_grad():
         ref7 = net((zt7, xt7))
     np.savez_compressed(os.path.join(OUT, "reference_forward_seed7.npz"), reg=ref7[R].numpy(), cls=ref7[C].numpy())
+    record_feature_shapes(net)
 
     # ---- fixture 1 (C1): seed-0 randn pair ----------------------------------------------
     torch.manual_seed(0)
@@ -185,4 +205,10 @@ def main() -> None:
 
 
 if __name__ == "__main__":
-    main()
+    import sys
+
+    if sys.argv[1:] == ["shapes"]:
+        torch.set_num_threads(os.cpu_count())
+        record_feature_shapes()
+    else:
+        main()

@@ -149,3 +149,15 @@ def test_restatement_equals_reference_source(state_dict):
     zt, xt, _, _ = fo.synthetic_crops(2, seed=7)
     mine = fo.forward(state_dict, zt, xt)
     assert np.array_equal(g["reg"], mine[R].numpy()) and np.array_equal(g["cls"], mine[C].numpy())
+
+
+@pytest.mark.parametrize("h,w", [(16, 16), (48, 48), (128, 256)])
+def test_features_at_other_crop_sizes_equal_reference(state_dict, h, w):
+    """get_features is fully convolutional: at a 1x1 final map (16x16), an untiled 3x3 one (48x48) and a non-square
+    crop (128x256) the fp32 oracle reproduces the reference's own output (recorded by oracle/make_golden.py) bit for
+    bit, so it can stand in for the reference when the CUDA path is checked at these sizes."""
+    want = golden("features_shapes.npz")[f"feat_{h}x{w}"]
+    x, _ = fo.shape_crops(h, w, 2)
+    mine = fo.get_features(state_dict, x)
+    assert mine.shape == (2, 256, h // 16, w // 16)
+    assert np.array_equal(want, mine.numpy()), float(np.abs(want - mine.numpy()).max())
