@@ -25,6 +25,11 @@ BOX_DTYPE = np.dtype(
 )
 assert BOX_DTYPE.itemsize == ctypes.sizeof(FearBox) == 48
 
+# FearFrame / FearTarget of the multi-target tracking loop (include/fear_b200.h)
+FRAME_DTYPE = np.dtype([("offset", "<i8"), ("H", "<i4"), ("W", "<i4")])
+TARGET_INTS = 16  # a FearTarget is 16 int32: frame, x, y, w, h, cx, cy, cw, ch, pad_r, pad_g, pad_b, 4 reserved
+assert FRAME_DTYPE.itemsize == 16
+
 _SIGNATURES = {
     # name: (restype, argtypes)
     "fear_init": (c_int, [c_int]),
@@ -45,6 +50,8 @@ _SIGNATURES = {
     "fear_get_features_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "fear_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fear_crop_resize_u8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
+    "fear_crop_targets_u8": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_workspace_bytes": (c_size_t, [c_int, c_int]),

@@ -2,6 +2,7 @@
 // See include/fear_b200.h for the contract and DESIGN.md for the data layout.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -17,6 +18,7 @@
 #include "kernels_stem_fused.cuh"
 #include "kernels_irf_fused.cuh"
 #include "kernels_dwpw_small.cuh"
+#include "kernels_track_loop.cuh"
 
 using namespace fear;
 
@@ -1035,6 +1037,34 @@ extern "C" int fear_crop_resize_u8(const uint8_t* d_frame, int H, int W, const i
   const int n = out_size * out_size;
   crop_resize_u8_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(d_frame, H, W, d_params, d_crop, out_size);
   return check_launch("crop_resize_u8_kernel");
+}
+
+// Multi-target tracking loop (kernels_track_loop.cuh): crop of every target in one launch, then the box update.
+static_assert(sizeof(FearTarget) == 64 && sizeof(FearFrame) == 16, "FearTarget / FearFrame layout is part of the ABI");
+extern "C" int fear_crop_targets_u8(const uint8_t* d_frames, const FearFrame* d_frame_table, int F, FearTarget* d_targets,
+                                    int N, double offset, int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_frames || !d_frame_table || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (N < 1 || N > 65535) return set_err(FEAR_EINVAL, "target count must be in [1, 65535] (got %d)", N);
+  if (F < 1) return set_err(FEAR_EINVAL, "frame count must be >= 1 (got %d)", F);
+  if (out_size < 1 || out_size > kTrackCropMaxSize)
+    return set_err(FEAR_EINVAL, "out_size must be in [1, %d] (got %d)", kTrackCropMaxSize, out_size);
+  if (!(offset >= 0.0) || !std::isfinite(offset))
+    return set_err(FEAR_EINVAL, "offset must be finite and >= 0 (got %g)", offset);
+  const dim3 grid((out_size + kTrackCropRows - 1) / kTrackCropRows, N);
+  crop_targets_u8_kernel<<<grid, kTrackCropThreads, 0, (cudaStream_t)stream>>>(d_frames, d_frame_table, F, d_targets,
+                                                                              offset, out_size, d_crops);
+  return check_launch("crop_targets_u8_kernel");
+}
+
+extern "C" int fear_advance_targets(const FearBox* d_boxes, const FearFrame* d_frame_table, int F, FearTarget* d_targets,
+                                    int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_frame_table || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (N < 1) return set_err(FEAR_EINVAL, "target count must be >= 1 (got %d)", N);
+  if (F < 1) return set_err(FEAR_EINVAL, "frame count must be >= 1 (got %d)", F);
+  if (instance_size < 1) return set_err(FEAR_EINVAL, "instance_size must be >= 1 (got %d)", instance_size);
+  advance_targets_kernel<<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(d_boxes, d_frame_table, F, d_targets, N,
+                                                                           instance_size);
+  return check_launch("advance_targets_kernel");
 }
 
 extern "C" int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,

@@ -18,6 +18,9 @@
  *
  *   fear_head_update      BoxTower.forward(search, kernel, update)   blocks.py:174-179
  *   fear_crop_resize_u8   get_extended_crop (crop + pad + resize)    model_training/utils/utils.py:215-253
+ *   fear_crop_targets_u8  get_extended_crop for N tracked targets (context box + resize tables on the device)
+ *   fear_advance_targets  FEARTracker.update's rescale + clamp of the decoded box, for N targets
+ *                         tracker/fear_tracker.py:63-64, base_tracker.py:83-90
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -60,6 +63,21 @@ typedef struct FearBox {
   int32_t row, col; /* argmax of sigmoid(cls), first maximum in row-major order         */
   int32_t flat;     /* row * 16 + col                                                   */
 } FearBox;
+
+/* Multi-target tracking loop (fear_crop_targets_u8 / fear_advance_targets).  Frames are HxWx3 uint8 RGB images packed
+ * into one device buffer; a frame table lists them.  Each target's tracking state lives in device memory, so a
+ * captured CUDA graph steps every target with the values of the current frame. */
+typedef struct FearFrame {
+  int64_t offset; /* byte offset of an HxWx3 uint8 frame in the packed buffer                */
+  int32_t H, W;
+} FearFrame;
+typedef struct FearTarget {      /* 64 bytes                                                         */
+  int32_t frame;                 /* index into the frame table                                       */
+  int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
+  int32_t cx, cy, cw, ch;        /* context box of the last crop (TrackingState.mapping)             */
+  int32_t pad_r, pad_g, pad_b;   /* padding colour = saturate(rint(mean colour of the init frame))   */
+  int32_t reserved[4];
+} FearTarget;
 
 typedef struct FearContext FearContext;
 
@@ -130,6 +148,28 @@ int fear_forward(FearContext* h, const float* d_template, const float* d_search,
  * cv::resize computes them (feartracker_b200.image_ops.resize_tables). */
 int fear_crop_resize_u8(const uint8_t* d_frame, int H, int W, const int32_t* d_params, uint8_t* d_crop, int out_size,
                         void* stream);
+
+/* Tracking loop of N targets on the device (FEARMultiTracker; every target behaves like its own FEARTracker).
+ * d_frames: packed uint8 frames; d_frame_table (F entries) locates them; d_targets (N) is read and updated in place.
+ * One step of the loop is  fear_crop_targets_u8 -> fear_track_u8(B = N, Bz = N) -> fear_advance_targets;  the number
+ * of launches does not depend on N.  Both calls are handle-free, never allocate and never synchronise; the
+ * arithmetic is bit-identical to the host helpers named below (feartracker_b200.image_ops).
+ *
+ * fear_crop_targets_u8: one launch for all targets.  Per target: context = context_box(bbox, offset) (float64,
+ * truncated), written back to the target's cx, cy, cw, ch; then the constant-padded, bilinearly resized crop of that
+ * context (get_extended_crop, as fear_crop_resize_u8, with the cv::resize tables of resize_tables built on the device)
+ * into d_crops (N, out_size, out_size, 3) uint8.  Search crops: offset = search_context, out_size 256; template crops:
+ * offset = template_bbox_offset, out_size 128.  A target whose frame index is outside [0, F) gets a crop of its
+ * padding colour and no frame is read.  FEAR_EINVAL: a null pointer, N < 1 or N > 65535, F < 1, out_size outside
+ * [1, 256], offset negative or not finite. */
+int fear_crop_targets_u8(const uint8_t* d_frames, const FearFrame* d_frame_table, int F, FearTarget* d_targets, int N,
+                         double offset, int out_size, uint8_t* d_crops, void* stream);
+/* fear_advance_targets: d_boxes (N) are the decoded boxes of the targets' search crops.  Each target's box becomes
+ * clamp_bbox(rescale_bbox(box, context, instance_size), its frame's H, W): float64 multiply then add (no FMA),
+ * round half to even, sides >= 3 and the trim / minimum-side rules of clamp_bbox.  A target whose frame index is
+ * outside [0, F) keeps its box.  FEAR_EINVAL: a null pointer, N < 1, F < 1, instance_size < 1. */
+int fear_advance_targets(const FearBox* d_boxes, const FearFrame* d_frame_table, int F, FearTarget* d_targets, int N,
+                         int instance_size, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)). */
