@@ -29,6 +29,10 @@ assert BOX_DTYPE.itemsize == ctypes.sizeof(FearBox) == 48
 FRAME_DTYPE = np.dtype([("offset", "<i8"), ("H", "<i4"), ("W", "<i4")])
 TARGET_INTS = 16  # a FearTarget is 16 int32: frame, x, y, w, h, cx, cy, cw, ch, pad_r, pad_g, pad_b, 4 reserved
 assert FRAME_DTYPE.itemsize == 16
+# FearFrameView: a frame anywhere in device memory, with byte strides (include/fear_b200.h)
+VIEW_DTYPE = np.dtype([("data", "<u8"), ("row_stride", "<i8"), ("pixel_stride", "<i8"), ("channel_stride", "<i8"),
+                       ("H", "<i4"), ("W", "<i4")])
+assert VIEW_DTYPE.itemsize == 40
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -52,6 +56,9 @@ _SIGNATURES = {
     "fear_crop_resize_u8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "fear_crop_targets_u8": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_crop_targets_view_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_view": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_workspace_bytes": (c_size_t, [c_int, c_int]),

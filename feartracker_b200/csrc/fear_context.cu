@@ -1041,30 +1041,81 @@ extern "C" int fear_crop_resize_u8(const uint8_t* d_frame, int H, int W, const i
 
 // Multi-target tracking loop (kernels_track_loop.cuh): crop of every target in one launch, then the box update.
 static_assert(sizeof(FearTarget) == 64 && sizeof(FearFrame) == 16, "FearTarget / FearFrame layout is part of the ABI");
-extern "C" int fear_crop_targets_u8(const uint8_t* d_frames, const FearFrame* d_frame_table, int F, FearTarget* d_targets,
-                                    int N, double offset, int out_size, uint8_t* d_crops, void* stream) {
-  if (!d_frames || !d_frame_table || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+static_assert(sizeof(FearFrameView) == 40, "FearFrameView layout is part of the ABI");
+
+static int check_crop_targets_args(int F, int N, double offset, int out_size) {
   if (N < 1 || N > 65535) return set_err(FEAR_EINVAL, "target count must be in [1, 65535] (got %d)", N);
   if (F < 1) return set_err(FEAR_EINVAL, "frame count must be >= 1 (got %d)", F);
   if (out_size < 1 || out_size > kTrackCropMaxSize)
     return set_err(FEAR_EINVAL, "out_size must be in [1, %d] (got %d)", kTrackCropMaxSize, out_size);
   if (!(offset >= 0.0) || !std::isfinite(offset))
     return set_err(FEAR_EINVAL, "offset must be finite and >= 0 (got %g)", offset);
+  return 0;
+}
+
+static int check_advance_targets_args(int F, int N, int instance_size) {
+  if (N < 1) return set_err(FEAR_EINVAL, "target count must be >= 1 (got %d)", N);
+  if (F < 1) return set_err(FEAR_EINVAL, "frame count must be >= 1 (got %d)", F);
+  if (instance_size < 1) return set_err(FEAR_EINVAL, "instance_size must be >= 1 (got %d)", instance_size);
+  return 0;
+}
+
+template <class Frames>
+static int launch_crop_targets(Frames frames, int F, FearTarget* d_targets, int N, double offset, int out_size,
+                               uint8_t* d_crops, void* stream) {
   const dim3 grid((out_size + kTrackCropRows - 1) / kTrackCropRows, N);
-  crop_targets_u8_kernel<<<grid, kTrackCropThreads, 0, (cudaStream_t)stream>>>(d_frames, d_frame_table, F, d_targets,
-                                                                              offset, out_size, d_crops);
+  crop_targets_u8_kernel<<<grid, kTrackCropThreads, 0, (cudaStream_t)stream>>>(frames, F, d_targets, offset, out_size,
+                                                                              d_crops);
   return check_launch("crop_targets_u8_kernel");
+}
+
+template <class Frames>
+static int launch_advance_targets(const FearBox* d_boxes, Frames frames, int F, FearTarget* d_targets, int N,
+                                  int instance_size, void* stream) {
+  advance_targets_kernel<<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(d_boxes, frames, F, d_targets, N,
+                                                                           instance_size);
+  return check_launch("advance_targets_kernel");
+}
+
+extern "C" int fear_crop_targets_u8(const uint8_t* d_frames, const FearFrame* d_frame_table, int F, FearTarget* d_targets,
+                                    int N, double offset, int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_frames || !d_frame_table || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(PackedFrames{d_frames, d_frame_table}, F, d_targets, N, offset, out_size, d_crops, stream);
+}
+
+extern "C" int fear_crop_targets_view_u8(const FearFrameView* d_views, int F, FearTarget* d_targets, int N,
+                                         double offset, int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_views || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(FrameViews{d_views}, F, d_targets, N, offset, out_size, d_crops, stream);
 }
 
 extern "C" int fear_advance_targets(const FearBox* d_boxes, const FearFrame* d_frame_table, int F, FearTarget* d_targets,
                                     int N, int instance_size, void* stream) {
   if (!d_boxes || !d_frame_table || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
-  if (N < 1) return set_err(FEAR_EINVAL, "target count must be >= 1 (got %d)", N);
-  if (F < 1) return set_err(FEAR_EINVAL, "frame count must be >= 1 (got %d)", F);
-  if (instance_size < 1) return set_err(FEAR_EINVAL, "instance_size must be >= 1 (got %d)", instance_size);
-  advance_targets_kernel<<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(d_boxes, d_frame_table, F, d_targets, N,
-                                                                           instance_size);
-  return check_launch("advance_targets_kernel");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  // the advance kernel reads only H and W: any non-null base keeps a frame from looking empty (a null one would make
+  // the frame at offset 0 empty)
+  const PackedFrames frames{reinterpret_cast<const uint8_t*>(d_frame_table), d_frame_table};
+  return launch_advance_targets(d_boxes, frames, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_advance_targets_view(const FearBox* d_boxes, const FearFrameView* d_views, int F,
+                                         FearTarget* d_targets, int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_views || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return launch_advance_targets(d_boxes, FrameViews{d_views}, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_frame_sums_u8(const FearFrameView* d_views, int F, uint64_t* d_sums, void* stream) {
+  if (!d_views || !d_sums) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (F < 1 || F > 65535) return set_err(FEAR_EINVAL, "frame count must be in [1, 65535] (got %d)", F);
+  const cudaError_t e = cudaMemsetAsync(d_sums, 0, sizeof(uint64_t) * 3 * F, (cudaStream_t)stream);
+  if (e != cudaSuccess) return set_err((int)e, "zeroing the frame sums failed: %s", cudaGetErrorString(e));
+  frame_sums_u8_kernel<<<dim3(kFrameSumCtas, F), kFrameSumThreads, 0, (cudaStream_t)stream>>>(
+      FrameViews{d_views}, reinterpret_cast<unsigned long long*>(d_sums));
+  return check_launch("frame_sums_u8_kernel");
 }
 
 extern "C" int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,

@@ -5,16 +5,23 @@
     out = trk.update(frames)                      # {"bbox": (N,4) int64, "score": (N,) float32, "ids": (N,) int64}
     trk.remove(ids); trk.reset()
 
+Frames are numpy arrays in host memory or uint8 (H, W, 3) CUDA tensors already on the tracker's device, strided views
+included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y0:y1, x0:x1]); tensors are read where
+they are, without a copy.
+
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
 features of its 128 x 128 context crop, and each frame runs crop -> network -> decode -> rescale -> clamp.  Instead of
 one batch-1 step and one host round trip per target, one step runs all N targets at batch N:
 
-    fear_crop_targets_u8 (N search crops)  ->  fear_track_u8 (B = N, Bz = N)  ->  fear_advance_targets
+    fear_crop_targets_view_u8 (N search crops)  ->  fear_track_u8 (B = N, Bz = N)  ->  fear_advance_targets_view
 
 on per-target state kept in device memory (an (N, 16) int32 tensor of FearTarget records, include/fear_b200.h), so the
-step is captured once as a CUDA graph and replayed every frame; the host packs the frames into one pinned buffer, sends
-them with one copy and reads back the boxes and scores.  The launch count of a step does not depend on N.
+step is captured once as a CUDA graph and replayed every frame.  The kernels find the frames through a table of
+FearFrameView records (address, byte strides, H, W) in a fixed device buffer, written before every step: numpy frames
+are packed into one pinned buffer and sent with one copy, and their views point into the packed device buffer; CUDA
+tensors' views point at the tensors.  The host then reads back the boxes and scores.  The launch count of a step
+depends neither on N nor on the kind of frames.
 """
 import math
 import warnings
@@ -26,6 +33,14 @@ import torch
 from . import _lib, image_ops
 
 _FRAME_ALIGN = 16  # byte alignment of each frame inside the packed buffer
+_MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView
+
+
+def frame_view(frame: torch.Tensor) -> tuple:
+    """The FearFrameView record (data, row_stride, pixel_stride, channel_stride, H, W) of a uint8 (H, W, 3) tensor, as
+    it lies in memory: the address of pixel (0, 0) channel R and the byte strides (a uint8 stride is a byte stride)."""
+    rs, ps, cs = frame.stride()
+    return (frame.data_ptr(), rs, ps, cs, frame.shape[0], frame.shape[1])
 
 
 class FEARMultiTracker:
@@ -49,8 +64,7 @@ class FEARMultiTracker:
         self.max_targets = int(max_targets)
         self.net.reserve(self.max_targets)  # the whole batch fits the workspace: graph capture never allocates
         self._buf = None  # device buffers, allocated on first use
-        self._frames_key = None  # frame shapes the packed buffer and the frame table are laid out for
-        self._epoch = 0  # bumped whenever the packed frame buffer or the frame table moves
+        self._frames_key = None  # numpy frame shapes the packed buffer is laid out for
         self._graph = None
         self._graph_key = None
         self._graph_gen = None
@@ -78,8 +92,11 @@ class FEARMultiTracker:
 
     def add(self, frames, rects, streams: Optional[Sequence[int]] = None) -> np.ndarray:
         """Start tracking ``rects`` ((n, 4) [x, y, w, h]); target i lives in stream ``streams[i]`` (default 0), whose
-        current frame is ``frames[streams[i]]``.  Returns the new targets' ids."""
-        frames = self._check_frames(frames)
+        current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
+
+        ``frames`` are all numpy arrays or all CUDA tensors (see ``update``).  A target's padding colour is the mean
+        colour of its frame, from exact per-channel sums computed on the device."""
+        frames, on_device = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
         if rects.ndim == 1 and rects.size == 4:
             rects = rects[None]
@@ -93,34 +110,40 @@ class FEARMultiTracker:
             return np.zeros(0, dtype=np.int64)
         cfg = self.tracking_config
         recs = np.zeros((n, _lib.TARGET_INTS), dtype=np.int32)
-        pads = {}
         for i, (rect, s) in enumerate(zip(rects, streams)):
-            frame = frames[s]
-            box = image_ops.clamp_bbox(rect, frame.shape)
+            box = image_ops.clamp_bbox(rect, tuple(frames[s].shape))
             ctx = image_ops.context_box(box, cfg["template_bbox_offset"])
             inner = image_ops.trim_box([box[0] - ctx[0], box[1] - ctx[1], box[2], box[3]], (ctx[3], ctx[2]))
             if inner[2] * inner[3] == 0:
                 raise IndexError("target box has zero area inside its context crop")
-            if s not in pads:  # cv::saturate_cast of the float64 mean colour, as FEARTracker's padding
-                pads[s] = np.clip(np.rint(np.mean(frame, axis=(0, 1))), 0, 255).astype(np.int32)
             recs[i, 0] = s
             recs[i, 1:5] = box
-            recs[i, 9:12] = pads[s]
         dev = self._device()
         with torch.cuda.device(dev):
             b = self._buffers(dev)
-            self._upload_frames(frames, dev)
+            num_frames = len(frames)
+            self._upload_frames(frames, on_device, dev)
             lib = _lib.load()
-            n0 = len(self._ids)
             stream = torch.cuda.current_stream(dev)
+            _lib.check(lib.fear_frame_sums_u8(b["views"].data_ptr(), num_frames, b["sums"].data_ptr(),
+                                              stream.cuda_stream), "fear_frame_sums_u8")
+            b["sums_pin"][:num_frames].copy_(b["sums"][:num_frames], non_blocking=True)
+            stream.synchronize()
+            # numpy's mean of uint8 is an exact float64 sum of integers over H * W; then cv::saturate_cast, as
+            # FEARTracker's padding
+            sums = b["sums_pin"].numpy()[:num_frames].view(np.uint64)
+            pixels = np.array([f.shape[0] * f.shape[1] for f in frames], dtype=np.float64)
+            pads = np.clip(np.rint(sums / pixels[:, None]), 0, 255).astype(np.int32)
+            recs[:, 9:12] = pads[streams]
+            n0 = len(self._ids)
             b["state"][n0:n0 + n].copy_(torch.from_numpy(recs).pin_memory(), non_blocking=True)
             size = int(cfg["template_size"])
             crops = b["tcrops"][:n]
-            _lib.check(lib.fear_crop_targets_u8(b["frames"].data_ptr(), b["table"].data_ptr(), len(frames),
-                                                b["state"][n0].data_ptr(), n, float(cfg["template_bbox_offset"]),
-                                                size, crops.data_ptr(), stream.cuda_stream), "fear_crop_targets_u8")
+            _lib.check(lib.fear_crop_targets_view_u8(b["views"].data_ptr(), num_frames, b["state"][n0].data_ptr(), n,
+                                                     float(cfg["template_bbox_offset"]), size, crops.data_ptr(),
+                                                     stream.cuda_stream), "fear_crop_targets_view_u8")
             b["zf"][n0:n0 + n].copy_(self.net.get_features(crops))
-            stream.synchronize()  # the pinned staging buffer is reused by the next call
+            stream.synchronize()  # the pinned staging buffers are reused by the next call
         new_ids = np.arange(self._next_id, self._next_id + n, dtype=np.int64)
         self._next_id += n
         self._ids = np.concatenate([self._ids, new_ids])
@@ -142,8 +165,15 @@ class FEARMultiTracker:
         self._ids, self._streams = self._ids[keep], self._streams[keep]
 
     def update(self, frames) -> Dict[str, np.ndarray]:
-        """One frame of every stream -> the new box and score of every target, in the order of ``ids``."""
-        frames = self._check_frames(frames)
+        """One frame of every stream -> the new box and score of every target, in the order of ``ids``.
+
+        ``frames`` (one frame or a list of F, stream i's frame at index i) are either all ``np.ndarray`` or all
+        ``torch.Tensor``; the kind may change from one call to the next.  A tensor frame is uint8 of shape (H, W, 3)
+        on the tracker's CUDA device, with any non-negative strides: views are read as they are, nothing is copied.
+        Tensor frames must be ready on the current CUDA stream (write them on that stream, or make it wait for the
+        stream that did, as for any torch op).  ``update`` synchronises that stream before it returns, so the tensors
+        only need to live until the call returns."""
+        frames, on_device = self._check_frames(frames)
         n = len(self._ids)
         if n and int(self._streams.max()) >= len(frames):
             raise ValueError(f"targets track stream {int(self._streams.max())} but only {len(frames)} frames were given")
@@ -153,7 +183,7 @@ class FEARMultiTracker:
         dev = self._device()
         with torch.cuda.device(dev):
             b = self._buffers(dev)
-            self._upload_frames(frames, dev)
+            self._upload_frames(frames, on_device, dev)
             boxes = self._run_step(n, len(frames), dev)
             b["state_pin"][:n].copy_(b["state"][:n], non_blocking=True)
             b["box_pin"][:n].copy_(boxes, non_blocking=True)
@@ -173,19 +203,37 @@ class FEARMultiTracker:
             raise RuntimeError(f"FEARMultiTracker (H100) needs a CUDA device, got {self.cuda_id!r}: there is no CPU path")
         return torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
 
-    @staticmethod
-    def _check_frames(frames):
-        if isinstance(frames, np.ndarray) and frames.ndim == 3:
+    def _check_frames(self, frames):
+        """-> (list of frames, True if they are CUDA tensors).  Raises ValueError before any device call."""
+        if isinstance(frames, (np.ndarray, torch.Tensor)) and frames.ndim == 3:
             frames = [frames]
         frames = list(frames)
         if not frames:
             raise ValueError("no frames given")
+        on_device = isinstance(frames[0], torch.Tensor)
+        if any(isinstance(f, torch.Tensor) != on_device for f in frames):
+            raise ValueError("frames of one call must be all numpy arrays or all CUDA tensors, not a mix")
         for i, f in enumerate(frames):
-            if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
+            if on_device:
+                self._check_tensor_frame(i, f)
+            elif not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
                     or f.shape[0] < 1 or f.shape[1] < 1:
                 what = f"{f.dtype} {f.shape}" if isinstance(f, np.ndarray) else type(f).__name__
                 raise ValueError(f"frame {i} must be a uint8 HxWx3 RGB array, got {what}")
-        return frames
+        return frames, on_device
+
+    def _check_tensor_frame(self, i: int, f: torch.Tensor) -> None:
+        if f.dtype != torch.uint8 or f.ndim != 3 or f.shape[2] != 3 or not (1 <= f.shape[0] <= _MAX_SIDE) \
+                or not (1 <= f.shape[1] <= _MAX_SIDE):
+            raise ValueError(f"frame {i} must be a uint8 HxWx3 RGB tensor, got {f.dtype} {tuple(f.shape)}")
+        if min(f.stride()) < 0:
+            raise ValueError(f"frame {i} has a negative stride {f.stride()}")
+        if f.device.type != "cuda":
+            raise ValueError(f"frame {i} is a {f.device} tensor: tensor frames must be on the tracker's CUDA device "
+                             "(pass host frames as numpy arrays)")
+        dev = self._device()
+        if f.device != dev:
+            raise ValueError(f"frame {i} is on {f.device}, the tracker on {dev}")
 
     @staticmethod
     def _check_streams(streams, n: int, num_frames: int) -> np.ndarray:
@@ -213,54 +261,66 @@ class FEARMultiTracker:
             tcrops=torch.empty((m, tsize, tsize, 3), dtype=torch.uint8, device=dev),
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
-            frames_pin=None, frames=None, table=None)
+            frames_pin=None, frames=None, views_pin=None, views=None, sums_pin=None, sums=None)
         return b
 
-    def _upload_frames(self, frames, dev: torch.device) -> None:
-        """Pack the frames into the pinned staging buffer and send them with one host-to-device copy.  The buffer and
-        the frame table are laid out again only when the frame shapes change."""
-        b = self._buf
-        key = tuple(f.shape for f in frames)
-        if key != self._frames_key:
-            table = np.zeros(len(frames), dtype=_lib.FRAME_DTYPE)
-            off = 0
+    def _upload_frames(self, frames, on_device: bool, dev: torch.device) -> None:
+        """Write the FearFrameView table of ``frames`` into the device table the kernels read.  Numpy frames are packed
+        into the pinned staging buffer first and sent with one host-to-device copy (the packed layout is recomputed
+        only when their shapes change); CUDA tensors are used where they are."""
+        b, num_frames, rec = self._buf, len(frames), _lib.VIEW_DTYPE.itemsize
+        if b["views"] is None or b["views"].numel() < num_frames * rec:  # grows only: the step graph keys on it
+            b["views_pin"] = torch.empty(num_frames * rec, dtype=torch.uint8).pin_memory()
+            b["views"] = torch.empty(num_frames * rec, dtype=torch.uint8, device=dev)
+            # fear_frame_sums_u8 writes uint64; int64 storage, read back as uint64
+            b["sums_pin"] = torch.empty((num_frames, 3), dtype=torch.int64).pin_memory()
+            b["sums"] = torch.empty((num_frames, 3), dtype=torch.int64, device=dev)
+        table = b["views_pin"].numpy()[:num_frames * rec].view(_lib.VIEW_DTYPE)
+        if on_device:
             for i, f in enumerate(frames):
-                table[i] = (off, f.shape[0], f.shape[1])
-                off += -(-f.size // _FRAME_ALIGN) * _FRAME_ALIGN
-            if b["frames"] is None or b["frames"].numel() < off:
-                b["frames_pin"] = torch.empty(off, dtype=torch.uint8).pin_memory()
-                b["frames"] = torch.empty(off, dtype=torch.uint8, device=dev)
-            b["table"] = torch.from_numpy(table.view(np.uint8).copy()).to(dev)
-            b["offsets"] = [int(o) for o in table["offset"]]
-            b["nbytes"] = off
-            self._frames_key = key
-            self._epoch += 1
-        pin = b["frames_pin"].numpy()
-        for f, o in zip(frames, b["offsets"]):
-            np.copyto(pin[o:o + f.size].reshape(f.shape), f)
-        nb = b["nbytes"]
-        b["frames"][:nb].copy_(b["frames_pin"][:nb], non_blocking=True)
+                table[i] = frame_view(f)
+        else:
+            key = tuple(f.shape for f in frames)
+            if key != self._frames_key:
+                offsets, off = [], 0
+                for f in frames:
+                    offsets.append(off)
+                    off += -(-f.size // _FRAME_ALIGN) * _FRAME_ALIGN
+                if b["frames"] is None or b["frames"].numel() < off:
+                    b["frames_pin"] = torch.empty(off, dtype=torch.uint8).pin_memory()
+                    b["frames"] = torch.empty(off, dtype=torch.uint8, device=dev)
+                b["offsets"], b["nbytes"] = offsets, off
+                self._frames_key = key
+            pin, base = b["frames_pin"].numpy(), b["frames"].data_ptr()
+            for i, (f, o) in enumerate(zip(frames, b["offsets"])):
+                np.copyto(pin[o:o + f.size].reshape(f.shape), f)
+                h, w = f.shape[:2]
+                table[i] = (base + o, 3 * w, 3, 1, h, w)
+            nb = b["nbytes"]
+            b["frames"][:nb].copy_(b["frames_pin"][:nb], non_blocking=True)
+        b["views"][:num_frames * rec].copy_(b["views_pin"][:num_frames * rec], non_blocking=True)
 
     def _step(self, n: int, num_frames: int, dev: torch.device) -> torch.Tensor:
         b, cfg, lib = self._buf, self.tracking_config, _lib.load()
         size = int(cfg["instance_size"])
         s = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.fear_crop_targets_u8(b["frames"].data_ptr(), b["table"].data_ptr(), num_frames,
-                                            b["state"].data_ptr(), n, float(cfg["search_context"]), size,
-                                            b["crops"].data_ptr(), s), "fear_crop_targets_u8")
+        _lib.check(lib.fear_crop_targets_view_u8(b["views"].data_ptr(), num_frames, b["state"].data_ptr(), n,
+                                                 float(cfg["search_context"]), size, b["crops"].data_ptr(), s),
+                   "fear_crop_targets_view_u8")
         boxes = self.net.track_boxes(b["crops"][:n], b["zf"][:n])
-        _lib.check(lib.fear_advance_targets(boxes.data_ptr(), b["table"].data_ptr(), num_frames, b["state"].data_ptr(),
-                                            n, size, s), "fear_advance_targets")
+        _lib.check(lib.fear_advance_targets_view(boxes.data_ptr(), b["views"].data_ptr(), num_frames,
+                                                 b["state"].data_ptr(), n, size, s), "fear_advance_targets_view")
         return boxes
 
     def _run_step(self, n: int, num_frames: int, dev: torch.device) -> torch.Tensor:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
-        graph is keyed by the target count, the frame layout and the net's generation; ``cuda_graph=False`` in the
-        tracking config keeps eager launches."""
-        key = (n, self._frames_key, self._epoch)
+        kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
+        keyed by the target count, the frame count, the table buffer and the net's generation.  ``cuda_graph=False``
+        in the tracking config keeps eager launches."""
+        key = (n, num_frames, self._buf["views"].data_ptr())
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):
-            # new target set or frame layout, or the net's workspace / weights / options changed: the pointers and
-            # sizes baked into the captured graph are stale -> warm up eagerly and capture again
+            # new target or frame count, a new table buffer, or the net's workspace / weights / options changed: the
+            # pointers and sizes baked into the captured graph are stale -> warm up eagerly and capture again
             self._graph, self._graph_key, self._calls = None, key, 0
         use_graph = self.tracking_config.get("cuda_graph", True) and self._graph_ok
         if use_graph and self._graph is None and self._calls >= 1:

@@ -21,6 +21,9 @@
  *   fear_crop_targets_u8  get_extended_crop for N tracked targets (context box + resize tables on the device)
  *   fear_advance_targets  FEARTracker.update's rescale + clamp of the decoded box, for N targets
  *                         tracker/fear_tracker.py:63-64, base_tracker.py:83-90
+ *   fear_crop_targets_view_u8 / fear_advance_targets_view   the same on frames located by FearFrameView (strided,
+ *                         anywhere in device memory)
+ *   fear_frame_sums_u8    np.mean(frame, axis=(0, 1)) of get_extended_crop's padding, as exact integer sums
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -71,6 +74,16 @@ typedef struct FearFrame {
   int64_t offset; /* byte offset of an HxWx3 uint8 frame in the packed buffer                */
   int32_t H, W;
 } FearFrame;
+/* A frame wherever it lives in device memory (FEARMultiTracker's frames, packed or the caller's own tensors): 40 bytes.
+ * Pixel (y, x) channel c (R, G, B) is data[y * row_stride + x * pixel_stride + c * channel_stride]; strides in bytes,
+ * >= 0.  A packed HxWx3 frame at byte `offset` of a buffer is {base + offset, 3W, 3, 1, H, W}; an RGB view of an RGBA
+ * surface has pixel_stride 4, a CHW tensor seen as HWC has (W, 1, H * W).  An entry with data == NULL, H < 1 or W < 1
+ * is treated like a frame index outside [0, F). */
+typedef struct FearFrameView {
+  const uint8_t* data;                              /* device address of pixel (0, 0), channel R        */
+  int64_t row_stride, pixel_stride, channel_stride; /* bytes, >= 0                                       */
+  int32_t H, W;
+} FearFrameView;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -159,17 +172,33 @@ int fear_crop_resize_u8(const uint8_t* d_frame, int H, int W, const int32_t* d_p
  * truncated), written back to the target's cx, cy, cw, ch; then the constant-padded, bilinearly resized crop of that
  * context (get_extended_crop, as fear_crop_resize_u8, with the cv::resize tables of resize_tables built on the device)
  * into d_crops (N, out_size, out_size, 3) uint8.  Search crops: offset = search_context, out_size 256; template crops:
- * offset = template_bbox_offset, out_size 128.  A target whose frame index is outside [0, F) gets a crop of its
- * padding colour and no frame is read.  FEAR_EINVAL: a null pointer, N < 1 or N > 65535, F < 1, out_size outside
- * [1, 256], offset negative or not finite. */
+ * offset = template_bbox_offset, out_size 128.  A target whose frame index is outside [0, F), or whose frame has H < 1
+ * or W < 1, gets a crop of its padding colour and no frame is read.  FEAR_EINVAL: a null pointer, N < 1 or N > 65535,
+ * F < 1, out_size outside [1, 256], offset negative or not finite. */
 int fear_crop_targets_u8(const uint8_t* d_frames, const FearFrame* d_frame_table, int F, FearTarget* d_targets, int N,
                          double offset, int out_size, uint8_t* d_crops, void* stream);
 /* fear_advance_targets: d_boxes (N) are the decoded boxes of the targets' search crops.  Each target's box becomes
  * clamp_bbox(rescale_bbox(box, context, instance_size), its frame's H, W): float64 multiply then add (no FMA),
  * round half to even, sides >= 3 and the trim / minimum-side rules of clamp_bbox.  A target whose frame index is
- * outside [0, F) keeps its box.  FEAR_EINVAL: a null pointer, N < 1, F < 1, instance_size < 1. */
+ * outside [0, F), or whose frame has H < 1 or W < 1, keeps its box.  FEAR_EINVAL: a null pointer, N < 1, F < 1,
+ * instance_size < 1. */
 int fear_advance_targets(const FearBox* d_boxes, const FearFrame* d_frame_table, int F, FearTarget* d_targets, int N,
                          int instance_size, void* stream);
+
+/* The same pair with frames located through d_views (F FearFrameView entries in device memory) instead of a packed
+ * buffer and FearFrame table, so frames can stay where a decoder or a CUDA pre-processing step left them (strided views
+ * included).  Same semantics, arithmetic and FEAR_EINVAL rules as fear_crop_targets_u8 / fear_advance_targets; the
+ * views are read when the kernels run, so a captured graph does not depend on frame addresses or shapes.  A target
+ * whose view has data == NULL, H < 1 or W < 1 gets a padding-colour crop and keeps its box. */
+int fear_crop_targets_view_u8(const FearFrameView* d_views, int F, FearTarget* d_targets, int N, double offset,
+                              int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_view(const FearBox* d_boxes, const FearFrameView* d_views, int F, FearTarget* d_targets, int N,
+                              int instance_size, void* stream);
+/* Exact per-channel sums of F frames: d_sums (F, 3) uint64 = sum over all H * W pixels of channel R, G, B (0 for an
+ * entry with data == NULL, H < 1 or W < 1).  sums / (H * W) in float64 is numpy's mean of the uint8 frame bit for bit
+ * (the padding colour of a new target).  Zeroes d_sums with cudaMemsetAsync, then one launch.  FEAR_EINVAL: a null
+ * pointer, F < 1 or F > 65535. */
+int fear_frame_sums_u8(const FearFrameView* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)). */
