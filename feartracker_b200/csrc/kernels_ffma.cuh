@@ -585,6 +585,14 @@ __global__ void __launch_bounds__(256) pred_pw_kernel(const float* __restrict__ 
 // (the reference's grid is float64, utils/utils.py:183-199, so torch promotes).  One 256-thread
 // block per frame.
 // ------------------------------------------------------------------------------------------
+// Does (ov, oi) beat (v, i) in the argmax?  As torch.argmax: NaN is greater than every number, and between equal
+// values or between NaNs the lower index wins.
+__device__ __forceinline__ bool decode_beats(float ov, int oi, float v, int i) {
+  const bool onan = ov != ov, vnan = v != v;
+  if (onan || vnan) return onan && (!vnan || oi < i);
+  return ov > v || (ov == v && oi < i);
+}
+
 __global__ void __launch_bounds__(256) decode_kernel(const float* __restrict__ bbox, const float* __restrict__ cls,
                                                      int apply_sigmoid, FearBox* __restrict__ boxes) {
   __shared__ float sv[8];
@@ -597,7 +605,7 @@ __global__ void __launch_bounds__(256) decode_kernel(const float* __restrict__ b
   for (int d = 16; d > 0; d >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, v, d);
     const int oi = __shfl_xor_sync(0xffffffffu, i, d);
-    if (ov > v || (ov == v && oi < i)) {
+    if (decode_beats(ov, oi, v, i)) {
       v = ov;
       i = oi;
     }
@@ -609,7 +617,7 @@ __global__ void __launch_bounds__(256) decode_kernel(const float* __restrict__ b
   __syncthreads();
   if (t == 0) {
     for (int k = 1; k < 8; ++k)
-      if (sv[k] > v || (sv[k] == v && si[k] < i)) {
+      if (decode_beats(sv[k], si[k], v, i)) {
         v = sv[k];
         i = si[k];
       }

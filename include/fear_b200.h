@@ -201,7 +201,9 @@ int fear_advance_targets_view(const FearBox* d_boxes, const FearFrameView* d_vie
 int fear_frame_sums_u8(const FearFrameView* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
- * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)). */
+ * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
+ * The argmax follows torch.argmax: the first maximum in row-major order, with NaN greater than every number (the
+ * first NaN wins), so -0.0 and 0.0 tie and +inf beats every finite score. */
 int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,
                 void* stream);
 

@@ -179,20 +179,20 @@ def test_track_synthetic_golden_and_boxes(net):
 
 
 def test_batch_chunking_and_invariance(net):
-    """A batch larger than the reserved workspace is chunked; results do not depend on batch position."""
-    zt, xt, _, _ = fo.synthetic_crops(4)
-    zf = net.get_features(zt.cuda())
-    big_x = xt.cuda().repeat(5, 1, 1, 1)[:19]  # 19 > reserve(8): chunks 8, 8, 3
-    big_z = zf.repeat(5, 1, 1, 1)[:19]
+    """A batch larger than the reserved workspace is chunked; results do not depend on batch position.  Every frame is
+    distinct, so a chunk that read its search crop or template, or wrote its maps, at the wrong frame offset shows."""
+    zt, xt, _, _ = fo.synthetic_crops(19)  # 19 > reserve(8): chunks 8, 8, 3
+    big_x = xt.cuda()
+    big_z = torch.cat([net.get_features(zt[i:i + 1].cuda()) for i in range(19)])
     handle_reserved = net._reserved
     net._reserved = 10 ** 9  # keep the library at its 8-frame reservation: forces the chunk loop
     try:
         m = net.track(big_x, big_z)
     finally:
         net._reserved = handle_reserved
-    ref = net.track(xt.cuda(), zf)
     for i in range(19):
-        assert torch.equal(m[R][i], ref[R][i % 4]) and torch.equal(m[C][i], ref[C][i % 4]), i
+        ref = net.track(big_x[i:i + 1], big_z[i:i + 1])
+        assert torch.equal(m[R][i], ref[R][0]) and torch.equal(m[C][i], ref[C][0]), i
 
 
 def test_teacher_forced_video_frames(net):
