@@ -33,6 +33,10 @@ assert FRAME_DTYPE.itemsize == 16
 VIEW_DTYPE = np.dtype([("data", "<u8"), ("row_stride", "<i8"), ("pixel_stride", "<i8"), ("channel_stride", "<i8"),
                        ("H", "<i4"), ("W", "<i4")])
 assert VIEW_DTYPE.itemsize == 40
+# FearFrameYUV420: a YUV 4:2:0 frame (NV12, I420) anywhere in device memory, with byte strides (include/fear_b200.h)
+YUV420_DTYPE = np.dtype([("y", "<u8"), ("u", "<u8"), ("v", "<u8"), ("y_row_stride", "<i8"), ("y_pixel_stride", "<i8"),
+                         ("uv_row_stride", "<i8"), ("uv_pixel_stride", "<i8"), ("H", "<i4"), ("W", "<i4")])
+assert YUV420_DTYPE.itemsize == 64
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -59,6 +63,9 @@ _SIGNATURES = {
     "fear_crop_targets_view_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_view": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_yuv420_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_yuv420": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_yuv420_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_workspace_bytes": (c_size_t, [c_int, c_int]),

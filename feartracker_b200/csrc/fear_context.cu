@@ -1042,6 +1042,7 @@ extern "C" int fear_crop_resize_u8(const uint8_t* d_frame, int H, int W, const i
 // Multi-target tracking loop (kernels_track_loop.cuh): crop of every target in one launch, then the box update.
 static_assert(sizeof(FearTarget) == 64 && sizeof(FearFrame) == 16, "FearTarget / FearFrame layout is part of the ABI");
 static_assert(sizeof(FearFrameView) == 40, "FearFrameView layout is part of the ABI");
+static_assert(sizeof(FearFrameYUV420) == 64, "FearFrameYUV420 layout is part of the ABI");
 
 static int check_crop_targets_args(int F, int N, double offset, int out_size) {
   if (N < 1 || N > 65535) return set_err(FEAR_EINVAL, "target count must be in [1, 65535] (got %d)", N);
@@ -1108,14 +1109,38 @@ extern "C" int fear_advance_targets_view(const FearBox* d_boxes, const FearFrame
   return launch_advance_targets(d_boxes, FrameViews{d_views}, F, d_targets, N, instance_size, stream);
 }
 
-extern "C" int fear_frame_sums_u8(const FearFrameView* d_views, int F, uint64_t* d_sums, void* stream) {
+template <class Frames>
+static int launch_frame_sums(const void* d_views, Frames frames, int F, uint64_t* d_sums, void* stream) {
   if (!d_views || !d_sums) return set_err(FEAR_EINVAL, "null pointer argument");
   if (F < 1 || F > 65535) return set_err(FEAR_EINVAL, "frame count must be in [1, 65535] (got %d)", F);
   const cudaError_t e = cudaMemsetAsync(d_sums, 0, sizeof(uint64_t) * 3 * F, (cudaStream_t)stream);
   if (e != cudaSuccess) return set_err((int)e, "zeroing the frame sums failed: %s", cudaGetErrorString(e));
   frame_sums_u8_kernel<<<dim3(kFrameSumCtas, F), kFrameSumThreads, 0, (cudaStream_t)stream>>>(
-      FrameViews{d_views}, reinterpret_cast<unsigned long long*>(d_sums));
+      frames, reinterpret_cast<unsigned long long*>(d_sums));
   return check_launch("frame_sums_u8_kernel");
+}
+
+extern "C" int fear_frame_sums_u8(const FearFrameView* d_views, int F, uint64_t* d_sums, void* stream) {
+  return launch_frame_sums(d_views, FrameViews{d_views}, F, d_sums, stream);
+}
+
+// YUV 4:2:0 frames: the same kernels, reading through YUV420Frames (each pixel converted as cv2.cvtColor does).
+extern "C" int fear_crop_targets_yuv420_u8(const FearFrameYUV420* d_views, int F, FearTarget* d_targets, int N,
+                                           double offset, int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_views || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(YUV420Frames{d_views}, F, d_targets, N, offset, out_size, d_crops, stream);
+}
+
+extern "C" int fear_advance_targets_yuv420(const FearBox* d_boxes, const FearFrameYUV420* d_views, int F,
+                                           FearTarget* d_targets, int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_views || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return launch_advance_targets(d_boxes, YUV420Frames{d_views}, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_frame_sums_yuv420_u8(const FearFrameYUV420* d_views, int F, uint64_t* d_sums, void* stream) {
+  return launch_frame_sums(d_views, YUV420Frames{d_views}, F, d_sums, stream);
 }
 
 extern "C" int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,

@@ -8,9 +8,11 @@
 //                            image_ops.clamp_bbox)
 //   frame_sums_u8_kernel     exact per-channel sums of whole frames                    (np.mean of the padding colour)
 //
-// The crop and advance kernels are templates over where the frames are: a packed buffer + FearFrame table
-// (PackedFrames) or a FearFrameView table of strided frames anywhere in device memory (FrameViews).  Both read a frame
-// through the same TrackFrame (address, byte strides, H, W), so there is one copy of the arithmetic.
+// The three kernels are templates over where the frames are and what they hold: a packed buffer + FearFrame table
+// (PackedFrames) or a FearFrameView table of strided RGB frames anywhere in device memory (FrameViews), both read
+// through TrackFrame; or a FearFrameYUV420 table of YUV 4:2:0 frames (YUV420Frames), read through YUV420Frame, which
+// converts each pixel it reads to RGB as cv2.cvtColor does.  A frame type gives H, W, empty() and the RGB triple of
+// one pixel, rgb(y, x, p); the context box, resize tables, interpolation and sums exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
 // into an FMA by default, which rounds once instead of twice, so every multiply-add here is spelled with the explicitly
@@ -29,17 +31,47 @@ constexpr int kTrackCropThreads = 256;
 constexpr int kFrameSumCtas = 128;       // CTAs per frame of frame_sums_u8_kernel
 constexpr int kFrameSumThreads = 256;
 
-// A frame as the kernels read it: pixel (y, x) channel c is data[y * rs + x * ps + c * cs] (byte strides, int64).
+// An RGB frame as the kernels read it: pixel (y, x) channel c is data[y * rs + x * ps + c * cs] (byte strides, int64).
+// A value-initialised TrackFrame{} is empty.
 struct TrackFrame {
   const uint8_t* data;
   long long rs, ps, cs;
   int H, W;
+  // an entry the kernels treat like a frame index outside [0, F): no pixels, or nothing to read
+  __device__ __forceinline__ bool empty() const { return data == nullptr || H < 1 || W < 1; }
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    const uint8_t* q = data + (long long)y * rs + (long long)x * ps;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) p[c] = __ldg(q + c * cs);
+  }
 };
 
-// An entry the kernels treat like a frame index outside [0, F): no pixels, or nothing to read.
-__device__ __forceinline__ bool track_frame_empty(const TrackFrame& f) {
-  return f.data == nullptr || f.H < 1 || f.W < 1;
+// OpenCV 4.x cv::cvtColor(COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420) of one pixel, bit for bit: BT.601 limited range in
+// 20-bit fixed point, with OpenCV's ITUR_BT_601_CY / CVR / CVG / CUG / CUB coefficients and round-half-up.  int32 is
+// exact (every intermediate is below 2^30 in magnitude); >> is an arithmetic shift.
+__device__ __forceinline__ void yuv_to_rgb_bt601(int Y, int U, int V, int p[3]) {
+  const int yy = max(0, Y - 16) * 1220542 + (1 << 19);
+  const int u = U - 128, v = V - 128;
+  p[0] = min(max((yy + 1673527 * v) >> 20, 0), 255);
+  p[1] = min(max((yy - 852492 * v - 409993 * u) >> 20, 0), 255);
+  p[2] = min(max((yy + 2116026 * u) >> 20, 0), 255);
 }
+
+// A YUV 4:2:0 frame (FearFrameYUV420): luma (y, x) is Y[y * yrs + x * yps]; its chroma is sample (y >> 1, x >> 1) of
+// the U and V planes (shared strides uvrs, uvps).  rgb() converts the pixel with yuv_to_rgb_bt601, so every kernel sees
+// the RGB frame cv2.cvtColor would produce.  H and W must be even.  A value-initialised YUV420Frame{} is empty.
+struct YUV420Frame {
+  const uint8_t *Y, *U, *V;
+  long long yrs, yps, uvrs, uvps;
+  int H, W;
+  __device__ __forceinline__ bool empty() const {
+    return Y == nullptr || U == nullptr || V == nullptr || H < 1 || W < 1 || (H & 1) || (W & 1);
+  }
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    const long long c = (long long)(y >> 1) * uvrs + (long long)(x >> 1) * uvps;
+    yuv_to_rgb_bt601(__ldg(Y + (long long)y * yrs + (long long)x * yps), __ldg(U + c), __ldg(V + c), p);
+  }
+};
 
 // Frame i of a packed buffer located by a FearFrame table (fear_crop_targets_u8 / fear_advance_targets).
 struct PackedFrames {
@@ -59,6 +91,26 @@ struct FrameViews {
     return TrackFrame{v.data, v.row_stride, v.pixel_stride, v.channel_stride, v.H, v.W};
   }
 };
+
+// Frame i of a FearFrameYUV420 table (the *_yuv420 entry points).
+struct YUV420Frames {
+  const FearFrameYUV420* views;
+  __device__ __forceinline__ YUV420Frame operator()(int i) const {
+    const FearFrameYUV420 v = views[i];
+    return YUV420Frame{v.y, v.u, v.v, v.y_row_stride, v.y_pixel_stride, v.uv_row_stride, v.uv_pixel_stride, v.H, v.W};
+  }
+};
+
+// One bilinear tap: the RGB triple of pixel (y, x) of the frame, or the padding colour when the tap lies outside it.
+template <class Frame>
+__device__ __forceinline__ void track_tap(const Frame& fr, bool inside, int y, int x, const int pad[3], int p[3]) {
+  if (inside) {
+    fr.rgb(y, x, p);
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) p[c] = pad[c];
+  }
+}
 
 // context_box(bbox, offset) of image_ops (reference utils.py get_extended_crop): float64, truncated to int32.
 __device__ __forceinline__ void track_context_box(int x, int y, int w, int h, double off, int& cx, int& cy, int& cw,
@@ -97,7 +149,8 @@ __device__ __forceinline__ void track_axis_entry(int d, int src, int dst, bool c
 // context box from the target's bbox; the CTA of tile 0 also stores it in the target (cx, cy, cw, ch), which the
 // advance kernel reads after the network has run.  The x tables (S entries) and this tile's y tables are built in
 // shared memory; the pixel arithmetic is crop_resize_u8_kernel's.  A target whose frame index is outside [0, F), or
-// whose frame is empty (track_frame_empty), gets a crop of its padding colour and reads no pixel.
+// whose frame is empty (empty()), gets a crop of its padding colour and reads no pixel.  Each tap is converted to RGB
+// (rgb()) before it is interpolated, as cv2 converts a whole frame before copyMakeBorder + resize.
 template <class Frames>
 __global__ void __launch_bounds__(kTrackCropThreads) crop_targets_u8_kernel(Frames frames, int F,
                                                                             FearTarget* __restrict__ targets,
@@ -122,8 +175,9 @@ __global__ void __launch_bounds__(kTrackCropThreads) crop_targets_u8_kernel(Fram
   }
   uint8_t* out = crops + ((long long)n * S + row0) * S * 3;
   const bool in_range = frame_idx >= 0 && frame_idx < F;
-  const TrackFrame fr = in_range ? frames(frame_idx) : TrackFrame{nullptr, 0, 0, 0, 0, 0};
-  if (track_frame_empty(fr)) {
+  using Frame = decltype(frames(0));
+  const Frame fr = in_range ? frames(frame_idx) : Frame{};
+  if (fr.empty()) {
     for (int i = threadIdx.x; i < rows * S * 3; i += blockDim.x) out[i] = (uint8_t)pad[i % 3];
     return;
   }
@@ -142,18 +196,15 @@ __global__ void __launch_bounds__(kTrackCropThreads) crop_targets_u8_kernel(Fram
     const int fx0 = cx + x0, fx1 = cx + x1, fy0 = cy + y0, fy1 = cy + y1;
     const bool in_x0 = fx0 >= 0 && fx0 < W, in_x1 = fx1 >= 0 && fx1 < W;
     const bool in_y0 = fy0 >= 0 && fy0 < H, in_y1 = fy1 >= 0 && fy1 < H;
-    const uint8_t* r0 = fr.data + (long long)fy0 * fr.rs;
-    const uint8_t* r1 = fr.data + (long long)fy1 * fr.rs;
-    const long long o0 = (long long)fx0 * fr.ps, o1 = (long long)fx1 * fr.ps;
+    int p00[3], p01[3], p10[3], p11[3];
+    track_tap(fr, in_y0 && in_x0, fy0, fx0, pad, p00);
+    track_tap(fr, in_y0 && in_x1, fy0, fx1, pad, p01);
+    track_tap(fr, in_y1 && in_x0, fy1, fx0, pad, p10);
+    track_tap(fr, in_y1 && in_x1, fy1, fx1, pad, p11);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const long long oc = c * fr.cs;
-      const int p00 = (in_y0 && in_x0) ? (int)__ldg(r0 + o0 + oc) : pad[c];
-      const int p01 = (in_y0 && in_x1) ? (int)__ldg(r0 + o1 + oc) : pad[c];
-      const int p10 = (in_y1 && in_x0) ? (int)__ldg(r1 + o0 + oc) : pad[c];
-      const int p11 = (in_y1 && in_x1) ? (int)__ldg(r1 + o1 + oc) : pad[c];
-      const int s0 = p00 * a0 + p01 * a1;
-      const int s1 = p10 * a0 + p11 * a1;
+      const int s0 = p00[c] * a0 + p01[c] * a1;
+      const int s1 = p10[c] * a0 + p11[c] * a1;
       const int v = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
       out[(long long)i * 3 + c] = (uint8_t)min(max(v, 0), 255);
     }
@@ -164,7 +215,8 @@ __global__ void __launch_bounds__(kTrackCropThreads) crop_targets_u8_kernel(Fram
 //   sx = cw / instance_size;  x = round(box.x * sx + cx);  w = max(3, round(box.w * sx))   (y, h alike)
 // Python's round() is half-to-even = rint.  The values stay in float64 (they are integers there) until trim_box has
 // clamped them into the frame, so no int32 overflow can differ from Python's unbounded ints.  A target whose frame
-// index is outside [0, F), or whose frame is empty (track_frame_empty), keeps its box.
+// index is outside [0, F), or whose frame is empty (empty()), keeps its box.  Of the frame, only H, W and
+// empty() are used.
 template <class Frames>
 __global__ void __launch_bounds__(128) advance_targets_kernel(const FearBox* __restrict__ boxes, Frames frames, int F,
                                                               FearTarget* __restrict__ targets, int N,
@@ -173,8 +225,8 @@ __global__ void __launch_bounds__(128) advance_targets_kernel(const FearBox* __r
   if (n >= N) return;
   FearTarget t = targets[n];
   if (t.frame < 0 || t.frame >= F) return;
-  const TrackFrame fr = frames(t.frame);
-  if (track_frame_empty(fr)) return;
+  const auto fr = frames(t.frame);
+  if (fr.empty()) return;
   const FearBox b = boxes[n];
   const double sx = __ddiv_rn((double)t.cw, (double)instance_size);
   const double sy = __ddiv_rn((double)t.ch, (double)instance_size);
@@ -207,19 +259,22 @@ __global__ void __launch_bounds__(128) advance_targets_kernel(const FearBox* __r
 // CTA (g, f) visits (a grid-stride loop over the frame's H * W pixels, row-major; the (y, x) position advances by the
 // stride's quotient and remainder, so the loop needs no division).  One uint64 atomicAdd per channel per CTA: integer
 // sums in any order are the same, so the result is deterministic.  sums must be zero on entry; an empty frame adds 0.
-__global__ void __launch_bounds__(kFrameSumThreads) frame_sums_u8_kernel(FrameViews frames,
+// The sums are of rgb(), so a YUV frame sums its converted RGB pixels.
+template <class Frames>
+__global__ void __launch_bounds__(kFrameSumThreads) frame_sums_u8_kernel(Frames frames,
                                                                          unsigned long long* __restrict__ sums) {
   __shared__ unsigned long long part[3][kFrameSumThreads / 32];
-  const TrackFrame fr = frames(blockIdx.y);
-  if (track_frame_empty(fr)) return;
+  const auto fr = frames(blockIdx.y);
+  if (fr.empty()) return;
   const long long W = fr.W, stride = (long long)gridDim.x * blockDim.x;
   const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long sy = stride / W, sx = stride - sy * W;
   unsigned long long acc[3] = {0, 0, 0};
   for (long long y = i0 / W, x = i0 - y * W; y < fr.H;) {
-    const uint8_t* p = fr.data + y * fr.rs + x * fr.ps;
+    int p[3];
+    fr.rgb((int)y, (int)x, p);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) acc[c] += __ldg(p + c * fr.cs);
+    for (int c = 0; c < 3; ++c) acc[c] += p[c];
     x += sx;
     y += sy;
     if (x >= W) {

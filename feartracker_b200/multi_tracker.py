@@ -5,9 +5,10 @@
     out = trk.update(frames)                      # {"bbox": (N,4) int64, "score": (N,) float32, "ids": (N,) int64}
     trk.remove(ids); trk.reset()
 
-Frames are numpy arrays in host memory or uint8 (H, W, 3) CUDA tensors already on the tracker's device, strided views
-included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y0:y1, x0:x1]); tensors are read where
-they are, without a copy.
+Frames are numpy arrays in host memory, uint8 (H, W, 3) CUDA tensors already on the tracker's device, strided views
+included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y0:y1, x0:x1]), or YUV420Frames: NV12 /
+I420 planes on the device as a video decoder writes them, converted to RGB inside the crop exactly as cv2.cvtColor
+converts them.  Tensors and YUV planes are read where they are, without a copy.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -20,8 +21,9 @@ on per-target state kept in device memory (an (N, 16) int32 tensor of FearTarget
 step is captured once as a CUDA graph and replayed every frame.  The kernels find the frames through a table of
 FearFrameView records (address, byte strides, H, W) in a fixed device buffer, written before every step: numpy frames
 are packed into one pinned buffer and sent with one copy, and their views point into the packed device buffer; CUDA
-tensors' views point at the tensors.  The host then reads back the boxes and scores.  The launch count of a step
-depends neither on N nor on the kind of frames.
+tensors' views point at the tensors.  YUV420Frames go into a second fixed table of FearFrameYUV420 records, read by the
+*_yuv420 entry points.  The host then reads back the boxes and scores.  The launch count of a step depends neither on
+N nor on the kind of frames.
 """
 import math
 import warnings
@@ -33,7 +35,13 @@ import torch
 from . import _lib, image_ops
 
 _FRAME_ALIGN = 16  # byte alignment of each frame inside the packed buffer
-_MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView
+_MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView and FearFrameYUV420
+# the entry points that read each frame table: frame sums, target crops, box advance
+_ENTRY_POINTS = {
+    "views": ("fear_frame_sums_u8", "fear_crop_targets_view_u8", "fear_advance_targets_view"),
+    "yuv": ("fear_frame_sums_yuv420_u8", "fear_crop_targets_yuv420_u8", "fear_advance_targets_yuv420"),
+}
+_TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV420_DTYPE}
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -41,6 +49,76 @@ def frame_view(frame: torch.Tensor) -> tuple:
     it lies in memory: the address of pixel (0, 0) channel R and the byte strides (a uint8 stride is a byte stride)."""
     rs, ps, cs = frame.stride()
     return (frame.data_ptr(), rs, ps, cs, frame.shape[0], frame.shape[1])
+
+
+class YUV420Frame:
+    """A YUV 4:2:0 frame as a video decoder writes it: 8-bit BT.601 limited range, a luma plane ``y`` (H, W) and
+    chroma planes ``u`` (Cb) and ``v`` (Cr) of (H/2, W/2), with H and W even.  Pixel (r, c) takes its chroma from
+    sample (r // 2, c // 2).  The planes are uint8 tensors or views with any non-negative strides, and ``u`` and ``v``
+    share their strides.  FEARMultiTracker reads the planes where they are and converts every pixel it reads exactly as
+    ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420)`` does, so no RGB copy of the frame is made.
+
+        YUV420Frame.nv12(t)    t (3H/2, W): H luma rows, then H/2 rows of interleaved (U, V) pairs; the rows may be
+                               pitched (t = surface[:, :W]), as NVDEC and cv2 lay out NV12
+        YUV420Frame.i420(t)    t contiguous (3H/2, W): the Y, U and V planes one after another (cv2's I420, ffmpeg's
+                               yuv420p)
+        YUV420Frame(y, u, v)   separate planes, regions of interest at even offsets
+
+    ``shape`` is (H, W, 3), the shape of the RGB frame it stands for.  The constructors raise ValueError on a malformed
+    frame; they do not look at the device (the tracker checks that)."""
+
+    def __init__(self, y: torch.Tensor, u: torch.Tensor, v: torch.Tensor) -> None:
+        for name, p in (("y", y), ("u", u), ("v", v)):
+            if not isinstance(p, torch.Tensor) or p.dtype != torch.uint8 or p.ndim != 2:
+                what = f"{p.dtype} {tuple(p.shape)}" if isinstance(p, torch.Tensor) else type(p).__name__
+                raise ValueError(f"YUV420Frame plane {name} must be a 2-D uint8 tensor, got {what}")
+            if min(p.stride()) < 0:
+                raise ValueError(f"YUV420Frame plane {name} has a negative stride {p.stride()}")
+        h, w = y.shape
+        if not (2 <= h <= _MAX_SIDE and 2 <= w <= _MAX_SIDE) or h % 2 or w % 2:
+            raise ValueError(f"YUV 4:2:0 luma must be (H, W) with H and W even and >= 2, got {tuple(y.shape)}")
+        if tuple(u.shape) != (h // 2, w // 2) or tuple(v.shape) != (h // 2, w // 2):
+            raise ValueError(f"YUV 4:2:0 chroma planes must be ({h // 2}, {w // 2}) for luma ({h}, {w}), got "
+                             f"{tuple(u.shape)} and {tuple(v.shape)}")
+        if u.stride() != v.stride():
+            raise ValueError(f"YUV420Frame u and v planes must share their strides, got {u.stride()} and {v.stride()}")
+        self.y, self.u, self.v = y, u, v
+        self.shape = (h, w, 3)
+
+    @classmethod
+    def nv12(cls, t: torch.Tensor) -> "YUV420Frame":
+        h = cls._luma_rows(t, "nv12")
+        uv = t[h:]
+        return cls(t[:h], uv[:, 0::2], uv[:, 1::2])
+
+    @classmethod
+    def i420(cls, t: torch.Tensor) -> "YUV420Frame":
+        h, w = cls._luma_rows(t, "i420"), t.shape[1]
+        if not t.is_contiguous():
+            raise ValueError(f"YUV420Frame.i420 takes a contiguous tensor, got strides {t.stride()}")
+        flat, luma, quarter = t.reshape(-1), h * w, h * w // 4
+        return cls(flat[:luma].view(h, w), flat[luma:luma + quarter].view(h // 2, w // 2),
+                   flat[luma + quarter:].view(h // 2, w // 2))
+
+    @staticmethod
+    def _luma_rows(t, layout: str) -> int:
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.ndim != 2 or t.shape[0] % 3 or t.shape[1] % 2:
+            what = f"{t.dtype} {tuple(t.shape)}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"YUV420Frame.{layout} takes a uint8 (3H/2, W) tensor with H and W even, got {what}")
+        return 2 * t.shape[0] // 3
+
+    def record(self) -> tuple:
+        """The FearFrameYUV420 record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W):
+        the addresses of luma sample (0, 0) and of the Cb and Cr samples (0, 0), and the byte strides (a uint8 stride
+        is a byte stride)."""
+        (yrs, yps), (uvrs, uvps) = self.y.stride(), self.u.stride()
+        return (self.y.data_ptr(), self.u.data_ptr(), self.v.data_ptr(), yrs, yps, uvrs, uvps, *self.shape[:2])
+
+
+def _frame_kind(frame) -> str:
+    if isinstance(frame, YUV420Frame):
+        return "yuv"
+    return "cuda" if isinstance(frame, torch.Tensor) else "numpy"
 
 
 class FEARMultiTracker:
@@ -94,9 +172,10 @@ class FEARMultiTracker:
         """Start tracking ``rects`` ((n, 4) [x, y, w, h]); target i lives in stream ``streams[i]`` (default 0), whose
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
-        ``frames`` are all numpy arrays or all CUDA tensors (see ``update``).  A target's padding colour is the mean
-        colour of its frame, from exact per-channel sums computed on the device."""
-        frames, on_device = self._check_frames(frames)
+        ``frames`` are all numpy arrays, all CUDA tensors or all YUV420Frames (see ``update``).  A target's padding
+        colour is the mean colour of its frame (of the cv2-converted RGB frame for a YUV420Frame), from exact
+        per-channel sums computed on the device."""
+        frames, kind = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
         if rects.ndim == 1 and rects.size == 4:
             rects = rects[None]
@@ -122,11 +201,12 @@ class FEARMultiTracker:
         with torch.cuda.device(dev):
             b = self._buffers(dev)
             num_frames = len(frames)
-            self._upload_frames(frames, on_device, dev)
+            table = self._upload_frames(frames, kind, dev)
+            sums_fn, crop_fn, _ = _ENTRY_POINTS[table]
             lib = _lib.load()
             stream = torch.cuda.current_stream(dev)
-            _lib.check(lib.fear_frame_sums_u8(b["views"].data_ptr(), num_frames, b["sums"].data_ptr(),
-                                              stream.cuda_stream), "fear_frame_sums_u8")
+            _lib.check(getattr(lib, sums_fn)(b[table].data_ptr(), num_frames, b["sums"].data_ptr(), stream.cuda_stream),
+                       sums_fn)
             b["sums_pin"][:num_frames].copy_(b["sums"][:num_frames], non_blocking=True)
             stream.synchronize()
             # numpy's mean of uint8 is an exact float64 sum of integers over H * W; then cv::saturate_cast, as
@@ -139,9 +219,9 @@ class FEARMultiTracker:
             b["state"][n0:n0 + n].copy_(torch.from_numpy(recs).pin_memory(), non_blocking=True)
             size = int(cfg["template_size"])
             crops = b["tcrops"][:n]
-            _lib.check(lib.fear_crop_targets_view_u8(b["views"].data_ptr(), num_frames, b["state"][n0].data_ptr(), n,
-                                                     float(cfg["template_bbox_offset"]), size, crops.data_ptr(),
-                                                     stream.cuda_stream), "fear_crop_targets_view_u8")
+            _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b["state"][n0].data_ptr(), n,
+                                             float(cfg["template_bbox_offset"]), size, crops.data_ptr(),
+                                             stream.cuda_stream), crop_fn)
             b["zf"][n0:n0 + n].copy_(self.net.get_features(crops))
             stream.synchronize()  # the pinned staging buffers are reused by the next call
         new_ids = np.arange(self._next_id, self._next_id + n, dtype=np.int64)
@@ -167,13 +247,16 @@ class FEARMultiTracker:
     def update(self, frames) -> Dict[str, np.ndarray]:
         """One frame of every stream -> the new box and score of every target, in the order of ``ids``.
 
-        ``frames`` (one frame or a list of F, stream i's frame at index i) are either all ``np.ndarray`` or all
-        ``torch.Tensor``; the kind may change from one call to the next.  A tensor frame is uint8 of shape (H, W, 3)
-        on the tracker's CUDA device, with any non-negative strides: views are read as they are, nothing is copied.
-        Tensor frames must be ready on the current CUDA stream (write them on that stream, or make it wait for the
-        stream that did, as for any torch op).  ``update`` synchronises that stream before it returns, so the tensors
-        only need to live until the call returns."""
-        frames, on_device = self._check_frames(frames)
+        ``frames`` (one frame or a list of F, stream i's frame at index i) are all ``np.ndarray``, all
+        ``torch.Tensor`` or all ``YUV420Frame``; the kind may change from one call to the next.  A tensor frame is
+        uint8 of shape (H, W, 3) on the tracker's CUDA device, with any non-negative strides: views are read as they
+        are, nothing is copied.  A ``YUV420Frame``'s planes must be on the tracker's CUDA device; they are read in
+        place too, and every target fed YUV420Frames gives exactly the ids, boxes and scores of the same tracker fed
+        ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420)`` as numpy arrays.  Device frames must be
+        ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
+        any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
+        call returns."""
+        frames, kind = self._check_frames(frames)
         n = len(self._ids)
         if n and int(self._streams.max()) >= len(frames):
             raise ValueError(f"targets track stream {int(self._streams.max())} but only {len(frames)} frames were given")
@@ -183,8 +266,8 @@ class FEARMultiTracker:
         dev = self._device()
         with torch.cuda.device(dev):
             b = self._buffers(dev)
-            self._upload_frames(frames, on_device, dev)
-            boxes = self._run_step(n, len(frames), dev)
+            table = self._upload_frames(frames, kind, dev)
+            boxes = self._run_step(n, len(frames), table, dev)
             b["state_pin"][:n].copy_(b["state"][:n], non_blocking=True)
             b["box_pin"][:n].copy_(boxes, non_blocking=True)
             torch.cuda.current_stream(dev).synchronize()
@@ -204,23 +287,26 @@ class FEARMultiTracker:
         return torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
 
     def _check_frames(self, frames):
-        """-> (list of frames, True if they are CUDA tensors).  Raises ValueError before any device call."""
-        if isinstance(frames, (np.ndarray, torch.Tensor)) and frames.ndim == 3:
+        """-> (list of frames, their kind: "numpy", "cuda" or "yuv").  Raises ValueError before any device call."""
+        if isinstance(frames, YUV420Frame) or (isinstance(frames, (np.ndarray, torch.Tensor)) and frames.ndim == 3):
             frames = [frames]
         frames = list(frames)
         if not frames:
             raise ValueError("no frames given")
-        on_device = isinstance(frames[0], torch.Tensor)
-        if any(isinstance(f, torch.Tensor) != on_device for f in frames):
-            raise ValueError("frames of one call must be all numpy arrays or all CUDA tensors, not a mix")
+        kind = _frame_kind(frames[0])
+        if any(_frame_kind(f) != kind for f in frames):
+            raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV420Frames, "
+                             "not a mix")
         for i, f in enumerate(frames):
-            if on_device:
+            if kind == "yuv":
+                self._check_device(i, f.y, f.u, f.v)
+            elif kind == "cuda":
                 self._check_tensor_frame(i, f)
             elif not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
                     or f.shape[0] < 1 or f.shape[1] < 1:
                 what = f"{f.dtype} {f.shape}" if isinstance(f, np.ndarray) else type(f).__name__
                 raise ValueError(f"frame {i} must be a uint8 HxWx3 RGB array, got {what}")
-        return frames, on_device
+        return frames, kind
 
     def _check_tensor_frame(self, i: int, f: torch.Tensor) -> None:
         if f.dtype != torch.uint8 or f.ndim != 3 or f.shape[2] != 3 or not (1 <= f.shape[0] <= _MAX_SIDE) \
@@ -228,12 +314,16 @@ class FEARMultiTracker:
             raise ValueError(f"frame {i} must be a uint8 HxWx3 RGB tensor, got {f.dtype} {tuple(f.shape)}")
         if min(f.stride()) < 0:
             raise ValueError(f"frame {i} has a negative stride {f.stride()}")
-        if f.device.type != "cuda":
-            raise ValueError(f"frame {i} is a {f.device} tensor: tensor frames must be on the tracker's CUDA device "
-                             "(pass host frames as numpy arrays)")
-        dev = self._device()
-        if f.device != dev:
-            raise ValueError(f"frame {i} is on {f.device}, the tracker on {dev}")
+        self._check_device(i, f)
+
+    def _check_device(self, i: int, *tensors: torch.Tensor) -> None:
+        for t in tensors:
+            if t.device.type != "cuda":
+                raise ValueError(f"frame {i} is in a {t.device} tensor: tensor frames and YUV planes must be on the "
+                                 "tracker's CUDA device (pass host frames as numpy arrays)")
+            dev = self._device()
+            if t.device != dev:
+                raise ValueError(f"frame {i} is on {t.device}, the tracker on {dev}")
 
     @staticmethod
     def _check_streams(streams, n: int, num_frames: int) -> np.ndarray:
@@ -261,22 +351,31 @@ class FEARMultiTracker:
             tcrops=torch.empty((m, tsize, tsize, 3), dtype=torch.uint8, device=dev),
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
-            frames_pin=None, frames=None, views_pin=None, views=None, sums_pin=None, sums=None)
+            frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, sums_pin=None,
+            sums=None)
         return b
 
-    def _upload_frames(self, frames, on_device: bool, dev: torch.device) -> None:
-        """Write the FearFrameView table of ``frames`` into the device table the kernels read.  Numpy frames are packed
-        into the pinned staging buffer first and sent with one host-to-device copy (the packed layout is recomputed
-        only when their shapes change); CUDA tensors are used where they are."""
-        b, num_frames, rec = self._buf, len(frames), _lib.VIEW_DTYPE.itemsize
-        if b["views"] is None or b["views"].numel() < num_frames * rec:  # grows only: the step graph keys on it
-            b["views_pin"] = torch.empty(num_frames * rec, dtype=torch.uint8).pin_memory()
-            b["views"] = torch.empty(num_frames * rec, dtype=torch.uint8, device=dev)
-            # fear_frame_sums_u8 writes uint64; int64 storage, read back as uint64
+    def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
+        """Write the frame table of ``frames`` into the fixed device table the kernels read, and return its name:
+        "yuv" (FearFrameYUV420 records) for YUV420Frames, "views" (FearFrameView records) otherwise.  Numpy frames are
+        packed into the pinned staging buffer first and sent with one host-to-device copy (the packed layout is
+        recomputed only when their shapes change); CUDA tensors and YUV planes are used where they are."""
+        b, num_frames = self._buf, len(frames)
+        name = "yuv" if kind == "yuv" else "views"
+        dtype = _TABLE_DTYPES[name]
+        nbytes = num_frames * dtype.itemsize
+        if b[name] is None or b[name].numel() < nbytes:  # grows only: the step graph keys on it
+            b[name + "_pin"] = torch.empty(nbytes, dtype=torch.uint8).pin_memory()
+            b[name] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        if b["sums"] is None or b["sums"].shape[0] < num_frames:
+            # the frame sums entry points write uint64; int64 storage, read back as uint64
             b["sums_pin"] = torch.empty((num_frames, 3), dtype=torch.int64).pin_memory()
             b["sums"] = torch.empty((num_frames, 3), dtype=torch.int64, device=dev)
-        table = b["views_pin"].numpy()[:num_frames * rec].view(_lib.VIEW_DTYPE)
-        if on_device:
+        table = b[name + "_pin"].numpy()[:nbytes].view(dtype)
+        if kind == "yuv":
+            for i, f in enumerate(frames):
+                table[i] = f.record()
+        elif kind == "cuda":
             for i, f in enumerate(frames):
                 table[i] = frame_view(f)
         else:
@@ -298,36 +397,38 @@ class FEARMultiTracker:
                 table[i] = (base + o, 3 * w, 3, 1, h, w)
             nb = b["nbytes"]
             b["frames"][:nb].copy_(b["frames_pin"][:nb], non_blocking=True)
-        b["views"][:num_frames * rec].copy_(b["views_pin"][:num_frames * rec], non_blocking=True)
+        b[name][:nbytes].copy_(b[name + "_pin"][:nbytes], non_blocking=True)
+        return name
 
-    def _step(self, n: int, num_frames: int, dev: torch.device) -> torch.Tensor:
+    def _step(self, n: int, num_frames: int, dev: torch.device, table: str = "views") -> torch.Tensor:
         b, cfg, lib = self._buf, self.tracking_config, _lib.load()
+        _, crop_fn, advance_fn = _ENTRY_POINTS[table]
         size = int(cfg["instance_size"])
         s = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.fear_crop_targets_view_u8(b["views"].data_ptr(), num_frames, b["state"].data_ptr(), n,
-                                                 float(cfg["search_context"]), size, b["crops"].data_ptr(), s),
-                   "fear_crop_targets_view_u8")
+        _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b["state"].data_ptr(), n,
+                                         float(cfg["search_context"]), size, b["crops"].data_ptr(), s), crop_fn)
         boxes = self.net.track_boxes(b["crops"][:n], b["zf"][:n])
-        _lib.check(lib.fear_advance_targets_view(boxes.data_ptr(), b["views"].data_ptr(), num_frames,
-                                                 b["state"].data_ptr(), n, size, s), "fear_advance_targets_view")
+        _lib.check(getattr(lib, advance_fn)(boxes.data_ptr(), b[table].data_ptr(), num_frames, b["state"].data_ptr(),
+                                            n, size, s), advance_fn)
         return boxes
 
-    def _run_step(self, n: int, num_frames: int, dev: torch.device) -> torch.Tensor:
+    def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device) -> torch.Tensor:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
-        keyed by the target count, the frame count, the table buffer and the net's generation.  ``cuda_graph=False``
-        in the tracking config keeps eager launches."""
-        key = (n, num_frames, self._buf["views"].data_ptr())
+        keyed by the target count, the frame count, which table the step reads (RGB views or YUV 4:2:0 records) and
+        its buffer, and the net's generation.  ``cuda_graph=False`` in the tracking config keeps eager launches."""
+        key = (n, num_frames, table, self._buf[table].data_ptr())
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):
-            # new target or frame count, a new table buffer, or the net's workspace / weights / options changed: the
-            # pointers and sizes baked into the captured graph are stale -> warm up eagerly and capture again
+            # new target or frame count, another table or a new table buffer, or the net's workspace / weights /
+            # options changed: the pointers and sizes baked into the captured graph are stale -> warm up eagerly and
+            # capture again
             self._graph, self._graph_key, self._calls = None, key, 0
         use_graph = self.tracking_config.get("cuda_graph", True) and self._graph_ok
         if use_graph and self._graph is None and self._calls >= 1:
             try:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    self._graph_boxes = self._step(n, num_frames, dev)
+                    self._graph_boxes = self._step(n, num_frames, dev, table)
                 self._graph, self._graph_gen = g, self.net.generation()
             except RuntimeError as exc:
                 warnings.warn(f"FEARMultiTracker: CUDA-graph capture of the step failed ({exc}); using eager launches")
@@ -337,4 +438,4 @@ class FEARMultiTracker:
         if use_graph and self._graph is not None:
             self._graph.replay()
             return self._graph_boxes
-        return self._step(n, num_frames, dev)
+        return self._step(n, num_frames, dev, table)

@@ -24,6 +24,9 @@
  *   fear_crop_targets_view_u8 / fear_advance_targets_view   the same on frames located by FearFrameView (strided,
  *                         anywhere in device memory)
  *   fear_frame_sums_u8    np.mean(frame, axis=(0, 1)) of get_extended_crop's padding, as exact integer sums
+ *   fear_crop_targets_yuv420_u8 / fear_advance_targets_yuv420 / fear_frame_sums_yuv420_u8   the same three on YUV 4:2:0
+ *                         frames (NV12, I420) located by FearFrameYUV420, each pixel converted to RGB exactly as
+ *                         cv2.cvtColor(COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420) converts it
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -84,6 +87,21 @@ typedef struct FearFrameView {
   int64_t row_stride, pixel_stride, channel_stride; /* bytes, >= 0                                       */
   int32_t H, W;
 } FearFrameView;
+/* A YUV 4:2:0 frame (8-bit BT.601 limited range, as a video decoder writes it) wherever it lives in device memory:
+ * 64 bytes.  Luma of pixel (y, x) is y[y * y_row_stride + x * y_pixel_stride]; its chroma is sample (y / 2, x / 2) of
+ * u (Cb) and v (Cr), at u[(y / 2) * uv_row_stride + (x / 2) * uv_pixel_stride] and likewise in v.  Strides in bytes,
+ * >= 0; H, W is the luma size.  NV12 with row pitch P at address b is {b, b + H*P, b + H*P + 1, P, 1, P, 2, H, W};
+ * packed I420 is {b, b + H*W, b + H*W + H*W/4, W, 1, W/2, 1, H, W}; separate planes and even-offset regions of interest
+ * are the same record with other addresses.  The kernels read the frame as the RGB image
+ * cv2.cvtColor(frame, COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420) gives, bit for bit (OpenCV 4.x's fixed-point conversion,
+ * nearest chroma).  An entry with a null plane, H < 1, W < 1, or an odd H or W is treated like a frame index outside
+ * [0, F). */
+typedef struct FearFrameYUV420 {
+  const uint8_t *y, *u, *v;                /* device addresses of luma sample (0, 0), Cb and Cr samples (0, 0) */
+  int64_t y_row_stride, y_pixel_stride;    /* bytes, >= 0                                                      */
+  int64_t uv_row_stride, uv_pixel_stride;  /* bytes, >= 0, shared by u and v                                   */
+  int32_t H, W;                            /* luma size, both even                                             */
+} FearFrameYUV420;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -199,6 +217,19 @@ int fear_advance_targets_view(const FearBox* d_boxes, const FearFrameView* d_vie
  * (the padding colour of a new target).  Zeroes d_sums with cudaMemsetAsync, then one launch.  FEAR_EINVAL: a null
  * pointer, F < 1 or F > 65535. */
 int fear_frame_sums_u8(const FearFrameView* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* The same three on YUV 4:2:0 frames located through d_views (F FearFrameYUV420 entries in device memory), so NV12 or
+ * I420 surfaces can stay where a decoder left them and no RGB copy of the frame is made.  Every pixel a kernel reads is
+ * converted as cv2.cvtColor converts it (each bilinear tap is converted, then interpolated; padding taps use the
+ * target's RGB padding colour), so crops, boxes and sums equal those of the *_view entry points on the cv2-converted
+ * RGB frame.  fear_frame_sums_yuv420_u8 sums the converted R, G and B.  fear_advance_targets_yuv420 reads only H and W.
+ * Same semantics and FEAR_EINVAL rules as fear_crop_targets_view_u8 / fear_advance_targets_view / fear_frame_sums_u8;
+ * an entry with a null plane, H < 1, W < 1 or an odd H or W gets a padding-colour crop, keeps its box and sums to 0. */
+int fear_crop_targets_yuv420_u8(const FearFrameYUV420* d_views, int F, FearTarget* d_targets, int N, double offset,
+                                int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_yuv420(const FearBox* d_boxes, const FearFrameYUV420* d_views, int F, FearTarget* d_targets,
+                                int N, int instance_size, void* stream);
+int fear_frame_sums_yuv420_u8(const FearFrameYUV420* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
