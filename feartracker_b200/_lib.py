@@ -37,6 +37,10 @@ assert VIEW_DTYPE.itemsize == 40
 YUV420_DTYPE = np.dtype([("y", "<u8"), ("u", "<u8"), ("v", "<u8"), ("y_row_stride", "<i8"), ("y_pixel_stride", "<i8"),
                          ("uv_row_stride", "<i8"), ("uv_pixel_stride", "<i8"), ("H", "<i4"), ("W", "<i4")])
 assert YUV420_DTYPE.itemsize == 64
+# FearFrameYUV: FearFrameYUV420 plus its colour format (matrix, range, bit depth, sample alignment)
+YUV_DTYPE = np.dtype(YUV420_DTYPE.descr + [("matrix", "<i4"), ("full_range", "<i4"), ("bits", "<i4"),
+                                           ("shift", "<i4")])
+assert YUV_DTYPE.itemsize == 80
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -66,6 +70,9 @@ _SIGNATURES = {
     "fear_crop_targets_yuv420_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_yuv420": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_yuv420_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_yuv_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_yuv": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_yuv_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_workspace_bytes": (c_size_t, [c_int, c_int]),

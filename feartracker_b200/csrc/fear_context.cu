@@ -1043,6 +1043,7 @@ extern "C" int fear_crop_resize_u8(const uint8_t* d_frame, int H, int W, const i
 static_assert(sizeof(FearTarget) == 64 && sizeof(FearFrame) == 16, "FearTarget / FearFrame layout is part of the ABI");
 static_assert(sizeof(FearFrameView) == 40, "FearFrameView layout is part of the ABI");
 static_assert(sizeof(FearFrameYUV420) == 64, "FearFrameYUV420 layout is part of the ABI");
+static_assert(sizeof(FearFrameYUV) == 80, "FearFrameYUV layout is part of the ABI");
 
 static int check_crop_targets_args(int F, int N, double offset, int out_size) {
   if (N < 1 || N > 65535) return set_err(FEAR_EINVAL, "target count must be in [1, 65535] (got %d)", N);
@@ -1141,6 +1142,26 @@ extern "C" int fear_advance_targets_yuv420(const FearBox* d_boxes, const FearFra
 
 extern "C" int fear_frame_sums_yuv420_u8(const FearFrameYUV420* d_views, int F, uint64_t* d_sums, void* stream) {
   return launch_frame_sums(d_views, YUV420Frames{d_views}, F, d_sums, stream);
+}
+
+// YUV 4:2:0 frames of any FearFrameYUV format: the same kernels, reading through YUVFrames (each entry's format is
+// read, checked and converted on the device).
+extern "C" int fear_crop_targets_yuv_u8(const FearFrameYUV* d_views, int F, FearTarget* d_targets, int N, double offset,
+                                        int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_views || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(YUVFrames{d_views}, F, d_targets, N, offset, out_size, d_crops, stream);
+}
+
+extern "C" int fear_advance_targets_yuv(const FearBox* d_boxes, const FearFrameYUV* d_views, int F,
+                                        FearTarget* d_targets, int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_views || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return launch_advance_targets(d_boxes, YUVFrames{d_views}, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_frame_sums_yuv_u8(const FearFrameYUV* d_views, int F, uint64_t* d_sums, void* stream) {
+  return launch_frame_sums(d_views, YUVFrames{d_views}, F, d_sums, stream);
 }
 
 extern "C" int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,

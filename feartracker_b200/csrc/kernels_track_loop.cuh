@@ -10,9 +10,10 @@
 //
 // The three kernels are templates over where the frames are and what they hold: a packed buffer + FearFrame table
 // (PackedFrames) or a FearFrameView table of strided RGB frames anywhere in device memory (FrameViews), both read
-// through TrackFrame; or a FearFrameYUV420 table of YUV 4:2:0 frames (YUV420Frames), read through YUV420Frame, which
-// converts each pixel it reads to RGB as cv2.cvtColor does.  A frame type gives H, W, empty() and the RGB triple of
-// one pixel, rgb(y, x, p); the context box, resize tables, interpolation and sums exist once.
+// through TrackFrame; or a table of YUV 4:2:0 frames, FearFrameYUV420 (YUV420Frames, 8-bit BT.601 limited range) or
+// FearFrameYUV (YUVFrames, the format named per entry), both read through YUVFrame, which converts each pixel it reads
+// to RGB.  A frame type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize
+// tables, interpolation, sums and the colour conversion exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
 // into an FMA by default, which rounds once instead of twice, so every multiply-add here is spelled with the explicitly
@@ -57,19 +58,77 @@ __device__ __forceinline__ void yuv_to_rgb_bt601(int Y, int U, int V, int p[3]) 
   p[2] = min(max((yy + 2116026 * u) >> 20, 0), 255);
 }
 
-// A YUV 4:2:0 frame (FearFrameYUV420): luma (y, x) is Y[y * yrs + x * yps]; its chroma is sample (y >> 1, x >> 1) of
-// the U and V planes (shared strides uvrs, uvps).  rgb() converts the pixel with yuv_to_rgb_bt601, so every kernel sees
-// the RGB frame cv2.cvtColor would produce.  H and W must be even.  A value-initialised YUV420Frame{} is empty.
-struct YUV420Frame {
+// min(max(rint(255 * v), 0), 255): one channel of the H.273 conversion (rint rounds half to even).
+__device__ __forceinline__ int yuv_unit_to_u8(double v) {
+  return (int)fmin(fmax(rint(__dmul_rn(255.0, v)), 0.0), 255.0);
+}
+
+// The constants of the ITU-T H.273 inverse for one format (include/fear_b200.h, FearFrameYUV): yn = (Y - y0) * ys,
+// pb = (U - c0) * cs, pr = (V - c0) * cs, then R = yn + cR * pr, G = (yn - gB * pb) - gR * pr, B = yn + cB * pb.
+// Derived at run time from the decimal Kr, Kb with the rounded intrinsics, step by step in the documented order, so
+// neither host nor device constant folding can change a bit and image_ops.yuv420_to_rgb restates them exactly.
+struct YUVCoefs {
+  double y0, ys, c0, cs, cR, gB, gR, cB;
+};
+
+__device__ __forceinline__ YUVCoefs yuv_coefs(int matrix, bool full_range, int bits) {
+  const double Kr = matrix == FEAR_YUV_BT709 ? 0.2126 : matrix == FEAR_YUV_BT2020 ? 0.2627 : 0.299;
+  const double Kb = matrix == FEAR_YUV_BT709 ? 0.0722 : matrix == FEAR_YUV_BT2020 ? 0.0593 : 0.114;
+  const double m = (double)(1 << (bits - 8));
+  YUVCoefs k;
+  if (full_range) {
+    k.y0 = 0.0;
+    k.ys = __ddiv_rn(1.0, (double)((1 << bits) - 1));
+    k.c0 = (double)(1 << (bits - 1));
+    k.cs = k.ys;
+  } else {
+    k.y0 = 16.0 * m;  // exact: small integers
+    k.ys = __ddiv_rn(1.0, 219.0 * m);
+    k.c0 = 128.0 * m;
+    k.cs = __ddiv_rn(1.0, 224.0 * m);
+  }
+  const double Kg = __dsub_rn(__dsub_rn(1.0, Kr), Kb);
+  k.cR = __dmul_rn(2.0, __dsub_rn(1.0, Kr));
+  k.cB = __dmul_rn(2.0, __dsub_rn(1.0, Kb));
+  k.gB = __ddiv_rn(__dmul_rn(__dmul_rn(2.0, Kb), __dsub_rn(1.0, Kb)), Kg);
+  k.gR = __ddiv_rn(__dmul_rn(__dmul_rn(2.0, Kr), __dsub_rn(1.0, Kr)), Kg);
+  return k;
+}
+
+// A YUV 4:2:0 frame: luma (y, x) is the sample at Y + y * yrs + x * yps; its chroma is sample (y >> 1, x >> 1) of the
+// U and V planes (shared strides uvrs, uvps); strides in bytes.  A sample is a byte, or when `wide` a uint16 whose code
+// is (s >> shift) & (2^bits - 1).  rgb() converts the pixel with yuv_to_rgb_bt601 for the default format (BT.601,
+// limited, 8-bit), so every kernel sees the RGB frame cv2.cvtColor would produce, and with the H.273 constants k when
+// `h273`.  `bad` marks an entry the kernels cannot read (FearFrameYUV).  H and W must be even.  A value-initialised
+// YUVFrame{} is empty; its flags are those of the default format, so a source that only yields default-format frames
+// (YUV420Frames) compiles to the cv2 conversion alone.
+struct YUVFrame {
   const uint8_t *Y, *U, *V;
   long long yrs, yps, uvrs, uvps;
   int H, W;
+  int bits, shift;
+  bool wide, h273, bad;
+  YUVCoefs k;
   __device__ __forceinline__ bool empty() const {
-    return Y == nullptr || U == nullptr || V == nullptr || H < 1 || W < 1 || (H & 1) || (W & 1);
+    return bad || Y == nullptr || U == nullptr || V == nullptr || H < 1 || W < 1 || (H & 1) || (W & 1);
+  }
+  __device__ __forceinline__ int sample(const uint8_t* q) const {
+    if (!wide) return __ldg(q);
+    return (__ldg(reinterpret_cast<const uint16_t*>(q)) >> shift) & ((1 << bits) - 1);
   }
   __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
     const long long c = (long long)(y >> 1) * uvrs + (long long)(x >> 1) * uvps;
-    yuv_to_rgb_bt601(__ldg(Y + (long long)y * yrs + (long long)x * yps), __ldg(U + c), __ldg(V + c), p);
+    const int Yc = sample(Y + (long long)y * yrs + (long long)x * yps), Uc = sample(U + c), Vc = sample(V + c);
+    if (!h273) {
+      yuv_to_rgb_bt601(Yc, Uc, Vc, p);
+      return;
+    }
+    const double yn = __dmul_rn(__dsub_rn((double)Yc, k.y0), k.ys);
+    const double pb = __dmul_rn(__dsub_rn((double)Uc, k.c0), k.cs);
+    const double pr = __dmul_rn(__dsub_rn((double)Vc, k.c0), k.cs);
+    p[0] = yuv_unit_to_u8(__dadd_rn(yn, __dmul_rn(k.cR, pr)));
+    p[1] = yuv_unit_to_u8(__dsub_rn(__dsub_rn(yn, __dmul_rn(k.gB, pb)), __dmul_rn(k.gR, pr)));
+    p[2] = yuv_unit_to_u8(__dadd_rn(yn, __dmul_rn(k.cB, pb)));
   }
 };
 
@@ -92,12 +151,32 @@ struct FrameViews {
   }
 };
 
-// Frame i of a FearFrameYUV420 table (the *_yuv420 entry points).
+// Frame i of a FearFrameYUV420 table (the *_yuv420 entry points): the default format, known at compile time, so only
+// the cv2 conversion is compiled into these instantiations.
 struct YUV420Frames {
   const FearFrameYUV420* views;
-  __device__ __forceinline__ YUV420Frame operator()(int i) const {
+  __device__ __forceinline__ YUVFrame operator()(int i) const {
     const FearFrameYUV420 v = views[i];
-    return YUV420Frame{v.y, v.u, v.v, v.y_row_stride, v.y_pixel_stride, v.uv_row_stride, v.uv_pixel_stride, v.H, v.W};
+    return YUVFrame{v.y, v.u, v.v, v.y_row_stride, v.y_pixel_stride, v.uv_row_stride, v.uv_pixel_stride, v.H, v.W,
+                    8, 0, false, false, false, YUVCoefs{}};
+  }
+};
+
+// Frame i of a FearFrameYUV table (the *_yuv entry points): the format is read with the entry, checked, and its H.273
+// constants derived once per thread.
+struct YUVFrames {
+  const FearFrameYUV* views;
+  __device__ __forceinline__ YUVFrame operator()(int i) const {
+    const FearFrameYUV v = views[i];
+    const bool wide = v.bits == 10 || v.bits == 12;
+    const bool odd = ((uintptr_t)v.y | (uintptr_t)v.u | (uintptr_t)v.v | v.y_row_stride | v.y_pixel_stride |
+                      v.uv_row_stride | v.uv_pixel_stride) & 1;
+    const bool ok = v.matrix >= FEAR_YUV_BT601 && v.matrix <= FEAR_YUV_BT2020 && (v.full_range == 0 || v.full_range == 1)
+                    && (v.bits == 8 ? v.shift == 0 : wide && v.shift >= 0 && v.shift <= 16 - v.bits && !odd);
+    const bool h273 = ok && !(v.matrix == FEAR_YUV_BT601 && v.full_range == 0 && v.bits == 8);
+    return YUVFrame{static_cast<const uint8_t*>(v.y), static_cast<const uint8_t*>(v.u), static_cast<const uint8_t*>(v.v),
+                    v.y_row_stride, v.y_pixel_stride, v.uv_row_stride, v.uv_pixel_stride, v.H, v.W,
+                    v.bits, v.shift, wide, h273, !ok, h273 ? yuv_coefs(v.matrix, v.full_range, v.bits) : YUVCoefs{}};
   }
 };
 

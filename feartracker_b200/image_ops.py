@@ -148,3 +148,45 @@ def crop_resize_reference(frame: np.ndarray, params: np.ndarray, crop_size: int)
     s1 = px(y1, xo) * a0[None, :, None] + px(y1, x1) * a1[None, :, None]
     out = (((b0[:, None, None] * (s0 >> 4)) >> 16) + ((b1[:, None, None] * (s1 >> 4)) >> 16) + 2) >> 2
     return np.clip(out, 0, 255).astype(np.uint8)
+
+
+# YUV matrices of YUV420Frame / FearFrameYUV: name -> (FEAR_YUV_* id, Kr, Kb)
+YUV_MATRICES = {"bt601": (0, 0.299, 0.114), "bt709": (1, 0.2126, 0.0722), "bt2020": (2, 0.2627, 0.0593)}
+
+
+def yuv420_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601", full_range: bool = False,
+                  bits: int = 8, shift: int = 0) -> np.ndarray:
+    """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for a YUV 4:2:0 frame: luma ``y`` (H, W), chroma ``u`` (Cb)
+    and ``v`` (Cr) (H/2, W/2) of raw samples (uint8, or uint16 at 10 / 12 bits, code = (sample >> shift) &
+    (2^bits - 1)), pixel (r, c) taking chroma sample (r // 2, c // 2).  A numpy restatement of the crop kernel's
+    conversion (include/fear_b200.h, FearFrameYUV): for (bt601, limited, 8) cv2.cvtColor's fixed point, bit for bit;
+    otherwise the ITU-T H.273 inverse in float64 with the same constants, derived in the same order, each operation
+    rounded on its own, then rint (half to even) and saturation to [0, 255]."""
+    if matrix not in YUV_MATRICES:
+        raise ValueError(f"matrix must be one of {sorted(YUV_MATRICES)}, got {matrix!r}")
+    if bits not in (8, 10, 12) or not (0 <= shift <= 16 - bits) or (bits == 8 and shift):
+        raise ValueError(f"bits must be 8, 10 or 12 with 0 <= shift <= 16 - bits (0 at 8 bits), got {bits}, {shift}")
+    mask = (1 << bits) - 1
+    Y = (np.asarray(y).astype(np.int64) >> shift) & mask
+    U, V = ((np.asarray(c).astype(np.int64) >> shift) & mask for c in (u, v))
+    U, V = (c.repeat(2, 0).repeat(2, 1) for c in (U, V))
+    if matrix == "bt601" and not full_range and bits == 8:  # yuv_to_rgb_bt601
+        yy = np.maximum(Y - 16, 0) * 1220542 + (1 << 19)
+        U, V = U - 128, V - 128
+        rgb = [(yy + 1673527 * V) >> 20, (yy - 852492 * V - 409993 * U) >> 20, (yy + 2116026 * U) >> 20]
+        return np.clip(np.stack(rgb, -1), 0, 255).astype(np.uint8)
+    _, kr, kb = YUV_MATRICES[matrix]
+    m = float(1 << (bits - 8))
+    if full_range:
+        y0, ys, c0 = 0.0, 1.0 / float((1 << bits) - 1), float(1 << (bits - 1))
+        cs = ys
+    else:
+        y0, ys, c0, cs = 16.0 * m, 1.0 / (219.0 * m), 128.0 * m, 1.0 / (224.0 * m)
+    kg = (1.0 - kr) - kb
+    cr, cb = 2.0 * (1.0 - kr), 2.0 * (1.0 - kb)
+    gb, gr = 2.0 * kb * (1.0 - kb) / kg, 2.0 * kr * (1.0 - kr) / kg
+    yn = (Y.astype(np.float64) - y0) * ys
+    pb = (U.astype(np.float64) - c0) * cs
+    pr = (V.astype(np.float64) - c0) * cs
+    rgb = [yn + cr * pr, (yn - gb * pb) - gr * pr, yn + cb * pb]
+    return np.stack([np.clip(np.rint(255.0 * c), 0, 255) for c in rgb], -1).astype(np.uint8)

@@ -7,8 +7,9 @@
 
 Frames are numpy arrays in host memory, uint8 (H, W, 3) CUDA tensors already on the tracker's device, strided views
 included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y0:y1, x0:x1]), or YUV420Frames: NV12 /
-I420 planes on the device as a video decoder writes them, converted to RGB inside the crop exactly as cv2.cvtColor
-converts them.  Tensors and YUV planes are read where they are, without a copy.
+I420 planes on the device as a video decoder writes them (BT.601, BT.709 or BT.2020, limited or full range, 8-bit or
+10 / 12-bit P010 / P016 / yuv420p10le), converted to RGB inside the crop (8-bit BT.601 limited range exactly as
+cv2.cvtColor converts it).  Tensors and YUV planes are read where they are, without a copy.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -21,8 +22,8 @@ on per-target state kept in device memory (an (N, 16) int32 tensor of FearTarget
 step is captured once as a CUDA graph and replayed every frame.  The kernels find the frames through a table of
 FearFrameView records (address, byte strides, H, W) in a fixed device buffer, written before every step: numpy frames
 are packed into one pinned buffer and sent with one copy, and their views point into the packed device buffer; CUDA
-tensors' views point at the tensors.  YUV420Frames go into a second fixed table of FearFrameYUV420 records, read by the
-*_yuv420 entry points.  The host then reads back the boxes and scores.  The launch count of a step depends neither on
+tensors' views point at the tensors.  YUV420Frames go into a second fixed table of FearFrameYUV records (planes and colour
+format), read by the *_yuv entry points.  The host then reads back the boxes and scores.  The launch count of a step depends neither on
 N nor on the kind of frames.
 """
 import math
@@ -35,13 +36,13 @@ import torch
 from . import _lib, image_ops
 
 _FRAME_ALIGN = 16  # byte alignment of each frame inside the packed buffer
-_MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView and FearFrameYUV420
+_MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView and FearFrameYUV
 # the entry points that read each frame table: frame sums, target crops, box advance
 _ENTRY_POINTS = {
     "views": ("fear_frame_sums_u8", "fear_crop_targets_view_u8", "fear_advance_targets_view"),
-    "yuv": ("fear_frame_sums_yuv420_u8", "fear_crop_targets_yuv420_u8", "fear_advance_targets_yuv420"),
+    "yuv": ("fear_frame_sums_yuv_u8", "fear_crop_targets_yuv_u8", "fear_advance_targets_yuv"),
 }
-_TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV420_DTYPE}
+_TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE}
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -52,26 +53,43 @@ def frame_view(frame: torch.Tensor) -> tuple:
 
 
 class YUV420Frame:
-    """A YUV 4:2:0 frame as a video decoder writes it: 8-bit BT.601 limited range, a luma plane ``y`` (H, W) and
-    chroma planes ``u`` (Cb) and ``v`` (Cr) of (H/2, W/2), with H and W even.  Pixel (r, c) takes its chroma from
-    sample (r // 2, c // 2).  The planes are uint8 tensors or views with any non-negative strides, and ``u`` and ``v``
-    share their strides.  FEARMultiTracker reads the planes where they are and converts every pixel it reads exactly as
-    ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420)`` does, so no RGB copy of the frame is made.
+    """A YUV 4:2:0 frame as a video decoder writes it: a luma plane ``y`` (H, W) and chroma planes ``u`` (Cb) and
+    ``v`` (Cr) of (H/2, W/2), with H and W even.  Pixel (r, c) takes its chroma from sample (r // 2, c // 2).  The
+    planes are tensors or views with any non-negative strides, and ``u`` and ``v`` share their strides.
+    FEARMultiTracker reads the planes where they are and converts every pixel it reads, so no RGB copy of the frame is
+    made.
+
+    The colour format:
+        matrix       "bt601" (Kr, Kb = 0.299, 0.114), "bt709" (0.2126, 0.0722; HD H.264 / HEVC) or "bt2020"
+                     (0.2627, 0.0593, non-constant luminance; HDR / 10-bit content)
+        full_range   False: limited range (Y in [16, 235] * 2^(bits-8)); True: full range (MJPEG's yuvj420p)
+        bits         8: uint8 planes; 10 or 12: torch.uint16 planes (view byte surfaces as ``t.view(torch.uint16)``)
+        msb          at 10 / 12 bits, whether samples sit in the high bits of their uint16 (P010 / P016) rather than
+                     the low bits (yuv420p10le / yuv420p12le)
+    The default (bt601, limited, 8 bits) is converted exactly as ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 /
+    COLOR_YUV2RGB_I420)`` converts it; every other format by the ITU-T H.273 inverse in float64 (include/fear_b200.h,
+    FearFrameYUV).  ``image_ops.yuv420_to_rgb`` restates both in numpy: it gives the RGB frame the tracker sees.  Only
+    the matrix is applied: transfer functions (PQ, HLG) are not.  NV21 / YV12 are ``YUV420Frame(y, u, v)`` with the
+    planes in the right order.
 
         YUV420Frame.nv12(t)    t (3H/2, W): H luma rows, then H/2 rows of interleaved (U, V) pairs; the rows may be
-                               pitched (t = surface[:, :W]), as NVDEC and cv2 lay out NV12
+                               pitched (t = surface[:, :W]), as NVDEC and cv2 lay out NV12; at 10 / 12 bits a uint16
+                               P010 / P016 surface (MSB-aligned)
         YUV420Frame.i420(t)    t contiguous (3H/2, W): the Y, U and V planes one after another (cv2's I420, ffmpeg's
-                               yuv420p)
+                               yuv420p); at 10 / 12 bits uint16 yuv420p10le / yuv420p12le (LSB-aligned)
         YUV420Frame(y, u, v)   separate planes, regions of interest at even offsets
 
     ``shape`` is (H, W, 3), the shape of the RGB frame it stands for.  The constructors raise ValueError on a malformed
-    frame; they do not look at the device (the tracker checks that)."""
+    frame or format; they do not look at the device (the tracker checks that)."""
 
-    def __init__(self, y: torch.Tensor, u: torch.Tensor, v: torch.Tensor) -> None:
+    def __init__(self, y: torch.Tensor, u: torch.Tensor, v: torch.Tensor, *, matrix: str = "bt601",
+                 full_range: bool = False, bits: int = 8, msb: bool = False) -> None:
+        self._check_format(matrix, full_range, bits, msb)
+        dtype = self._dtype(bits)
         for name, p in (("y", y), ("u", u), ("v", v)):
-            if not isinstance(p, torch.Tensor) or p.dtype != torch.uint8 or p.ndim != 2:
+            if not isinstance(p, torch.Tensor) or p.dtype != dtype or p.ndim != 2:
                 what = f"{p.dtype} {tuple(p.shape)}" if isinstance(p, torch.Tensor) else type(p).__name__
-                raise ValueError(f"YUV420Frame plane {name} must be a 2-D uint8 tensor, got {what}")
+                raise ValueError(f"YUV420Frame plane {name} must be a 2-D {dtype} tensor at {bits} bits, got {what}")
             if min(p.stride()) < 0:
                 raise ValueError(f"YUV420Frame plane {name} has a negative stride {p.stride()}")
         h, w = y.shape
@@ -84,35 +102,71 @@ class YUV420Frame:
             raise ValueError(f"YUV420Frame u and v planes must share their strides, got {u.stride()} and {v.stride()}")
         self.y, self.u, self.v = y, u, v
         self.shape = (h, w, 3)
+        self.matrix, self.full_range, self.bits = matrix, bool(full_range), int(bits)
+        self.shift = 16 - self.bits if msb else 0
+
+    @staticmethod
+    def _check_format(matrix, full_range, bits, msb) -> None:
+        if matrix not in image_ops.YUV_MATRICES:
+            raise ValueError(f"YUV420Frame matrix must be one of {sorted(image_ops.YUV_MATRICES)}, got {matrix!r}")
+        if isinstance(bits, bool) or bits not in (8, 10, 12):
+            raise ValueError(f"YUV420Frame bits must be 8, 10 or 12, got {bits!r}")
+        if bits == 8 and msb:
+            raise ValueError("YUV420Frame msb applies to 10- and 12-bit samples, not 8-bit ones")
+
+    @staticmethod
+    def _dtype(bits: int) -> torch.dtype:
+        return torch.uint8 if bits == 8 else torch.uint16
 
     @classmethod
-    def nv12(cls, t: torch.Tensor) -> "YUV420Frame":
-        h = cls._luma_rows(t, "nv12")
+    def nv12(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV420Frame":
+        cls._check_format(matrix, full_range, bits, False)
+        h = cls._luma_rows(t, "nv12", bits)
         uv = t[h:]
-        return cls(t[:h], uv[:, 0::2], uv[:, 1::2])
+        return cls(t[:h], uv[:, 0::2], uv[:, 1::2], matrix=matrix, full_range=full_range, bits=bits, msb=bits > 8)
 
     @classmethod
-    def i420(cls, t: torch.Tensor) -> "YUV420Frame":
-        h, w = cls._luma_rows(t, "i420"), t.shape[1]
+    def i420(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV420Frame":
+        cls._check_format(matrix, full_range, bits, False)
+        h, w = cls._luma_rows(t, "i420", bits), t.shape[1]
         if not t.is_contiguous():
             raise ValueError(f"YUV420Frame.i420 takes a contiguous tensor, got strides {t.stride()}")
         flat, luma, quarter = t.reshape(-1), h * w, h * w // 4
         return cls(flat[:luma].view(h, w), flat[luma:luma + quarter].view(h // 2, w // 2),
-                   flat[luma + quarter:].view(h // 2, w // 2))
+                   flat[luma + quarter:].view(h // 2, w // 2), matrix=matrix, full_range=full_range, bits=bits)
 
-    @staticmethod
-    def _luma_rows(t, layout: str) -> int:
-        if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.ndim != 2 or t.shape[0] % 3 or t.shape[1] % 2:
+    @classmethod
+    def _luma_rows(cls, t, layout: str, bits: int = 8) -> int:
+        dtype = cls._dtype(bits)
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.ndim != 2 or t.shape[0] % 3 or t.shape[1] % 2:
             what = f"{t.dtype} {tuple(t.shape)}" if isinstance(t, torch.Tensor) else type(t).__name__
-            raise ValueError(f"YUV420Frame.{layout} takes a uint8 (3H/2, W) tensor with H and W even, got {what}")
+            raise ValueError(f"YUV420Frame.{layout} takes a {dtype} (3H/2, W) tensor with H and W even at {bits} "
+                             f"bits, got {what}")
         return 2 * t.shape[0] // 3
+
+    @property
+    def default_format(self) -> bool:
+        """Whether the frame is 8-bit BT.601 limited range, the format FearFrameYUV420 records describe."""
+        return self.matrix == "bt601" and not self.full_range and self.bits == 8
 
     def record(self) -> tuple:
         """The FearFrameYUV420 record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W):
         the addresses of luma sample (0, 0) and of the Cb and Cr samples (0, 0), and the byte strides (a uint8 stride
-        is a byte stride)."""
+        is a byte stride).  Only for the default format (8-bit BT.601 limited range); ``yuv_record`` describes any."""
+        if not self.default_format:
+            raise ValueError(f"a FearFrameYUV420 record describes 8-bit BT.601 limited range only, not this "
+                             f"{self.matrix} {'full' if self.full_range else 'limited'} range {self.bits}-bit frame: "
+                             "use yuv_record()")
+        return self.yuv_record()[:9]
+
+    def yuv_record(self) -> tuple:
+        """The FearFrameYUV record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W,
+        matrix, full_range, bits, shift): the FearFrameYUV420 fields, with byte strides (element strides times the
+        sample size), then the format."""
+        es = self.y.element_size()
         (yrs, yps), (uvrs, uvps) = self.y.stride(), self.u.stride()
-        return (self.y.data_ptr(), self.u.data_ptr(), self.v.data_ptr(), yrs, yps, uvrs, uvps, *self.shape[:2])
+        return (self.y.data_ptr(), self.u.data_ptr(), self.v.data_ptr(), yrs * es, yps * es, uvrs * es, uvps * es,
+                *self.shape[:2], image_ops.YUV_MATRICES[self.matrix][0], int(self.full_range), self.bits, self.shift)
 
 
 def _frame_kind(frame) -> str:
@@ -173,7 +227,7 @@ class FEARMultiTracker:
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
         ``frames`` are all numpy arrays, all CUDA tensors or all YUV420Frames (see ``update``).  A target's padding
-        colour is the mean colour of its frame (of the cv2-converted RGB frame for a YUV420Frame), from exact
+        colour is the mean colour of its frame (of the converted RGB frame for a YUV420Frame), from exact
         per-channel sums computed on the device."""
         frames, kind = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
@@ -252,7 +306,9 @@ class FEARMultiTracker:
         uint8 of shape (H, W, 3) on the tracker's CUDA device, with any non-negative strides: views are read as they
         are, nothing is copied.  A ``YUV420Frame``'s planes must be on the tracker's CUDA device; they are read in
         place too, and every target fed YUV420Frames gives exactly the ids, boxes and scores of the same tracker fed
-        ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420)`` as numpy arrays.  Device frames must be
+        ``image_ops.yuv420_to_rgb`` of the planes as numpy arrays (for the default format that is
+        ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420)``).  Frames of one call may have different
+        colour formats.  Device frames must be
         ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
@@ -357,7 +413,7 @@ class FEARMultiTracker:
 
     def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
         """Write the frame table of ``frames`` into the fixed device table the kernels read, and return its name:
-        "yuv" (FearFrameYUV420 records) for YUV420Frames, "views" (FearFrameView records) otherwise.  Numpy frames are
+        "yuv" (FearFrameYUV records) for YUV420Frames, "views" (FearFrameView records) otherwise.  Numpy frames are
         packed into the pinned staging buffer first and sent with one host-to-device copy (the packed layout is
         recomputed only when their shapes change); CUDA tensors and YUV planes are used where they are."""
         b, num_frames = self._buf, len(frames)
@@ -374,7 +430,7 @@ class FEARMultiTracker:
         table = b[name + "_pin"].numpy()[:nbytes].view(dtype)
         if kind == "yuv":
             for i, f in enumerate(frames):
-                table[i] = f.record()
+                table[i] = f.yuv_record()
         elif kind == "cuda":
             for i, f in enumerate(frames):
                 table[i] = frame_view(f)

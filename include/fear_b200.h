@@ -27,6 +27,10 @@
  *   fear_crop_targets_yuv420_u8 / fear_advance_targets_yuv420 / fear_frame_sums_yuv420_u8   the same three on YUV 4:2:0
  *                         frames (NV12, I420) located by FearFrameYUV420, each pixel converted to RGB exactly as
  *                         cv2.cvtColor(COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420) converts it
+ *   fear_crop_targets_yuv_u8 / fear_advance_targets_yuv / fear_frame_sums_yuv_u8   the same three on YUV 4:2:0 frames
+ *                         located by FearFrameYUV, which also names the colour format: BT.601 / BT.709 / BT.2020
+ *                         matrix, limited or full range, 8-bit or 10 / 12-bit samples in uint16 (P010, P016,
+ *                         yuv420p10le)
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -102,6 +106,36 @@ typedef struct FearFrameYUV420 {
   int64_t uv_row_stride, uv_pixel_stride;  /* bytes, >= 0, shared by u and v                                   */
   int32_t H, W;                            /* luma size, both even                                             */
 } FearFrameYUV420;
+/* A YUV 4:2:0 frame of any of the formats below: 80 bytes.  The planes are addressed as in FearFrameYUV420, with byte
+ * strides; a sample is one byte when bits == 8 and a little-endian uint16 when bits is 10 or 12, whose code is
+ * (sample >> shift) & (2^bits - 1): shift 16 - bits for MSB-aligned samples (NVDEC's P010 / P016), 0 for LSB-aligned
+ * ones (ffmpeg's yuv420p10le / yuv420p12le).  NV12-layout P010 with row pitch P bytes at address b is
+ * {b, b + H*P, b + H*P + 2, P, 2, P, 4, H, W, matrix, full_range, 10, 6}.
+ *
+ * (matrix FEAR_YUV_BT601, full_range 0, bits 8) is converted exactly as FearFrameYUV420 is (cv2.cvtColor, OpenCV's
+ * fixed point).  Every other format uses the inverse equations of ITU-T H.273 in float64, each step rounded on its own
+ * (no FMA), with Kr, Kb = 0.299, 0.114 (BT.601), 0.2126, 0.0722 (BT.709), 0.2627, 0.0593 (BT.2020 non-constant
+ * luminance), m = 2^(bits - 8):
+ *   limited: yn = (Y - 16m) * (1 / (219m));  pb = (U - 128m) * (1 / (224m));  pr = (V - 128m) * (1 / (224m))
+ *   full:    yn = Y * (1 / (2^bits - 1));  pb = (U - 2^(bits-1)) * (1 / (2^bits - 1));  pr likewise
+ *   Kg = (1 - Kr) - Kb;  cR = 2 * (1 - Kr);  cB = 2 * (1 - Kb);  gB = 2 * Kb * (1 - Kb) / Kg;  gR = 2 * Kr * (1 - Kr) / Kg
+ *   R = yn + cR * pr;  G = (yn - gB * pb) - gR * pr;  B = yn + cB * pb;  out = min(max(rint(255 * v), 0), 255)
+ * evaluated left to right, rint rounding half to even.  Codes outside the nominal range are not clamped; only the 8-bit
+ * result saturates.  Chroma is nearest (sample (y / 2, x / 2)).  Transfer functions (PQ, HLG) are not applied.
+ *
+ * An entry is treated like a frame index outside [0, F) when it has a null plane, H < 1, W < 1, an odd H or W, a matrix
+ * other than the three below, full_range other than 0 or 1, bits not 8, 10 or 12, a shift other than 0 at 8 bits or
+ * outside [0, 16 - bits] at 10 / 12 bits, or, at 10 / 12 bits, an odd plane address or an odd stride. */
+#define FEAR_YUV_BT601 0
+#define FEAR_YUV_BT709 1
+#define FEAR_YUV_BT2020 2
+typedef struct FearFrameYUV {              /* 80 bytes                                                          */
+  const void *y, *u, *v;                   /* device addresses of luma (0, 0), Cb (0, 0), Cr (0, 0)             */
+  int64_t y_row_stride, y_pixel_stride;    /* bytes, >= 0                                                       */
+  int64_t uv_row_stride, uv_pixel_stride;  /* bytes, >= 0, shared by u and v                                    */
+  int32_t H, W;                            /* luma size, both even                                              */
+  int32_t matrix, full_range, bits, shift; /* bits 8: uint8 samples, shift 0; bits 10/12: uint16, 0 <= shift <= 16-bits */
+} FearFrameYUV;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -230,6 +264,18 @@ int fear_crop_targets_yuv420_u8(const FearFrameYUV420* d_views, int F, FearTarge
 int fear_advance_targets_yuv420(const FearBox* d_boxes, const FearFrameYUV420* d_views, int F, FearTarget* d_targets,
                                 int N, int instance_size, void* stream);
 int fear_frame_sums_yuv420_u8(const FearFrameYUV420* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* The same three on YUV 4:2:0 frames of the formats FearFrameYUV describes (F entries in device memory; formats may
+ * differ between entries).  Each pixel a kernel reads is converted by the entry's format, so BT.709 NV12, P010 / P016
+ * and yuv420p10le surfaces are read where the decoder left them.  A (BT.601, limited, 8-bit) entry gives exactly what
+ * the *_yuv420 entry points give on the same planes.  Same semantics and FEAR_EINVAL rules as the *_yuv420 entry
+ * points; the table is read when the kernels run, so an entry they cannot read (see FearFrameYUV) gets a padding-colour
+ * crop, keeps its box and sums to 0. */
+int fear_crop_targets_yuv_u8(const FearFrameYUV* d_views, int F, FearTarget* d_targets, int N, double offset,
+                             int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_yuv(const FearBox* d_boxes, const FearFrameYUV* d_views, int F, FearTarget* d_targets, int N,
+                             int instance_size, void* stream);
+int fear_frame_sums_yuv_u8(const FearFrameYUV* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
