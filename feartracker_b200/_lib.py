@@ -5,7 +5,7 @@ There is no fallback: if the shared object is missing or a call fails, a Runtime
 """
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint32, c_uint64, c_void_p
 
 import numpy as np
 
@@ -80,6 +80,7 @@ _SIGNATURES = {
     "fear_corr_nhwc_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "fear_debug_backbone_prefix": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "fear_debug_head_tensor": (c_int, [c_void_p, c_char_p, c_int, c_void_p, c_void_p]),
+    "fear_debug_fill_workspace": (c_int, [c_void_p, c_uint32, c_void_p]),
     "fear_set_option": (c_int, [c_void_p, c_char_p, c_char_p]),
     "fear_launch_count": (c_int64, [c_void_p]),
     "fear_generation": (c_int64, [c_void_p]),

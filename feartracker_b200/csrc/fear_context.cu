@@ -129,6 +129,7 @@ struct FearContext {
 
   int reserved = 0;
   float* ws = nullptr;
+  int64_t ws_floats = 0;  // size of ws, slot padding included (fear_debug_fill_workspace)
   // backbone ping-pong (per frame sizes in floats)
   float *bufX = nullptr, *bufY = nullptr, *bufE = nullptr, *bufD = nullptr;
   // head
@@ -813,6 +814,7 @@ extern "C" int fear_reserve(FearContext* c, int max_batch) {
   CUDA_TRY(cudaDeviceSynchronize());
   if (c->ws) cudaFree(c->ws);
   c->ws = nullptr;
+  c->ws_floats = 0;
   c->reserved = 0;
   const int64_t per_frame[] = {
       kActX, kActX, kActE, kActD,                                   // bufX bufY bufE bufD
@@ -836,6 +838,7 @@ extern "C" int fear_reserve(FearContext* c, int max_batch) {
   if (e != cudaSuccess)
     return set_err(FEAR_ENOMEM, "workspace cudaMalloc(%lld MB) failed: %s", (long long)(total * 4 >> 20),
                    cudaGetErrorString(e));
+  c->ws_floats = total;
   float* p = c->ws;
   c->bufX = p + offs[0];
   c->bufY = p + offs[1];
@@ -1260,6 +1263,22 @@ extern "C" int fear_debug_head_tensor(FearContext* c, const char* name, int B, f
   else return set_err(FEAR_EINVAL, "unknown head tensor '%s'", name);
   return launch_transpose(c, (cudaStream_t)stream, src, ch, (long long)kScorePix * ch, d_out, kScorePix,
                           (long long)ch * kScorePix, kScorePix, ch, B);
+}
+
+// Fill every 32-bit word of the workspace (slot padding included) with `word`.  Not a LaunchScope: the fill is no
+// part of any computation, so launch and stage counts stay those of the entry points the tests count.
+__global__ void __launch_bounds__(256) fill_u32_kernel(uint32_t* __restrict__ p, long long n, uint32_t word) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    p[i] = word;
+}
+
+extern "C" int fear_debug_fill_workspace(FearContext* c, uint32_t word, void* stream) {
+  FEAR_TRY(check_ctx(c));
+  DeviceGuard guard(c->device);
+  const long long blocks = (c->ws_floats + 255) / 256;
+  fill_u32_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<uint32_t*>(c->ws), c->ws_floats, word);
+  return check_launch("fill_u32_kernel");
 }
 
 extern "C" int fear_set_option(FearContext* c, const char* key, const char* value) {

@@ -336,6 +336,11 @@ int fear_debug_backbone_prefix(FearContext* h, const float* d_img, int B, int H,
  * (B,C,16,16): "search_features" | "cat_cls" | "cat_reg" (320 ch: encode output + correlation) |
  * "cls_dw" | "reg_dw" | "x_reg" | "cls_tower" (256 ch).  (BoxTower.forward's 3rd/4th outputs.) */
 int fear_debug_head_tensor(FearContext* h, const char* name, int B, float* d_out, void* stream);
+/* Debug: write `word` into every 32-bit word of the handle's workspace (every buffer fear_reserve allocated, the
+ * padding between them included), ordered on `stream` (also while it is being captured).  Tests fill the workspace
+ * with a poison pattern before a call to show that the call reads nothing it did not write.  The weights, the launch and
+ * stage counts and fear_generation are unchanged.  FEAR_ESTATE: a null handle or one without a workspace. */
+int fear_debug_fill_workspace(FearContext* h, uint32_t word, void* stream);
 
 #ifdef __cplusplus
 }

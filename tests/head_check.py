@@ -23,7 +23,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import feartracker_b200 as fb  # noqa: E402
 from feartracker_b200 import _lib  # noqa: E402
 from oracle import fear_oracle as fo  # noqa: E402
-from tests.helpers import TOL, load_full_state, map_errors  # noqa: E402
+from tests.helpers import TOL, load_full_state, map_errors, poison_workspace  # noqa: E402
 
 R, C = fo.TARGET_REGRESSION_LABEL_KEY, fo.TARGET_CLASSIFICATION_KEY
 FEAR_EINVAL = -1
@@ -342,6 +342,7 @@ def group_options():
             bits.eq(base[0][k:k + 1], rb, f"R={R_} B={B} default frame {k} reg")
             bits.eq(base[1][k:k + 1], rc, f"R={R_} B={B} default frame {k} cls")
         net.set_option("fuse_dwpw", "13")
+        poison_workspace(net)  # each variant may not pass on values an earlier run left in the workspace
         try:
             got = head(net, z, xs, u)
         finally:
@@ -352,6 +353,7 @@ def group_options():
             for corr in ("ffma", "wgmma"):
                 net.set_option("pw", pw)
                 net.set_option("corr", corr)
+                poison_workspace(net)
                 try:
                     bbox, cls = head(net, z, xs, u)
                 finally:

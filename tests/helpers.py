@@ -7,6 +7,9 @@ import torch
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 TOL = 1e-3  # BASELINE.json north_star: maps within 1e-3 fp32 relative tolerance
+# Workspace / guard poison words (tests/poison_check.py): A is a quiet NaN with a payload no kernel emits; B is finite
+# (+16 777 218.0) and survives a ReLU, which would turn a NaN read by mistake into 0
+POISON_A, POISON_B = 0x7FA5A5A5, 0x4B800001
 
 
 def load_hotpath_state():
@@ -24,6 +27,16 @@ def load_full_state():
     for k, (shape, dtype) in keys.items():
         sd[k] = hot[k] if k in hot else torch.zeros(shape, dtype=getattr(torch, dtype))
     return sd
+
+
+def poison_workspace(net, word=POISON_B):
+    """Fill every word of the library workspace of ``net``'s handle with ``word`` (fear_debug_fill_workspace), on the
+    current stream: a later call that reads a workspace value it did not write in the same call no longer matches."""
+    from feartracker_b200 import _lib
+
+    h, lib = net._ensure_handle(next(net.parameters()).device)
+    _lib.check(lib.fear_debug_fill_workspace(h, word, torch.cuda.current_stream().cuda_stream),
+               "fear_debug_fill_workspace")
 
 
 def golden(name):

@@ -16,7 +16,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import feartracker_b200 as fb  # noqa: E402
 from oracle import fear_oracle as fo  # noqa: E402
-from tests.helpers import load_full_state, map_errors  # noqa: E402
+from tests.helpers import load_full_state, map_errors, poison_workspace  # noqa: E402
 
 BLOCK_NAMES = ["xif0_0"] + [s.name for s in fo.FBNET_C[1:fo.NUM_HOT_BLOCKS] if s.kind == "ir"]
 DEFAULTS = {"fuse_stem": "1", "fuse_irf": "1", "fuse_dwpw": "15", "dw": "auto", "pw": "auto"}
@@ -41,6 +41,7 @@ def make_net(reserve):
 
 def with_option(net, key, value, fn):
     net.set_option(key, value)
+    poison_workspace(net)  # the variant may not pass on values an earlier run left in the workspace
     try:
         return fn()
     finally:

@@ -11,7 +11,7 @@ import torch
 import feartracker_b200 as fb
 from feartracker_b200 import _lib
 from oracle import fear_oracle as fo
-from tests.helpers import GOLDEN, TOL, assert_maps_close, golden, load_full_state, map_errors
+from tests.helpers import GOLDEN, TOL, assert_maps_close, golden, load_full_state, map_errors, poison_workspace
 
 pytestmark = pytest.mark.gpu
 R, C = fo.TARGET_REGRESSION_LABEL_KEY, fo.TARGET_CLASSIFICATION_KEY
@@ -242,6 +242,7 @@ def test_depthwise_variants_are_bit_identical(net, impl):
     zf = net.get_features(zt.cuda())
     ref = net.track(xt.cuda(), zf)
     net.set_option("dw", impl)
+    poison_workspace(net)  # the variant may not pass on values the reference run left in the workspace
     try:
         zf2 = net.get_features(zt.cuda())
         out = net.track(xt.cuda(), zf2)
@@ -258,6 +259,7 @@ def test_fused_stem_block_is_bit_identical(net):
     xu8 = xu.permute(0, 2, 3, 1).contiguous().cuda()
     fused = [net.get_features(zt.cuda()), net.get_features(xt.cuda()), net.get_features(zu8), net.get_features(xu8)]
     net.set_option("fuse_stem", "0")
+    poison_workspace(net)  # the variant may not pass on values the reference run left in the workspace
     try:
         plain = [net.get_features(zt.cuda()), net.get_features(xt.cuda()), net.get_features(zu8), net.get_features(xu8)]
     finally:
@@ -277,6 +279,7 @@ def test_fused_depthwise_pointwise_is_bit_identical(net, mask):
     ref_f = net.get_features(xt.cuda())
     ref = net.track(xt.cuda(), zf)
     net.set_option("fuse_dwpw", mask)
+    poison_workspace(net)  # the variant may not pass on values the reference run left in the workspace
     try:
         got_f = net.get_features(xt.cuda())
         got = net.track(xt.cuda(), zf)
