@@ -41,6 +41,9 @@ assert YUV420_DTYPE.itemsize == 64
 YUV_DTYPE = np.dtype(YUV420_DTYPE.descr + [("matrix", "<i4"), ("full_range", "<i4"), ("bits", "<i4"),
                                            ("shift", "<i4")])
 assert YUV_DTYPE.itemsize == 80
+# FearFrameYCbCr: FearFrameYUV plus its chroma subsampling (4:2:0, 4:2:2, 4:4:4)
+YCBCR_DTYPE = np.dtype(YUV_DTYPE.descr + [("chroma_shift_x", "<i4"), ("chroma_shift_y", "<i4")])
+assert YCBCR_DTYPE.itemsize == 88
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -73,6 +76,9 @@ _SIGNATURES = {
     "fear_crop_targets_yuv_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_yuv": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_yuv_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_ycbcr_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_ycbcr": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_ycbcr_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_workspace_bytes": (c_size_t, [c_int, c_int]),

@@ -10,10 +10,11 @@
 //
 // The three kernels are templates over where the frames are and what they hold: a packed buffer + FearFrame table
 // (PackedFrames) or a FearFrameView table of strided RGB frames anywhere in device memory (FrameViews), both read
-// through TrackFrame; or a table of YUV 4:2:0 frames, FearFrameYUV420 (YUV420Frames, 8-bit BT.601 limited range) or
-// FearFrameYUV (YUVFrames, the format named per entry), both read through YUVFrame, which converts each pixel it reads
-// to RGB.  A frame type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize
-// tables, interpolation, sums and the colour conversion exist once.
+// through TrackFrame; or a table of YUV frames, FearFrameYUV420 (YUV420Frames, 4:2:0, 8-bit BT.601 limited range),
+// FearFrameYUV (YUVFrames, 4:2:0, the format named per entry) or FearFrameYCbCr (YCbCrFrames, 4:2:0, 4:2:2 or 4:4:4 and
+// the format named per entry), all read through YUVFrame, which converts each pixel it reads to RGB.  A frame type gives
+// H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables, interpolation, sums and
+// the colour conversion exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
 // into an FMA by default, which rounds once instead of twice, so every multiply-add here is spelled with the explicitly
@@ -95,29 +96,32 @@ __device__ __forceinline__ YUVCoefs yuv_coefs(int matrix, bool full_range, int b
   return k;
 }
 
-// A YUV 4:2:0 frame: luma (y, x) is the sample at Y + y * yrs + x * yps; its chroma is sample (y >> 1, x >> 1) of the
-// U and V planes (shared strides uvrs, uvps); strides in bytes.  A sample is a byte, or when `wide` a uint16 whose code
-// is (s >> shift) & (2^bits - 1).  rgb() converts the pixel with yuv_to_rgb_bt601 for the default format (BT.601,
+// A YUV frame: luma (y, x) is the sample at Y + y * yrs + x * yps; its chroma is sample (y >> csy, x >> csx) of the U
+// and V planes (shared strides uvrs, uvps); strides in bytes.  (csx, csy) is (1, 1) for 4:2:0, (1, 0) for 4:2:2 and
+// (0, 0) for 4:4:4; a subsampled side must be even.  A sample is a byte, or when `wide` a uint16 whose code is
+// (s >> shift) & (2^bits - 1).  rgb() converts the pixel with yuv_to_rgb_bt601 for the default format (BT.601,
 // limited, 8-bit), so every kernel sees the RGB frame cv2.cvtColor would produce, and with the H.273 constants k when
-// `h273`.  `bad` marks an entry the kernels cannot read (FearFrameYUV).  H and W must be even.  A value-initialised
+// `h273`.  `bad` marks an entry the kernels cannot read (FearFrameYUV, FearFrameYCbCr).  A value-initialised
 // YUVFrame{} is empty; its flags are those of the default format, so a source that only yields default-format frames
-// (YUV420Frames) compiles to the cv2 conversion alone.
+// (YUV420Frames) compiles to the cv2 conversion alone, and a source whose shifts are the constants (1, 1)
+// (YUV420Frames, YUVFrames) compiles to the 4:2:0 indexing alone.
 struct YUVFrame {
   const uint8_t *Y, *U, *V;
   long long yrs, yps, uvrs, uvps;
   int H, W;
+  int csx = 1, csy = 1;  // also those of YUVFrame{}, so a source with constant (1, 1) shifts folds them everywhere
   int bits, shift;
   bool wide, h273, bad;
   YUVCoefs k;
   __device__ __forceinline__ bool empty() const {
-    return bad || Y == nullptr || U == nullptr || V == nullptr || H < 1 || W < 1 || (H & 1) || (W & 1);
+    return bad || Y == nullptr || U == nullptr || V == nullptr || H < 1 || W < 1 || (H & csy) || (W & csx);
   }
   __device__ __forceinline__ int sample(const uint8_t* q) const {
     if (!wide) return __ldg(q);
     return (__ldg(reinterpret_cast<const uint16_t*>(q)) >> shift) & ((1 << bits) - 1);
   }
   __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
-    const long long c = (long long)(y >> 1) * uvrs + (long long)(x >> 1) * uvps;
+    const long long c = (long long)(y >> csy) * uvrs + (long long)(x >> csx) * uvps;
     const int Yc = sample(Y + (long long)y * yrs + (long long)x * yps), Uc = sample(U + c), Vc = sample(V + c);
     if (!h273) {
       yuv_to_rgb_bt601(Yc, Uc, Vc, p);
@@ -158,25 +162,44 @@ struct YUV420Frames {
   __device__ __forceinline__ YUVFrame operator()(int i) const {
     const FearFrameYUV420 v = views[i];
     return YUVFrame{v.y, v.u, v.v, v.y_row_stride, v.y_pixel_stride, v.uv_row_stride, v.uv_pixel_stride, v.H, v.W,
-                    8, 0, false, false, false, YUVCoefs{}};
+                    1, 1, 8, 0, false, false, false, YUVCoefs{}};
   }
 };
 
-// Frame i of a FearFrameYUV table (the *_yuv entry points): the format is read with the entry, checked, and its H.273
-// constants derived once per thread.
+// The YUVFrame of the FearFrameYUV or FearFrameYCbCr record at p with chroma shifts (csx, csy): the format is checked
+// and its H.273 constants derived once per thread.
+template <class Record>
+__device__ __forceinline__ YUVFrame yuv_frame_of(const Record* p, int csx, int csy) {
+  const Record v = *p;
+  const bool wide = v.bits == 10 || v.bits == 12;
+  const bool odd = ((uintptr_t)v.y | (uintptr_t)v.u | (uintptr_t)v.v | v.y_row_stride | v.y_pixel_stride |
+                    v.uv_row_stride | v.uv_pixel_stride) & 1;
+  const bool ok = v.matrix >= FEAR_YUV_BT601 && v.matrix <= FEAR_YUV_BT2020 && (v.full_range == 0 || v.full_range == 1)
+                  && (v.bits == 8 ? v.shift == 0 : wide && v.shift >= 0 && v.shift <= 16 - v.bits && !odd);
+  const bool h273 = ok && !(v.matrix == FEAR_YUV_BT601 && v.full_range == 0 && v.bits == 8);
+  return YUVFrame{static_cast<const uint8_t*>(v.y), static_cast<const uint8_t*>(v.u), static_cast<const uint8_t*>(v.v),
+                  v.y_row_stride, v.y_pixel_stride, v.uv_row_stride, v.uv_pixel_stride, v.H, v.W,
+                  csx, csy, v.bits, v.shift, wide, h273, !ok,
+                  h273 ? yuv_coefs(v.matrix, v.full_range, v.bits) : YUVCoefs{}};
+}
+
+// Frame i of a FearFrameYUV table (the *_yuv entry points): 4:2:0, the format read with the entry.
 struct YUVFrames {
   const FearFrameYUV* views;
   __device__ __forceinline__ YUVFrame operator()(int i) const {
-    const FearFrameYUV v = views[i];
-    const bool wide = v.bits == 10 || v.bits == 12;
-    const bool odd = ((uintptr_t)v.y | (uintptr_t)v.u | (uintptr_t)v.v | v.y_row_stride | v.y_pixel_stride |
-                      v.uv_row_stride | v.uv_pixel_stride) & 1;
-    const bool ok = v.matrix >= FEAR_YUV_BT601 && v.matrix <= FEAR_YUV_BT2020 && (v.full_range == 0 || v.full_range == 1)
-                    && (v.bits == 8 ? v.shift == 0 : wide && v.shift >= 0 && v.shift <= 16 - v.bits && !odd);
-    const bool h273 = ok && !(v.matrix == FEAR_YUV_BT601 && v.full_range == 0 && v.bits == 8);
-    return YUVFrame{static_cast<const uint8_t*>(v.y), static_cast<const uint8_t*>(v.u), static_cast<const uint8_t*>(v.v),
-                    v.y_row_stride, v.y_pixel_stride, v.uv_row_stride, v.uv_pixel_stride, v.H, v.W,
-                    v.bits, v.shift, wide, h273, !ok, h273 ? yuv_coefs(v.matrix, v.full_range, v.bits) : YUVCoefs{}};
+    return yuv_frame_of(views + i, 1, 1);
+  }
+};
+
+// Frame i of a FearFrameYCbCr table (the *_ycbcr entry points): 4:2:0, 4:2:2 or 4:4:4, the subsampling read with the
+// entry too.  Any other shift pair (4:4:0, negative or large shifts) is an entry the kernels cannot read.
+struct YCbCrFrames {
+  const FearFrameYCbCr* views;
+  __device__ __forceinline__ YUVFrame operator()(int i) const {
+    const int csx = views[i].chroma_shift_x, csy = views[i].chroma_shift_y;
+    YUVFrame f = yuv_frame_of(views + i, csx, csy);
+    f.bad |= !(csx == 1 ? (csy == 0 || csy == 1) : (csx == 0 && csy == 0));
+    return f;
   }
 };
 

@@ -157,19 +157,38 @@ YUV_MATRICES = {"bt601": (0, 0.299, 0.114), "bt709": (1, 0.2126, 0.0722), "bt202
 def yuv420_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601", full_range: bool = False,
                   bits: int = 8, shift: int = 0) -> np.ndarray:
     """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for a YUV 4:2:0 frame: luma ``y`` (H, W), chroma ``u`` (Cb)
-    and ``v`` (Cr) (H/2, W/2) of raw samples (uint8, or uint16 at 10 / 12 bits, code = (sample >> shift) &
-    (2^bits - 1)), pixel (r, c) taking chroma sample (r // 2, c // 2).  A numpy restatement of the crop kernel's
-    conversion (include/fear_b200.h, FearFrameYUV): for (bt601, limited, 8) cv2.cvtColor's fixed point, bit for bit;
-    otherwise the ITU-T H.273 inverse in float64 with the same constants, derived in the same order, each operation
-    rounded on its own, then rint (half to even) and saturation to [0, 255]."""
+    and ``v`` (Cr) (H/2, W/2) of raw samples, pixel (r, c) taking chroma sample (r // 2, c // 2).  ``yuv_to_rgb`` with
+    ``chroma_shift=(1, 1)``."""
+    return yuv_to_rgb(y, u, v, matrix, full_range, bits, shift, (1, 1))
+
+
+# (chroma_shift_x, chroma_shift_y) of the subsamplings FearFrameYCbCr describes: 4:2:0, 4:2:2, 4:4:4
+CHROMA_SHIFTS = ((1, 1), (1, 0), (0, 0))
+
+
+def yuv_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601", full_range: bool = False,
+               bits: int = 8, shift: int = 0, chroma_shift=(1, 1)) -> np.ndarray:
+    """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for a YUV frame: luma ``y`` (H, W), chroma ``u`` (Cb) and
+    ``v`` (Cr) of (H >> sy, W >> sx) raw samples (uint8, or uint16 at 10 / 12 bits, code = (sample >> shift) &
+    (2^bits - 1)), where ``chroma_shift`` = (sx, sy) is (1, 1) for 4:2:0, (1, 0) for 4:2:2 and (0, 0) for 4:4:4, and
+    pixel (r, c) takes chroma sample (r >> sy, c >> sx).  A numpy restatement of the crop kernel's conversion
+    (include/fear_b200.h, FearFrameYUV and FearFrameYCbCr): for (bt601, limited, 8) cv2.cvtColor's fixed point, bit for
+    bit; otherwise the ITU-T H.273 inverse in float64 with the same constants, derived in the same order, each
+    operation rounded on its own, then rint (half to even) and saturation to [0, 255]."""
     if matrix not in YUV_MATRICES:
         raise ValueError(f"matrix must be one of {sorted(YUV_MATRICES)}, got {matrix!r}")
     if bits not in (8, 10, 12) or not (0 <= shift <= 16 - bits) or (bits == 8 and shift):
         raise ValueError(f"bits must be 8, 10 or 12 with 0 <= shift <= 16 - bits (0 at 8 bits), got {bits}, {shift}")
+    sx, sy = chroma_shift
+    if (sx, sy) not in CHROMA_SHIFTS:
+        raise ValueError(f"chroma_shift must be one of {CHROMA_SHIFTS} (4:2:0, 4:2:2, 4:4:4), got {chroma_shift!r}")
     mask = (1 << bits) - 1
     Y = (np.asarray(y).astype(np.int64) >> shift) & mask
     U, V = ((np.asarray(c).astype(np.int64) >> shift) & mask for c in (u, v))
-    U, V = (c.repeat(2, 0).repeat(2, 1) for c in (U, V))
+    U, V = (c.repeat(1 << sy, 0).repeat(1 << sx, 1) for c in (U, V))
+    if U.shape != Y.shape or V.shape != Y.shape:
+        raise ValueError(f"chroma of {np.shape(u)} and {np.shape(v)} does not cover luma of {Y.shape} at chroma "
+                         f"shift {(sx, sy)}")
     if matrix == "bt601" and not full_range and bits == 8:  # yuv_to_rgb_bt601
         yy = np.maximum(Y - 16, 0) * 1220542 + (1 << 19)
         U, V = U - 128, V - 128

@@ -6,10 +6,11 @@
     trk.remove(ids); trk.reset()
 
 Frames are numpy arrays in host memory, uint8 (H, W, 3) CUDA tensors already on the tracker's device, strided views
-included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y0:y1, x0:x1]), or YUV420Frames: NV12 /
-I420 planes on the device as a video decoder writes them (BT.601, BT.709 or BT.2020, limited or full range, 8-bit or
-10 / 12-bit P010 / P016 / yuv420p10le), converted to RGB inside the crop (8-bit BT.601 limited range exactly as
-cv2.cvtColor converts it).  Tensors and YUV planes are read where they are, without a copy.
+included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y0:y1, x0:x1]), or YUV frames on the
+device as a video decoder, webcam or capture card writes them: YUV420Frame (NV12 / I420, P010 / P016 / yuv420p10le),
+YUV422Frame (YUYV / UYVY / YVYU, Y210, NV16 / P210, yuv422p) and YUV444Frame (yuv444p, NVDEC's 4:4:4 surfaces), in
+BT.601, BT.709 or BT.2020, limited or full range, 8, 10 or 12 bits, converted to RGB inside the crop (8-bit BT.601
+limited range exactly as cv2.cvtColor converts it).  Tensors and YUV planes are read where they are, without a copy.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -23,8 +24,9 @@ step is captured once as a CUDA graph and replayed every frame.  The kernels fin
 FearFrameView records (address, byte strides, H, W) in a fixed device buffer, written before every step: numpy frames
 are packed into one pinned buffer and sent with one copy, and their views point into the packed device buffer; CUDA
 tensors' views point at the tensors.  YUV420Frames go into a second fixed table of FearFrameYUV records (planes and colour
-format), read by the *_yuv entry points.  The host then reads back the boxes and scores.  The launch count of a step depends neither on
-N nor on the kind of frames.
+format), read by the *_yuv entry points; a call with any 4:2:2 or 4:4:4 frame puts all its frames into a third, of
+FearFrameYCbCr records (the same plus the chroma subsampling), read by the *_ycbcr entry points.  The host then reads
+back the boxes and scores.  The launch count of a step depends neither on N nor on the kind of frames.
 """
 import math
 import warnings
@@ -36,13 +38,14 @@ import torch
 from . import _lib, image_ops
 
 _FRAME_ALIGN = 16  # byte alignment of each frame inside the packed buffer
-_MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView and FearFrameYUV
+_MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView, FearFrameYUV and FearFrameYCbCr
 # the entry points that read each frame table: frame sums, target crops, box advance
 _ENTRY_POINTS = {
     "views": ("fear_frame_sums_u8", "fear_crop_targets_view_u8", "fear_advance_targets_view"),
     "yuv": ("fear_frame_sums_yuv_u8", "fear_crop_targets_yuv_u8", "fear_advance_targets_yuv"),
+    "ycbcr": ("fear_frame_sums_ycbcr_u8", "fear_crop_targets_ycbcr_u8", "fear_advance_targets_ycbcr"),
 }
-_TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE}
+_TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE}
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -52,7 +55,79 @@ def frame_view(frame: torch.Tensor) -> tuple:
     return (frame.data_ptr(), rs, ps, cs, frame.shape[0], frame.shape[1])
 
 
-class YUV420Frame:
+class _YUVFrame:
+    """What YUV420Frame, YUV422Frame and YUV444Frame share: three planes on the device, a colour format, the checks of
+    both, and the FearFrameYCbCr record.  ``CHROMA_SHIFT`` (x, y) is the subsampling: chroma sample
+    (r >> y, c >> x) belongs to pixel (r, c)."""
+    CHROMA_SHIFT = (1, 1)
+    _NAME = "4:2:0"
+    _SIZES = "H and W even and >= 2"  # the luma sizes the subsampling allows, for error messages
+
+    def __init__(self, y: torch.Tensor, u: torch.Tensor, v: torch.Tensor, *, matrix: str = "bt601",
+                 full_range: bool = False, bits: int = 8, msb: bool = False) -> None:
+        cls = type(self).__name__
+        self._check_format(matrix, full_range, bits, msb)
+        dtype = self._dtype(bits)
+        for name, p in (("y", y), ("u", u), ("v", v)):
+            if not isinstance(p, torch.Tensor) or p.dtype != dtype or p.ndim != 2:
+                what = f"{p.dtype} {tuple(p.shape)}" if isinstance(p, torch.Tensor) else type(p).__name__
+                raise ValueError(f"{cls} plane {name} must be a 2-D {dtype} tensor at {bits} bits, got {what}")
+            if min(p.stride()) < 0:
+                raise ValueError(f"{cls} plane {name} has a negative stride {p.stride()}")
+        h, w = y.shape
+        sx, sy = self.CHROMA_SHIFT
+        if not (1 << sy <= h <= _MAX_SIDE and 1 << sx <= w <= _MAX_SIDE) or h % (1 << sy) or w % (1 << sx):
+            raise ValueError(f"YUV {self._NAME} luma must be (H, W) with {self._SIZES}, got {tuple(y.shape)}")
+        ch, cw = h >> sy, w >> sx
+        if tuple(u.shape) != (ch, cw) or tuple(v.shape) != (ch, cw):
+            raise ValueError(f"YUV {self._NAME} chroma planes must be ({ch}, {cw}) for luma ({h}, {w}), got "
+                             f"{tuple(u.shape)} and {tuple(v.shape)}")
+        if u.stride() != v.stride():
+            raise ValueError(f"{cls} u and v planes must share their strides, got {u.stride()} and {v.stride()}")
+        self.y, self.u, self.v = y, u, v
+        self.shape = (h, w, 3)
+        self.matrix, self.full_range, self.bits = matrix, bool(full_range), int(bits)
+        self.shift = 16 - self.bits if msb else 0
+
+    @classmethod
+    def _check_format(cls, matrix, full_range, bits, msb) -> None:
+        if matrix not in image_ops.YUV_MATRICES:
+            raise ValueError(f"{cls.__name__} matrix must be one of {sorted(image_ops.YUV_MATRICES)}, got {matrix!r}")
+        if isinstance(bits, bool) or bits not in (8, 10, 12):
+            raise ValueError(f"{cls.__name__} bits must be 8, 10 or 12, got {bits!r}")
+        if bits == 8 and msb:
+            raise ValueError(f"{cls.__name__} msb applies to 10- and 12-bit samples, not 8-bit ones")
+
+    @staticmethod
+    def _dtype(bits: int) -> torch.dtype:
+        return torch.uint8 if bits == 8 else torch.uint16
+
+    @classmethod
+    def _surface(cls, t, layout: str, bits: int, rows: int, cols: int, what: str) -> None:
+        """Check that ``t`` is a 2-D tensor of the bit depth's sample type whose sides divide by ``rows``, ``cols``."""
+        dtype = cls._dtype(bits)
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.ndim != 2 or t.shape[0] % rows or t.shape[1] % cols:
+            got = f"{t.dtype} {tuple(t.shape)}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"{cls.__name__}.{layout} takes a {dtype} {what} at {bits} bits, got {got}")
+
+    @property
+    def default_format(self) -> bool:
+        """Whether the frame is 8-bit BT.601 limited range, the format FearFrameYUV420 records describe."""
+        return self.matrix == "bt601" and not self.full_range and self.bits == 8
+
+    def ycbcr_record(self) -> tuple:
+        """The FearFrameYCbCr record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W,
+        matrix, full_range, bits, shift, chroma_shift_x, chroma_shift_y): the addresses of luma sample (0, 0) and of
+        the Cb and Cr samples (0, 0), byte strides (element strides times the sample size), the format, then the
+        subsampling."""
+        es = self.y.element_size()
+        (yrs, yps), (uvrs, uvps) = self.y.stride(), self.u.stride()
+        return (self.y.data_ptr(), self.u.data_ptr(), self.v.data_ptr(), yrs * es, yps * es, uvrs * es, uvps * es,
+                *self.shape[:2], image_ops.YUV_MATRICES[self.matrix][0], int(self.full_range), self.bits, self.shift,
+                *self.CHROMA_SHIFT)
+
+
+class YUV420Frame(_YUVFrame):
     """A YUV 4:2:0 frame as a video decoder writes it: a luma plane ``y`` (H, W) and chroma planes ``u`` (Cb) and
     ``v`` (Cr) of (H/2, W/2), with H and W even.  Pixel (r, c) takes its chroma from sample (r // 2, c // 2).  The
     planes are tensors or views with any non-negative strides, and ``u`` and ``v`` share their strides.
@@ -80,43 +155,8 @@ class YUV420Frame:
         YUV420Frame(y, u, v)   separate planes, regions of interest at even offsets
 
     ``shape`` is (H, W, 3), the shape of the RGB frame it stands for.  The constructors raise ValueError on a malformed
-    frame or format; they do not look at the device (the tracker checks that)."""
-
-    def __init__(self, y: torch.Tensor, u: torch.Tensor, v: torch.Tensor, *, matrix: str = "bt601",
-                 full_range: bool = False, bits: int = 8, msb: bool = False) -> None:
-        self._check_format(matrix, full_range, bits, msb)
-        dtype = self._dtype(bits)
-        for name, p in (("y", y), ("u", u), ("v", v)):
-            if not isinstance(p, torch.Tensor) or p.dtype != dtype or p.ndim != 2:
-                what = f"{p.dtype} {tuple(p.shape)}" if isinstance(p, torch.Tensor) else type(p).__name__
-                raise ValueError(f"YUV420Frame plane {name} must be a 2-D {dtype} tensor at {bits} bits, got {what}")
-            if min(p.stride()) < 0:
-                raise ValueError(f"YUV420Frame plane {name} has a negative stride {p.stride()}")
-        h, w = y.shape
-        if not (2 <= h <= _MAX_SIDE and 2 <= w <= _MAX_SIDE) or h % 2 or w % 2:
-            raise ValueError(f"YUV 4:2:0 luma must be (H, W) with H and W even and >= 2, got {tuple(y.shape)}")
-        if tuple(u.shape) != (h // 2, w // 2) or tuple(v.shape) != (h // 2, w // 2):
-            raise ValueError(f"YUV 4:2:0 chroma planes must be ({h // 2}, {w // 2}) for luma ({h}, {w}), got "
-                             f"{tuple(u.shape)} and {tuple(v.shape)}")
-        if u.stride() != v.stride():
-            raise ValueError(f"YUV420Frame u and v planes must share their strides, got {u.stride()} and {v.stride()}")
-        self.y, self.u, self.v = y, u, v
-        self.shape = (h, w, 3)
-        self.matrix, self.full_range, self.bits = matrix, bool(full_range), int(bits)
-        self.shift = 16 - self.bits if msb else 0
-
-    @staticmethod
-    def _check_format(matrix, full_range, bits, msb) -> None:
-        if matrix not in image_ops.YUV_MATRICES:
-            raise ValueError(f"YUV420Frame matrix must be one of {sorted(image_ops.YUV_MATRICES)}, got {matrix!r}")
-        if isinstance(bits, bool) or bits not in (8, 10, 12):
-            raise ValueError(f"YUV420Frame bits must be 8, 10 or 12, got {bits!r}")
-        if bits == 8 and msb:
-            raise ValueError("YUV420Frame msb applies to 10- and 12-bit samples, not 8-bit ones")
-
-    @staticmethod
-    def _dtype(bits: int) -> torch.dtype:
-        return torch.uint8 if bits == 8 else torch.uint16
+    frame or format; they do not look at the device (the tracker checks that).  YUV422Frame and YUV444Frame take the
+    same colour formats."""
 
     @classmethod
     def nv12(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV420Frame":
@@ -137,17 +177,8 @@ class YUV420Frame:
 
     @classmethod
     def _luma_rows(cls, t, layout: str, bits: int = 8) -> int:
-        dtype = cls._dtype(bits)
-        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.ndim != 2 or t.shape[0] % 3 or t.shape[1] % 2:
-            what = f"{t.dtype} {tuple(t.shape)}" if isinstance(t, torch.Tensor) else type(t).__name__
-            raise ValueError(f"YUV420Frame.{layout} takes a {dtype} (3H/2, W) tensor with H and W even at {bits} "
-                             f"bits, got {what}")
+        cls._surface(t, layout, bits, 3, 2, "(3H/2, W) tensor with H and W even")
         return 2 * t.shape[0] // 3
-
-    @property
-    def default_format(self) -> bool:
-        """Whether the frame is 8-bit BT.601 limited range, the format FearFrameYUV420 records describe."""
-        return self.matrix == "bt601" and not self.full_range and self.bits == 8
 
     def record(self) -> tuple:
         """The FearFrameYUV420 record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W):
@@ -162,15 +193,94 @@ class YUV420Frame:
     def yuv_record(self) -> tuple:
         """The FearFrameYUV record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W,
         matrix, full_range, bits, shift): the FearFrameYUV420 fields, with byte strides (element strides times the
-        sample size), then the format."""
-        es = self.y.element_size()
-        (yrs, yps), (uvrs, uvps) = self.y.stride(), self.u.stride()
-        return (self.y.data_ptr(), self.u.data_ptr(), self.v.data_ptr(), yrs * es, yps * es, uvrs * es, uvps * es,
-                *self.shape[:2], image_ops.YUV_MATRICES[self.matrix][0], int(self.full_range), self.bits, self.shift)
+        sample size), then the format.  ``ycbcr_record`` adds the chroma shifts (1, 1)."""
+        return self.ycbcr_record()[:13]
+
+
+class YUV422Frame(_YUVFrame):
+    """A YUV 4:2:2 frame: a luma plane ``y`` (H, W) and chroma planes ``u`` (Cb) and ``v`` (Cr) of (H, W/2), W even
+    (H may be odd).  Pixel (r, c) takes its chroma from sample (r, c // 2).  Planes, strides and the colour format
+    (matrix, full_range, bits, msb) are as for YUV420Frame; ``image_ops.yuv_to_rgb(..., chroma_shift=(1, 0))`` gives
+    the RGB frame the tracker sees (for the default format, ``cv2.cvtColor(yuyv, cv2.COLOR_YUV2RGB_YUY2)``).
+
+        YUV422Frame.yuyv(t)    t (H, 2W): each row Y0 U Y1 V ... (YUY2, what UVC webcams send); rows may be pitched;
+                               at 10 / 12 bits a uint16 Y210 / Y212 / Y216 surface (MSB-aligned)
+        YUV422Frame.uyvy(t)    t (H, 2W): each row U Y0 V Y1 ... (capture cards), as yuyv otherwise
+        YUV422Frame.yvyu(t)    t (H, 2W): each row Y0 V Y1 U ..., as yuyv otherwise
+        YUV422Frame.nv16(t)    t (2H, W): H luma rows, then H rows of interleaved (U, V) pairs; rows may be pitched;
+                               at 10 / 12 bits a uint16 P210 / P216 surface (MSB-aligned)
+        YUV422Frame.i422(t)    t contiguous (2H, W): the Y, U and V planes one after another (ffmpeg's yuv422p); at
+                               10 / 12 bits uint16 yuv422p10le / yuv422p12le (LSB-aligned)
+        YUV422Frame(y, u, v)   separate planes, regions of interest at even column offsets"""
+    CHROMA_SHIFT = (1, 0)
+    _NAME = "4:2:2"
+    _SIZES = "W even and >= 2, H >= 1"
+
+    @classmethod
+    def _packed(cls, t, layout: str, order: tuple, matrix, full_range, bits) -> "YUV422Frame":
+        cls._check_format(matrix, full_range, bits, False)
+        cls._surface(t, layout, bits, 1, 4, "(H, 2W) tensor with W even")
+        y0, u0, v0 = order  # sample offsets of Y0, U and V in each 4-sample group
+        return cls(t[:, y0::2], t[:, u0::4], t[:, v0::4], matrix=matrix, full_range=full_range, bits=bits,
+                   msb=bits > 8)
+
+    @classmethod
+    def yuyv(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
+        return cls._packed(t, "yuyv", (0, 1, 3), matrix, full_range, bits)
+
+    @classmethod
+    def uyvy(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
+        return cls._packed(t, "uyvy", (1, 0, 2), matrix, full_range, bits)
+
+    @classmethod
+    def yvyu(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
+        return cls._packed(t, "yvyu", (0, 3, 1), matrix, full_range, bits)
+
+    @classmethod
+    def nv16(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
+        cls._check_format(matrix, full_range, bits, False)
+        cls._surface(t, "nv16", bits, 2, 2, "(2H, W) tensor with W even")
+        h = t.shape[0] // 2
+        uv = t[h:]
+        return cls(t[:h], uv[:, 0::2], uv[:, 1::2], matrix=matrix, full_range=full_range, bits=bits, msb=bits > 8)
+
+    @classmethod
+    def i422(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
+        cls._check_format(matrix, full_range, bits, False)
+        cls._surface(t, "i422", bits, 2, 2, "(2H, W) tensor with W even")
+        if not t.is_contiguous():
+            raise ValueError(f"YUV422Frame.i422 takes a contiguous tensor, got strides {t.stride()}")
+        h, w = t.shape[0] // 2, t.shape[1]
+        flat, luma, half = t.reshape(-1), h * w, h * w // 2
+        return cls(flat[:luma].view(h, w), flat[luma:luma + half].view(h, w // 2), flat[luma + half:].view(h, w // 2),
+                   matrix=matrix, full_range=full_range, bits=bits)
+
+
+class YUV444Frame(_YUVFrame):
+    """A YUV 4:4:4 frame: luma ``y``, chroma ``u`` (Cb) and ``v`` (Cr), three planes of the same shape (H, W), any
+    size.  Planes, strides and the colour format (matrix, full_range, bits, msb) are as for YUV420Frame;
+    ``image_ops.yuv_to_rgb(..., chroma_shift=(0, 0))`` gives the RGB frame the tracker sees.  Packed 4:4:4 layouts
+    (AYUV, Y410, Y416) are ``YUV444Frame(y, u, v)`` of strided views.
+
+        YUV444Frame.i444(t)    t (3H, W): the Y, U and V planes one after another, rows may be pitched (ffmpeg's
+                               yuv444p, NVDEC's YUV444 surfaces); at 10 / 12 bits uint16, LSB-aligned
+                               (yuv444p10le) unless ``msb=True`` (NVDEC's YUV444_16Bit surfaces)
+        YUV444Frame(y, u, v)   separate planes, regions of interest at any offset"""
+    CHROMA_SHIFT = (0, 0)
+    _NAME = "4:4:4"
+    _SIZES = "H, W >= 1"
+
+    @classmethod
+    def i444(cls, t: torch.Tensor, *, msb: bool = False, matrix: str = "bt601", full_range: bool = False,
+             bits: int = 8) -> "YUV444Frame":
+        cls._check_format(matrix, full_range, bits, msb)
+        cls._surface(t, "i444", bits, 3, 1, "(3H, W) tensor")
+        h = t.shape[0] // 3
+        return cls(t[:h], t[h:2 * h], t[2 * h:], matrix=matrix, full_range=full_range, bits=bits, msb=msb)
 
 
 def _frame_kind(frame) -> str:
-    if isinstance(frame, YUV420Frame):
+    if isinstance(frame, _YUVFrame):
         return "yuv"
     return "cuda" if isinstance(frame, torch.Tensor) else "numpy"
 
@@ -226,8 +336,9 @@ class FEARMultiTracker:
         """Start tracking ``rects`` ((n, 4) [x, y, w, h]); target i lives in stream ``streams[i]`` (default 0), whose
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
-        ``frames`` are all numpy arrays, all CUDA tensors or all YUV420Frames (see ``update``).  A target's padding
-        colour is the mean colour of its frame (of the converted RGB frame for a YUV420Frame), from exact
+        ``frames`` are all numpy arrays, all CUDA tensors or all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame;
+        see ``update``).  A target's padding colour is the mean colour of its frame (of the converted RGB frame for a
+        YUV frame), from exact
         per-channel sums computed on the device."""
         frames, kind = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
@@ -302,13 +413,14 @@ class FEARMultiTracker:
         """One frame of every stream -> the new box and score of every target, in the order of ``ids``.
 
         ``frames`` (one frame or a list of F, stream i's frame at index i) are all ``np.ndarray``, all
-        ``torch.Tensor`` or all ``YUV420Frame``; the kind may change from one call to the next.  A tensor frame is
-        uint8 of shape (H, W, 3) on the tracker's CUDA device, with any non-negative strides: views are read as they
-        are, nothing is copied.  A ``YUV420Frame``'s planes must be on the tracker's CUDA device; they are read in
-        place too, and every target fed YUV420Frames gives exactly the ids, boxes and scores of the same tracker fed
-        ``image_ops.yuv420_to_rgb`` of the planes as numpy arrays (for the default format that is
-        ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420)``).  Frames of one call may have different
-        colour formats.  Device frames must be
+        ``torch.Tensor`` or all YUV frames (``YUV420Frame``, ``YUV422Frame``, ``YUV444Frame``, mixed freely); the kind
+        may change from one call to the next.  A tensor frame is uint8 of shape (H, W, 3) on the tracker's CUDA device,
+        with any non-negative strides: views are read as they are, nothing is copied.  A YUV frame's planes must be on
+        the tracker's CUDA device; they are read in place too, and every target fed YUV frames gives exactly the ids,
+        boxes and scores of the same tracker fed ``image_ops.yuv_to_rgb`` of the planes (with the frame's
+        ``CHROMA_SHIFT``) as numpy arrays (for the default format that is ``cv2.cvtColor(frame,
+        cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420 / COLOR_YUV2RGB_YUY2 / COLOR_YUV2RGB_UYVY)``).  Frames of one call
+        may have different colour formats and subsamplings.  Device frames must be
         ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
@@ -344,15 +456,15 @@ class FEARMultiTracker:
 
     def _check_frames(self, frames):
         """-> (list of frames, their kind: "numpy", "cuda" or "yuv").  Raises ValueError before any device call."""
-        if isinstance(frames, YUV420Frame) or (isinstance(frames, (np.ndarray, torch.Tensor)) and frames.ndim == 3):
+        if isinstance(frames, _YUVFrame) or (isinstance(frames, (np.ndarray, torch.Tensor)) and frames.ndim == 3):
             frames = [frames]
         frames = list(frames)
         if not frames:
             raise ValueError("no frames given")
         kind = _frame_kind(frames[0])
         if any(_frame_kind(f) != kind for f in frames):
-            raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV420Frames, "
-                             "not a mix")
+            raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV frames "
+                             "(YUV420Frame, YUV422Frame, YUV444Frame), not a mix")
         for i, f in enumerate(frames):
             if kind == "yuv":
                 self._check_device(i, f.y, f.u, f.v)
@@ -407,17 +519,20 @@ class FEARMultiTracker:
             tcrops=torch.empty((m, tsize, tsize, 3), dtype=torch.uint8, device=dev),
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
-            frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, sums_pin=None,
-            sums=None)
+            frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, ycbcr_pin=None,
+            ycbcr=None, sums_pin=None, sums=None)
         return b
 
     def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
         """Write the frame table of ``frames`` into the fixed device table the kernels read, and return its name:
-        "yuv" (FearFrameYUV records) for YUV420Frames, "views" (FearFrameView records) otherwise.  Numpy frames are
+        "yuv" (FearFrameYUV records) when every frame is a YUV420Frame, "ycbcr" (FearFrameYCbCr records) for YUV frames
+        of which any is 4:2:2 or 4:4:4, "views" (FearFrameView records) otherwise.  Numpy frames are
         packed into the pinned staging buffer first and sent with one host-to-device copy (the packed layout is
         recomputed only when their shapes change); CUDA tensors and YUV planes are used where they are."""
         b, num_frames = self._buf, len(frames)
-        name = "yuv" if kind == "yuv" else "views"
+        name = "views"
+        if kind == "yuv":
+            name = "yuv" if all(isinstance(f, YUV420Frame) for f in frames) else "ycbcr"
         dtype = _TABLE_DTYPES[name]
         nbytes = num_frames * dtype.itemsize
         if b[name] is None or b[name].numel() < nbytes:  # grows only: the step graph keys on it
@@ -428,9 +543,12 @@ class FEARMultiTracker:
             b["sums_pin"] = torch.empty((num_frames, 3), dtype=torch.int64).pin_memory()
             b["sums"] = torch.empty((num_frames, 3), dtype=torch.int64, device=dev)
         table = b[name + "_pin"].numpy()[:nbytes].view(dtype)
-        if kind == "yuv":
+        if name == "yuv":
             for i, f in enumerate(frames):
                 table[i] = f.yuv_record()
+        elif name == "ycbcr":
+            for i, f in enumerate(frames):
+                table[i] = f.ycbcr_record()
         elif kind == "cuda":
             for i, f in enumerate(frames):
                 table[i] = frame_view(f)
@@ -471,7 +589,8 @@ class FEARMultiTracker:
     def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device) -> torch.Tensor:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
-        keyed by the target count, the frame count, which table the step reads (RGB views or YUV 4:2:0 records) and
+        keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records or YCbCr
+        records of any subsampling) and
         its buffer, and the net's generation.  ``cuda_graph=False`` in the tracking config keeps eager launches."""
         key = (n, num_frames, table, self._buf[table].data_ptr())
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):

@@ -31,6 +31,9 @@
  *                         located by FearFrameYUV, which also names the colour format: BT.601 / BT.709 / BT.2020
  *                         matrix, limited or full range, 8-bit or 10 / 12-bit samples in uint16 (P010, P016,
  *                         yuv420p10le)
+ *   fear_crop_targets_ycbcr_u8 / fear_advance_targets_ycbcr / fear_frame_sums_ycbcr_u8   the same three on YUV 4:2:0,
+ *                         4:2:2 and 4:4:4 frames located by FearFrameYCbCr (YUYV / UYVY / Y210, NV16 / P210,
+ *                         yuv422p, yuv444p, NVDEC's YUV444 surfaces), in every FearFrameYUV colour format
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -136,6 +139,33 @@ typedef struct FearFrameYUV {              /* 80 bytes                          
   int32_t H, W;                            /* luma size, both even                                              */
   int32_t matrix, full_range, bits, shift; /* bits 8: uint8 samples, shift 0; bits 10/12: uint16, 0 <= shift <= 16-bits */
 } FearFrameYUV;
+/* A YUV frame of any chroma subsampling: 88 bytes, the fields of FearFrameYUV (same meaning, same formats) followed by
+ * the chroma shifts.  The chroma of pixel (y, x) is sample (y >> chroma_shift_y, x >> chroma_shift_x) of u and v.
+ * (chroma_shift_x, chroma_shift_y) is (1, 1) for 4:2:0, (1, 0) for 4:2:2 and (0, 0) for 4:4:4; W must be even when
+ * chroma_shift_x is 1 and H when chroma_shift_y is 1, so 4:2:2 may have an odd H and 4:4:4 any size.  For a surface
+ * with row pitch P bytes at address b (fields in order; "..." is H, W, matrix, full_range, bits, shift):
+ *   YUYV (YUY2)             {b, b + 1, b + 3, P, 2, P, 4, ..., 1, 0}
+ *   UYVY                    {b + 1, b, b + 2, P, 2, P, 4, ..., 1, 0}
+ *   YVYU                    {b, b + 3, b + 1, P, 2, P, 4, ..., 1, 0}
+ *   Y210 / Y212 / Y216      {b, b + 2, b + 6, P, 4, P, 8, H, W, matrix, full_range, 10 (12), 6 (4), 1, 0}
+ *                           (YUYV order in uint16, MSB-aligned)
+ *   NV16 / P210             {b, b + H*P, b + H*P + 1 (P210: + 2), P, 1 (2), P, 2 (4), ..., 1, 0}
+ *   I422 (yuv422p)          {b, b + H*W, b + H*W + H*W/2, W, 1, W/2, 1, ..., 1, 0} (uint16 samples: offsets and
+ *                           strides x2)
+ *   I444 / NVDEC YUV444     {b, b + H*P, b + 2*H*P, P, 1, P, 1, ..., 0, 0} (16-bit surfaces: P, 2, P, 2, shift
+ *                           16 - bits)
+ *   4:2:0                   the FearFrameYUV record, then 1, 1
+ * An entry is treated like a frame index outside [0, F) when FearFrameYUV's rules refuse it (read with these shifts:
+ * an odd H only matters when chroma_shift_y is 1, an odd W when chroma_shift_x is 1), or when the shift pair is not one
+ * of the three above (4:4:0 is refused). */
+typedef struct FearFrameYCbCr {            /* 88 bytes                                                          */
+  const void *y, *u, *v;                   /* device addresses of luma (0, 0), Cb (0, 0), Cr (0, 0)             */
+  int64_t y_row_stride, y_pixel_stride;    /* bytes, >= 0                                                       */
+  int64_t uv_row_stride, uv_pixel_stride;  /* bytes, >= 0, shared by u and v                                    */
+  int32_t H, W;                            /* luma size                                                         */
+  int32_t matrix, full_range, bits, shift; /* as in FearFrameYUV                                                */
+  int32_t chroma_shift_x, chroma_shift_y;  /* (1, 1) 4:2:0, (1, 0) 4:2:2, (0, 0) 4:4:4                          */
+} FearFrameYCbCr;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -276,6 +306,17 @@ int fear_crop_targets_yuv_u8(const FearFrameYUV* d_views, int F, FearTarget* d_t
 int fear_advance_targets_yuv(const FearBox* d_boxes, const FearFrameYUV* d_views, int F, FearTarget* d_targets, int N,
                              int instance_size, void* stream);
 int fear_frame_sums_yuv_u8(const FearFrameYUV* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* The same three on YUV frames of any subsampling FearFrameYCbCr describes (F entries in device memory; layouts,
+ * subsamplings and formats may differ between entries), so YUYV webcam frames, NV16 / P210 / Y210 capture surfaces,
+ * yuv422p and 4:4:4 decoder output are read where they are.  A 4:2:0 entry gives exactly what the *_yuv entry points
+ * give on its FearFrameYUV fields.  Same semantics and FEAR_EINVAL rules as the *_yuv entry points; an entry the
+ * kernels cannot read (see FearFrameYCbCr) gets a padding-colour crop, keeps its box and sums to 0. */
+int fear_crop_targets_ycbcr_u8(const FearFrameYCbCr* d_views, int F, FearTarget* d_targets, int N, double offset,
+                               int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_ycbcr(const FearBox* d_boxes, const FearFrameYCbCr* d_views, int F, FearTarget* d_targets,
+                               int N, int instance_size, void* stream);
+int fear_frame_sums_ycbcr_u8(const FearFrameYCbCr* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
