@@ -1194,6 +1194,13 @@ extern "C" int fear_decode(const float* d_bbox, const float* d_cls, int B, int a
   return run_decode(nullptr, (cudaStream_t)stream, d_bbox, d_cls, B, apply_sigmoid, d_boxes);
 }
 
+extern "C" int fear_decode_smooth(const float* d_bbox, const float* d_cls, int B, const double* d_prev_size,
+                                  const double* d_params, FearBox* d_boxes, void* stream) {
+  if (!d_bbox || !d_cls || !d_prev_size || !d_params || !d_boxes || B < 1) return set_err(FEAR_EINVAL, "bad argument");
+  decode_smooth_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(d_bbox, d_cls, d_prev_size, d_params, d_boxes);
+  return check_launch("decode_smooth_kernel");
+}
+
 extern "C" int fear_corr_nhwc_f32(const float* d_zt, int Bz, float* d_cat, int B, void* stream) {
   if (!d_zt || !d_cat || B < 1) return set_err(FEAR_EINVAL, "bad argument");
   if (Bz != 1 && Bz != B) return set_err(FEAR_EINVAL, "template batch must be 1 or B (got %d vs %d)", Bz, B);

@@ -639,4 +639,92 @@ __global__ void __launch_bounds__(256) decode_kernel(const float* __restrict__ b
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// Smoothed box decode (FEARTracker._smooth_postprocess, reference base_tracker.py:126-205): scale / ratio
+// penalty, window re-weighting and size smoothing.  One 256-thread block per frame, one thread per score cell.
+// Every float64 step is a rounded intrinsic (no FMA contraction) in numpy's order, so the only difference from the
+// host is CUDA's double exp (within 1 ulp).  params = penalty_k, window_influence, lr, window[256].
+// ------------------------------------------------------------------------------------------
+// decode_beats on the penalised float64 score (np.argmax: the first NaN wins, ties go to the lower index).
+__device__ __forceinline__ bool smooth_beats(double ov, int oi, double v, int i) {
+  const bool onan = ov != ov, vnan = v != v;
+  if (onan || vnan) return onan && (!vnan || oi < i);
+  return ov > v || (ov == v && oi < i);
+}
+
+// np.maximum(r, 1 / r): a NaN propagates
+__device__ __forceinline__ double smooth_limit(double r) {
+  const double inv = __ddiv_rn(1.0, r);
+  return (r != r || r > inv) ? r : inv;
+}
+
+// sqrt((w + p) * (h + p)), p = (w + h) * 0.5
+__device__ __forceinline__ double smooth_sq(double w, double h) {
+  const double pad = __dmul_rn(__dadd_rn(w, h), 0.5);
+  return __dsqrt_rn(__dmul_rn(__dadd_rn(w, pad), __dadd_rn(h, pad)));
+}
+
+__global__ void __launch_bounds__(256) decode_smooth_kernel(const float* __restrict__ bbox,
+                                                            const float* __restrict__ cls,
+                                                            const double* __restrict__ prev_size,
+                                                            const double* __restrict__ params,
+                                                            FearBox* __restrict__ boxes) {
+  __shared__ double sv[8];
+  __shared__ int si[8];
+  __shared__ int win;
+  const int f = blockIdx.x, t = threadIdx.x;
+  const float score = 1.0f / (1.0f + expf(-cls[(long long)f * 256 + t]));  // decode_kernel's sigmoid
+  const int r = t >> 4, c = t & 15;
+  const double gx = (double)((c - 8) * 16 + 128), gy = (double)((r - 8) * 16 + 128);
+  const float* bb = bbox + (long long)f * 4 * 256 + t;
+  const double x1 = __dsub_rn(gx, (double)bb[0]), y1 = __dsub_rn(gy, (double)bb[256]);
+  const double x2 = __dadd_rn(gx, (double)bb[512]), y2 = __dadd_rn(gy, (double)bb[768]);
+  const double w = __dsub_rn(x2, x1), h = __dsub_rn(y2, y1);
+  const double pw = prev_size[2LL * f], ph = prev_size[2LL * f + 1];
+  const double penalty_k = params[0], wi = params[1];
+  const double s_c = smooth_limit(__ddiv_rn(smooth_sq(w, h), smooth_sq(pw, ph)));
+  const double r_c = smooth_limit(__ddiv_rn(__ddiv_rn(pw, ph), __ddiv_rn(w, h)));
+  const double penalty = exp(__dmul_rn(-__dsub_rn(__dmul_rn(r_c, s_c), 1.0), penalty_k));
+  double v = __dadd_rn(__dmul_rn(__dmul_rn(penalty, (double)score), __dsub_rn(1.0, wi)), __dmul_rn(params[3 + t], wi));
+  int i = t;
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    const double ov = __shfl_xor_sync(0xffffffffu, v, d);
+    const int oi = __shfl_xor_sync(0xffffffffu, i, d);
+    if (smooth_beats(ov, oi, v, i)) {
+      v = ov;
+      i = oi;
+    }
+  }
+  if ((t & 31) == 0) {
+    sv[t >> 5] = v;
+    si[t >> 5] = i;
+  }
+  __syncthreads();
+  if (t == 0) {
+    for (int k = 1; k < 8; ++k)
+      if (smooth_beats(sv[k], si[k], v, i)) {
+        v = sv[k];
+        i = si[k];
+      }
+    win = i;
+  }
+  __syncthreads();
+  if (t == win) {  // the thread of the winning cell holds its box, penalty and score
+    // the reference's learning rate is a float32 torch scalar: f32(f32(f32(penalty) * score) * f32(lr))
+    const double lr = (double)__fmul_rn(__fmul_rn(__double2float_rn(penalty), score), __double2float_rn(params[2]));
+    const double keep = __dsub_rn(1.0, lr), pwk = __dmul_rn(pw, keep), phk = __dmul_rn(ph, keep);
+    FearBox o;
+    o.x = x1;
+    o.y = y1;
+    o.w = __dadd_rn(pwk, __dmul_rn(lr, __dadd_rn(__dmul_rn(w, lr), pwk)));
+    o.h = __dadd_rn(phk, __dmul_rn(lr, __dadd_rn(__dmul_rn(h, lr), phk)));
+    o.score = score;
+    o.row = r;
+    o.col = c;
+    o.flat = t;
+    boxes[f] = o;
+  }
+}
+
 }  // namespace fear

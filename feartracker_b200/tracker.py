@@ -129,9 +129,11 @@ class FEARTracker(Tracker):
         """``gpu_crop=True``: the frame is uploaded once and the context crop + constant padding + bilinear resize of
         get_extended_crop (reference utils/utils.py:215-253) runs on the device (fear_crop_resize_u8, bit-identical
         to cv2's 8-bit fixed-point INTER_LINEAR) in the same CUDA graph as the network and the decode; the host only
-        computes the integer context box and the 2 x 256 resize coefficients."""
+        computes the integer context box and the 2 x 256 resize coefficients.  With ``smooth: true`` the network
+        writes its maps and fear_decode_smooth runs the penalty, window and size smoothing of _smooth_postprocess in
+        the same graph."""
         st, cfg = self.tracking_state, self.tracking_config
-        if cfg.get("smooth", False) or cfg.get("host_normalize", False) or image.shape[2] != 3:
+        if cfg.get("host_normalize", False) or image.shape[2] != 3:
             raise NotImplementedError("gpu_crop covers the default uint8 RGB tracking path (no smooth / host_normalize)")
         params, search_bbox, context = image_ops.crop_params(st.bbox, cfg["instance_size"], cfg["search_context"],
                                                              st.mean_color)
@@ -150,9 +152,13 @@ class FEARTracker(Tracker):
         dev = self._device()
         size = int(self.tracking_config["instance_size"])
         h, w = image.shape[:2]
+        cfg = self.tracking_config
+        smooth = bool(cfg.get("smooth", False))
         st = getattr(self, "_gpu_crop_state", None)
-        if st is None or st["device"] != dev or st["shape"] != (h, w) or st["params_pin"].numel() != params.size:
-            st = dict(device=dev, shape=(h, w), frame_pin=torch.empty((h, w, 3), dtype=torch.uint8).pin_memory(),
+        if st is None or st["device"] != dev or st["shape"] != (h, w) or st["params_pin"].numel() != params.size \
+                or st["smooth"] != smooth:
+            st = dict(device=dev, shape=(h, w), smooth=smooth,
+                      frame_pin=torch.empty((h, w, 3), dtype=torch.uint8).pin_memory(),
                       frame=torch.empty((h, w, 3), dtype=torch.uint8, device=dev),
                       params_pin=torch.empty(params.size, dtype=torch.int32).pin_memory(),
                       params=torch.empty(params.size, dtype=torch.int32, device=dev),
@@ -160,20 +166,39 @@ class FEARTracker(Tracker):
                       zf=torch.empty((1, 256, 8, 8), dtype=torch.float32, device=dev),
                       box_pin=torch.empty((1, 48), dtype=torch.uint8).pin_memory(),
                       graph=None, boxes=None, generation=None, zf_src=None, calls=0, graph_ok=True)
+            if smooth:
+                # fear_decode_smooth's inputs in one float64 buffer: prev_size (w, h), then its 259 params (penalty_k,
+                # window_influence, lr, window).  The five scalars are copied per update, the window once here.
+                st["smooth_pin"] = torch.empty(5, dtype=torch.float64).pin_memory()
+                st["smooth_in"] = torch.empty(5 + 256, dtype=torch.float64, device=dev)
+                st["smooth_in"][5:].copy_(torch.from_numpy(np.asarray(self.window, dtype=np.float64).reshape(256)))
+                st["smooth_boxes"] = torch.empty((1, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8, device=dev)
             self._gpu_crop_state = st
         np.copyto(st["frame_pin"].numpy(), image)
         np.copyto(st["params_pin"].numpy(), params)
         st["frame"].copy_(st["frame_pin"], non_blocking=True)
         st["params"].copy_(st["params_pin"], non_blocking=True)
+        if smooth:
+            pw, ph = self.tracking_state.prev_size
+            st["smooth_pin"].numpy()[:] = (pw, ph, cfg["penalty_k"], cfg["window_influence"], cfg["lr"])
+            st["smooth_in"][:5].copy_(st["smooth_pin"], non_blocking=True)
         if st["zf_src"] is not self._template_features:
             st["zf"].copy_(self._template_features)
             st["zf_src"] = self._template_features
         lib = _lib.load()
 
         def step():
+            stream = torch.cuda.current_stream(dev).cuda_stream
             _lib.check(lib.fear_crop_resize_u8(st["frame"].data_ptr(), h, w, st["params"].data_ptr(), st["crop"].data_ptr(),
-                                               size, torch.cuda.current_stream(dev).cuda_stream), "fear_crop_resize_u8")
-            return self.net.track_boxes(st["crop"], st["zf"])
+                                               size, stream), "fear_crop_resize_u8")
+            if not smooth:
+                return self.net.track_boxes(st["crop"], st["zf"])
+            maps = self.net.track(st["crop"], st["zf"])  # maps only: the plain decode is skipped
+            sp = st["smooth_in"].data_ptr()
+            _lib.check(lib.fear_decode_smooth(maps[TARGET_REGRESSION_LABEL_KEY].data_ptr(),
+                                              maps[TARGET_CLASSIFICATION_KEY].data_ptr(), 1, sp, sp + 16,
+                                              st["smooth_boxes"].data_ptr(), stream), "fear_decode_smooth")
+            return st["smooth_boxes"]
 
         use_graph = self.tracking_config.get("cuda_graph", True) and st["graph_ok"]
         if st["graph"] is not None and st["generation"] != self.net.generation():

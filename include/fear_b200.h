@@ -14,6 +14,8 @@
  *   fear_corr_concat_f32  MobileCorrelation.forward front half (matmul + cat)  blocks.py:121-124
  *   fear_corr_nhwc_f32    same contraction on the library's internal channels-last layout
  *   fear_decode           FEARBoxCoder.decode                 dataset/box_coder.py:75-107
+ *   fear_decode_smooth    FEARTracker._postprocess with smooth: true (penalty, window, size smoothing)
+ *                         tracker/base_tracker.py:126-205
  *   fear_pack_weights     load_from_lighting + nn.Module.load_state_dict  utils/torch.py:11-24
  *
  *   fear_head_update      BoxTower.forward(search, kernel, update)   blocks.py:174-179
@@ -324,6 +326,22 @@ int fear_frame_sums_ycbcr_u8(const FearFrameYCbCr* d_views, int F, uint64_t* d_s
  * first NaN wins), so -0.0 and 0.0 tie and +inf beats every finite score. */
 int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,
                 void* stream);
+
+/* FEARTracker._postprocess with smooth: true (base_tracker.py:126-205) for B frames.  d_bbox (B,4,16,16),
+ * d_cls (B,1,16,16) logits as fear_track writes them; d_prev_size (B,2) float64: TrackingState.prev_size
+ * (target w, h in search-crop pixels); d_params (259) float64: penalty_k, window_influence, lr, then the
+ * 16x16 window row-major.  All in device memory, so a captured graph sees per-frame values.
+ * Per cell, in float64 with every step rounded (no FMA): score = sigmoid(cls) in float32 as fear_decode computes it;
+ * x1, y1, x2, y2 = grid -/+ distances; penalty = exp(-(limit(r_c) * limit(s_c) - 1) * penalty_k) with
+ * s_c = sq(x2 - x1, y2 - y1) / sq(pw, ph), r_c = (pw / ph) / ((x2 - x1) / (y2 - y1)), sq(w, h) = sqrt((w + p) (h + p)),
+ * p = (w + h) / 2, limit(r) = max(r, 1 / r); pscore = (penalty * score) * (1 - window_influence) + window *
+ * window_influence.  The argmax of pscore follows fear_decode's rules (first NaN, then first maximum).  The record
+ * holds that cell's x1, y1, its float32 score and (row, col, flat); w, h are the smoothed size
+ * pw * (1 - l) + l * (bw * l + pw * (1 - l)) with l = f32(f32(f32(penalty) * score) * f32(lr)), the float32
+ * learning rate of the reference.  Only exp may differ from numpy (by 1 ulp).  Handle-free: it never allocates and
+ * never synchronises.  FEAR_EINVAL: a null pointer or B < 1; device data is not validated. */
+int fear_decode_smooth(const float* d_bbox, const float* d_cls, int B, const double* d_prev_size,
+                       const double* d_params, FearBox* d_boxes, void* stream);
 
 /* z (Bz,256,64), x (B,256,256)  [= (B,256,16,16)]  ->  out (B,320,256):
  * out[:, :256] = x ; out[b, 256+k, p] = sum_c z[b,c,k] * x[b,c,p].   (blocks.py:121-124)
