@@ -111,20 +111,33 @@ def resize_tables(src_w: int, src_h: int, dst: int) -> np.ndarray:
     return np.concatenate(_axis_table(src_w, dst, True) + _axis_table(src_h, dst, False)).astype(np.int32)
 
 
-def crop_params(bbox: Sequence[float], crop_size: int, offset: float, padding_value: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
-    """Parameter block of fear_crop_resize_u8 for the context crop around ``bbox`` plus the two values
-    ``extended_crop`` returns besides the image: the box inside the crop and the context box."""
+def crop_geometry(bbox: Sequence[float], crop_size: int, offset: float) -> Tuple[np.ndarray, np.ndarray]:
+    """The two values ``extended_crop`` returns besides the image, without making the crop: the box inside the
+    ``crop_size`` crop and the context box in frame coordinates."""
     ctx = context_box(bbox, offset)
     cols, rows = int(ctx[2]), int(ctx[3])
     box = trim_box([bbox[0] - ctx[0], bbox[1] - ctx[1], bbox[2], bbox[3]], (rows, cols))
     if box[2] * box[3] == 0:
         raise IndexError("target box has zero area inside its context crop")
-    pad = np.clip(np.rint(np.asarray(padding_value, dtype=np.float64)), 0, 255).astype(np.int32)  # cv::saturate_cast
-    head = np.array([ctx[0], ctx[1], cols, rows, pad[0], pad[1], pad[2], 0], dtype=np.int32)
-    params = np.concatenate([head, resize_tables(cols, rows, crop_size)])
     x0, y0 = float(box[0]) / cols * crop_size, float(box[1]) / rows * crop_size
     x1, y1 = float(box[0] + box[2]) / cols * crop_size, float(box[1] + box[3]) / rows * crop_size
-    return params, np.array([x0, y0, x1 - x0, y1 - y0]), ctx
+    return np.array([x0, y0, x1 - x0, y1 - y0]), ctx
+
+
+def padding_color(mean_color: np.ndarray) -> np.ndarray:
+    """The int32 padding colour of a crop, cv::saturate_cast of the frame's mean colour, as copyMakeBorder takes it."""
+    return np.clip(np.rint(np.asarray(mean_color, dtype=np.float64)), 0, 255).astype(np.int32)
+
+
+def crop_params(bbox: Sequence[float], crop_size: int, offset: float, padding_value: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Parameter block of fear_crop_resize_u8 for the context crop around ``bbox`` plus the two values
+    ``extended_crop`` returns besides the image: the box inside the crop and the context box."""
+    search_bbox, ctx = crop_geometry(bbox, crop_size, offset)
+    cols, rows = int(ctx[2]), int(ctx[3])
+    pad = padding_color(padding_value)
+    head = np.array([ctx[0], ctx[1], cols, rows, pad[0], pad[1], pad[2], 0], dtype=np.int32)
+    params = np.concatenate([head, resize_tables(cols, rows, crop_size)])
+    return params, search_bbox, ctx
 
 
 def crop_resize_reference(frame: np.ndarray, params: np.ndarray, crop_size: int) -> np.ndarray:

@@ -40,12 +40,12 @@ from . import _lib, image_ops
 _FRAME_ALIGN = 16  # byte alignment of each frame inside the packed buffer
 _MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView, FearFrameYUV and FearFrameYCbCr
 # the entry points that read each frame table: frame sums, target crops, box advance
-_ENTRY_POINTS = {
+ENTRY_POINTS = {
     "views": ("fear_frame_sums_u8", "fear_crop_targets_view_u8", "fear_advance_targets_view"),
     "yuv": ("fear_frame_sums_yuv_u8", "fear_crop_targets_yuv_u8", "fear_advance_targets_yuv"),
     "ycbcr": ("fear_frame_sums_ycbcr_u8", "fear_crop_targets_ycbcr_u8", "fear_advance_targets_ycbcr"),
 }
-_TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE}
+TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE}
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -279,10 +279,54 @@ class YUV444Frame(_YUVFrame):
         return cls(t[:h], t[h:2 * h], t[2 * h:], matrix=matrix, full_range=full_range, bits=bits, msb=msb)
 
 
-def _frame_kind(frame) -> str:
+def frame_kind(frame) -> str:
+    """"yuv" for a YUV420Frame, YUV422Frame or YUV444Frame, "cuda" for a torch tensor (checked by
+    ``check_device_frame``), "numpy" for anything else."""
     if isinstance(frame, _YUVFrame):
         return "yuv"
     return "cuda" if isinstance(frame, torch.Tensor) else "numpy"
+
+
+def check_device(i: int, device, *tensors: torch.Tensor) -> None:
+    """ValueError unless every tensor is on the tracker's CUDA device; ``device()`` gives that device and is called
+    only once a tensor is known to be on some CUDA device."""
+    for t in tensors:
+        if t.device.type != "cuda":
+            raise ValueError(f"frame {i} is in a {t.device} tensor: tensor frames and YUV planes must be on the "
+                             "tracker's CUDA device (pass host frames as numpy arrays)")
+        dev = device()
+        if t.device != dev:
+            raise ValueError(f"frame {i} is on {t.device}, the tracker on {dev}")
+
+
+def check_tensor_frame(i: int, f: torch.Tensor, device) -> None:
+    """ValueError unless ``f`` is a uint8 (H, W, 3) tensor with non-negative strides on the tracker's device."""
+    if f.dtype != torch.uint8 or f.ndim != 3 or f.shape[2] != 3 or not (1 <= f.shape[0] <= _MAX_SIDE) \
+            or not (1 <= f.shape[1] <= _MAX_SIDE):
+        raise ValueError(f"frame {i} must be a uint8 HxWx3 RGB tensor, got {f.dtype} {tuple(f.shape)}")
+    if min(f.stride()) < 0:
+        raise ValueError(f"frame {i} has a negative stride {f.stride()}")
+    check_device(i, device, f)
+
+
+def check_device_frame(i: int, f, kind: str, device) -> None:
+    """The checks of a frame of kind "cuda" or "yuv" (``frame_kind``): ValueError before any device call."""
+    if kind == "yuv":
+        check_device(i, device, f.y, f.u, f.v)
+    else:
+        check_tensor_frame(i, f, device)
+
+
+def write_records(table: np.ndarray, frames, name: str) -> None:
+    """Write the records of device frames into rows of ``table`` (a numpy view of ``TABLE_DTYPES[name]``):
+    FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr"."""
+    for i, f in enumerate(frames):
+        if name == "yuv":
+            table[i] = f.yuv_record()
+        elif name == "ycbcr":
+            table[i] = f.ycbcr_record()
+        else:
+            table[i] = frame_view(f)
 
 
 class FEARMultiTracker:
@@ -367,7 +411,7 @@ class FEARMultiTracker:
             b = self._buffers(dev)
             num_frames = len(frames)
             table = self._upload_frames(frames, kind, dev)
-            sums_fn, crop_fn, _ = _ENTRY_POINTS[table]
+            sums_fn, crop_fn, _ = ENTRY_POINTS[table]
             lib = _lib.load()
             stream = torch.cuda.current_stream(dev)
             _lib.check(getattr(lib, sums_fn)(b[table].data_ptr(), num_frames, b["sums"].data_ptr(), stream.cuda_stream),
@@ -461,37 +505,18 @@ class FEARMultiTracker:
         frames = list(frames)
         if not frames:
             raise ValueError("no frames given")
-        kind = _frame_kind(frames[0])
-        if any(_frame_kind(f) != kind for f in frames):
+        kind = frame_kind(frames[0])
+        if any(frame_kind(f) != kind for f in frames):
             raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV frames "
                              "(YUV420Frame, YUV422Frame, YUV444Frame), not a mix")
         for i, f in enumerate(frames):
-            if kind == "yuv":
-                self._check_device(i, f.y, f.u, f.v)
-            elif kind == "cuda":
-                self._check_tensor_frame(i, f)
+            if kind != "numpy":
+                check_device_frame(i, f, kind, self._device)
             elif not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
                     or f.shape[0] < 1 or f.shape[1] < 1:
                 what = f"{f.dtype} {f.shape}" if isinstance(f, np.ndarray) else type(f).__name__
                 raise ValueError(f"frame {i} must be a uint8 HxWx3 RGB array, got {what}")
         return frames, kind
-
-    def _check_tensor_frame(self, i: int, f: torch.Tensor) -> None:
-        if f.dtype != torch.uint8 or f.ndim != 3 or f.shape[2] != 3 or not (1 <= f.shape[0] <= _MAX_SIDE) \
-                or not (1 <= f.shape[1] <= _MAX_SIDE):
-            raise ValueError(f"frame {i} must be a uint8 HxWx3 RGB tensor, got {f.dtype} {tuple(f.shape)}")
-        if min(f.stride()) < 0:
-            raise ValueError(f"frame {i} has a negative stride {f.stride()}")
-        self._check_device(i, f)
-
-    def _check_device(self, i: int, *tensors: torch.Tensor) -> None:
-        for t in tensors:
-            if t.device.type != "cuda":
-                raise ValueError(f"frame {i} is in a {t.device} tensor: tensor frames and YUV planes must be on the "
-                                 "tracker's CUDA device (pass host frames as numpy arrays)")
-            dev = self._device()
-            if t.device != dev:
-                raise ValueError(f"frame {i} is on {t.device}, the tracker on {dev}")
 
     @staticmethod
     def _check_streams(streams, n: int, num_frames: int) -> np.ndarray:
@@ -533,7 +558,7 @@ class FEARMultiTracker:
         name = "views"
         if kind == "yuv":
             name = "yuv" if all(isinstance(f, YUV420Frame) for f in frames) else "ycbcr"
-        dtype = _TABLE_DTYPES[name]
+        dtype = TABLE_DTYPES[name]
         nbytes = num_frames * dtype.itemsize
         if b[name] is None or b[name].numel() < nbytes:  # grows only: the step graph keys on it
             b[name + "_pin"] = torch.empty(nbytes, dtype=torch.uint8).pin_memory()
@@ -543,15 +568,8 @@ class FEARMultiTracker:
             b["sums_pin"] = torch.empty((num_frames, 3), dtype=torch.int64).pin_memory()
             b["sums"] = torch.empty((num_frames, 3), dtype=torch.int64, device=dev)
         table = b[name + "_pin"].numpy()[:nbytes].view(dtype)
-        if name == "yuv":
-            for i, f in enumerate(frames):
-                table[i] = f.yuv_record()
-        elif name == "ycbcr":
-            for i, f in enumerate(frames):
-                table[i] = f.ycbcr_record()
-        elif kind == "cuda":
-            for i, f in enumerate(frames):
-                table[i] = frame_view(f)
+        if kind != "numpy":
+            write_records(table, frames, name)
         else:
             key = tuple(f.shape for f in frames)
             if key != self._frames_key:
@@ -576,7 +594,7 @@ class FEARMultiTracker:
 
     def _step(self, n: int, num_frames: int, dev: torch.device, table: str = "views") -> torch.Tensor:
         b, cfg, lib = self._buf, self.tracking_config, _lib.load()
-        _, crop_fn, advance_fn = _ENTRY_POINTS[table]
+        _, crop_fn, advance_fn = ENTRY_POINTS[table]
         size = int(cfg["instance_size"])
         s = torch.cuda.current_stream(dev).cuda_stream
         _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b["state"].data_ptr(), n,

@@ -5,7 +5,12 @@ API mirror of reference model_training/tracker/base_tracker.py:28-124 and fear_t
 ``update(image) -> {"bbox": [x, y, w, h]}``, ``track(search_crop)``, ``get_template_features``,
 ``to_device``, ``reset``.  Cropping / normalisation stay on the host (cv2 fixed-point resize is part
 of the reference's observable behaviour); network + decode run in libfear_b200 and only the
-48-byte box record comes back per frame.
+48-byte box record comes back per frame.  With ``gpu_crop: true`` the numpy frame is uploaded and cropped on the device.
+
+Frames already in GPU memory -- uint8 (H, W, 3) CUDA tensors with any non-negative strides, and YUV420Frame /
+YUV422Frame / YUV444Frame decoder surfaces -- are read in place: the crop, the conversion to RGB, the network and the
+decode (plain or smoothed) run on the device, and the tracker returns exactly what it returns for the same pixels as a
+numpy array (``image_ops.yuv_to_rgb`` of a YUV frame's planes).
 """
 from collections import deque
 from typing import Any, Dict, Optional, Tuple, Union
@@ -14,9 +19,16 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import image_ops
+from . import image_ops, multi_tracker
 from .box_coder import FEARBoxCoder, TrackerDecodeResult
 from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY
+
+
+# byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCr), a FearTarget,
+# then five float64 inputs of fear_decode_smooth
+_TARGET_OFFSET = 88
+_SMOOTH_OFFSET = _TARGET_OFFSET + 64
+_DEVICE_INPUT_BYTES = _SMOOTH_OFFSET + 5 * 8
 
 
 class TrackingState:
@@ -94,25 +106,52 @@ class Tracker:
 
 
 class FEARTracker(Tracker):
+    """The reference's single-object tracker.  ``initialize``, ``update`` and ``get_template_features`` take a frame as
+    a uint8 (H, W, 3) RGB numpy array, as a uint8 (H, W, 3) CUDA tensor on the tracker's device (any non-negative
+    strides: ``rgba[..., :3]``, ``chw.permute(1, 2, 0)``, a region of interest), or as a YUV420Frame, YUV422Frame or
+    YUV444Frame whose planes are on the tracker's device; the kind may change from one call to the next.
+
+    Numpy frames take the host crop, or with ``gpu_crop: true`` an upload and the device crop.  Device frames always
+    take the device step, whatever ``gpu_crop`` says, since the host crop could only read them after copying them back:
+    fear_crop_targets_view_u8 (tensors) or fear_crop_targets_ycbcr_u8 (YUV frames, converted to RGB inside the crop)
+    makes the search crop, then the network and the decode, plain or with ``smooth: true`` the smoothed one, run as one
+    CUDA graph and one 48-byte record comes back.  The results, ``tracking_state`` included, are those of the same
+    tracker fed the same pixels as numpy arrays (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its
+    ``CHROMA_SHIFT``).  Device frames must be ready on the current CUDA stream; every call synchronises it before it
+    returns, so they only need to live for the call.  ``host_normalize: true`` takes numpy frames only."""
+
     def get_box_coder(self, tracking_config, cuda_id: int = 0):
         return FEARBoxCoder(tracker_config=tracking_config)
 
     def initialize(self, image: np.ndarray, rect: np.ndarray, **kwargs) -> None:
-        """image: RGB uint8 HxWx3; rect: [x, y, w, h], 0-based."""
+        """image: RGB uint8 HxWx3 (or a device frame, see the class docstring); rect: [x, y, w, h], 0-based."""
+        kind = self._frame_kind(image)
         rect = image_ops.clamp_bbox(rect, image.shape)
         st = self.tracking_state
+        if kind != "numpy":
+            mean_color = self._device_mean_color(image, kind)
+            features = self._device_template_features(image, kind, rect, mean_color)
+            st.bbox, st.paths, st.mean_color = rect, deque([rect], maxlen=10), mean_color
+            self._template_features = features
+            return
         st.bbox = rect
         st.paths = deque([rect], maxlen=10)
         st.mean_color = np.mean(image, axis=(0, 1))
         self._template_features = self.get_template_features(image, rect)
 
     def get_template_features(self, image: np.ndarray, rect: np.ndarray) -> torch.Tensor:
+        kind = self._frame_kind(image)
+        if kind != "numpy":
+            return self._device_template_features(image, kind, rect, self._device_mean_color(image, kind))
         crop, _, _ = image_ops.extended_crop(image, rect, self.tracking_config["template_size"],
                                              self.tracking_config["template_bbox_offset"])
         return self.net.get_features(self._preprocess_image(crop))
 
     def update(self, image: np.ndarray, *kw) -> Dict[str, Any]:
         st, cfg = self.tracking_state, self.tracking_config
+        kind = self._frame_kind(image)
+        if kind != "numpy":
+            return self._update_device_frame(image, kind)
         if cfg.get("gpu_crop", False):
             return self._update_gpu_crop(image)
         crop, search_bbox, context = image_ops.extended_crop(image, st.bbox, cfg["instance_size"],
@@ -223,6 +262,180 @@ class FEARTracker(Tracker):
         st["calls"] += 1
         st["box_pin"].copy_(boxes, non_blocking=True)
         torch.cuda.current_stream(dev).synchronize()
+        return st["box_pin"].numpy().view(_lib.BOX_DTYPE).reshape(-1)[0].copy()
+
+    # -- device frames: CUDA tensors and YUV frames, read in place by the crop-targets entry points (one target) --
+    def _frame_kind(self, image) -> str:
+        """"numpy", "cuda" or "yuv" (multi_tracker.frame_kind).  A device frame is checked here, before any device call
+        or state change: NotImplementedError with ``host_normalize``, ValueError when malformed."""
+        kind = multi_tracker.frame_kind(image)
+        if kind == "numpy":
+            return kind
+        if self.tracking_config.get("host_normalize", False):
+            raise NotImplementedError("host_normalize normalises numpy crops on the host; device frames (CUDA tensors, "
+                                      "YUV frames) are normalised on the device: drop host_normalize to track on them")
+        multi_tracker.check_device_frame(0, image, kind, self._device)
+        return kind
+
+    def _device_frame_state(self) -> dict:
+        """Buffers of the device-frame step, separate from the gpu_crop path's.  ``inputs`` (pinned) and ``dev_in``
+        share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView or a
+        FearFrameYCbCr) at byte 0, the FearTarget at byte 88, fear_decode_smooth's prev_size (w, h), penalty_k,
+        window_influence and lr as float64 at byte 152; then, on the device only, the 16 x 16 window."""
+        from . import _lib
+
+        dev = self._device()
+        smooth = bool(self.tracking_config.get("smooth", False))
+        st = getattr(self, "_device_state", None)
+        if st is not None and st["device"] == dev and st["smooth"] == smooth:
+            return st
+        size, tsize = int(self.tracking_config["instance_size"]), int(self.tracking_config["template_size"])
+        st = dict(device=dev, smooth=smooth,
+                  inputs=torch.zeros(_DEVICE_INPUT_BYTES, dtype=torch.uint8).pin_memory(),
+                  dev_in=torch.zeros(_DEVICE_INPUT_BYTES + 256 * 8, dtype=torch.uint8, device=dev),
+                  crop=torch.empty((1, size, size, 3), dtype=torch.uint8, device=dev),
+                  tcrop=torch.empty((1, tsize, tsize, 3), dtype=torch.uint8, device=dev),
+                  sums=torch.empty((1, 3), dtype=torch.int64, device=dev),
+                  sums_pin=torch.empty((1, 3), dtype=torch.int64).pin_memory(),
+                  zf=torch.empty((1, 256, 8, 8), dtype=torch.float32, device=dev),
+                  smooth_boxes=torch.empty((1, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8, device=dev),
+                  box_pin=torch.empty((1, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
+                  graph=None, boxes=None, key=None, zf_src=None, calls=0, graph_ok=True)
+        window = np.asarray(self.window, dtype=np.float64).reshape(256)
+        st["dev_in"][_DEVICE_INPUT_BYTES:].copy_(torch.from_numpy(window).view(torch.uint8))
+        self._device_state = st
+        return st
+
+    def _stage_device_inputs(self, st: dict, image, kind: str, bbox, pad, prev_size=None) -> str:
+        """Write the frame's record, the target (frame 0, ``bbox``, padding colour ``pad``) and, given ``prev_size``,
+        the smooth scalars into the pinned inputs and send them with one host-to-device copy.  Returns the table name:
+        "views" for a tensor, "ycbcr" for every YUV frame."""
+        table = "ycbcr" if kind == "yuv" else "views"
+        raw, dtype = st["inputs"].numpy(), multi_tracker.TABLE_DTYPES[table]
+        multi_tracker.write_records(raw[:dtype.itemsize].view(dtype), [image], table)
+        target = raw[_TARGET_OFFSET:_SMOOTH_OFFSET].view(np.int32)
+        target[:] = 0
+        target[1:5] = bbox
+        target[9:12] = pad
+        if prev_size is not None:
+            cfg = self.tracking_config
+            raw[_SMOOTH_OFFSET:].view(np.float64)[:] = (prev_size[0], prev_size[1], cfg["penalty_k"],
+                                                        cfg["window_influence"], cfg["lr"])
+        st["dev_in"][:_DEVICE_INPUT_BYTES].copy_(st["inputs"], non_blocking=True)
+        return table
+
+    def _device_mean_color(self, image, kind: str) -> np.ndarray:
+        """np.mean(frame, axis=(0, 1)) of the RGB frame, bit for bit: exact per-channel sums on the device over H * W."""
+        from . import _lib
+
+        st = self._device_frame_state()
+        dev = st["device"]
+        with torch.cuda.device(dev):
+            table = self._stage_device_inputs(st, image, kind, (0, 0, 0, 0), (0, 0, 0))
+            sums_fn = multi_tracker.ENTRY_POINTS[table][0]
+            stream = torch.cuda.current_stream(dev)
+            _lib.check(getattr(_lib.load(), sums_fn)(st["dev_in"].data_ptr(), 1, st["sums"].data_ptr(),
+                                                     stream.cuda_stream), sums_fn)
+            st["sums_pin"].copy_(st["sums"], non_blocking=True)
+            stream.synchronize()
+        h, w = image.shape[:2]
+        return st["sums_pin"].numpy()[0].view(np.uint64).astype(np.float64) / (h * w)
+
+    def _device_template_features(self, image, kind: str, rect, mean_color) -> torch.Tensor:
+        """The template of get_template_features: the 128 x 128 context crop (offset template_bbox_offset) made by the
+        crop-targets entry point on a one-row FearTarget, then net.get_features on the uint8 crop."""
+        from . import _lib
+
+        cfg = self.tracking_config
+        size, offset = int(cfg["template_size"]), float(cfg["template_bbox_offset"])
+        box = np.asarray(rect, dtype=np.float64)
+        if box.shape != (4,) or not np.array_equal(box, np.trunc(box)) or np.abs(box).max() > 2 ** 31 - 1:
+            raise ValueError(f"a device frame's template box must be 4 integers [x, y, w, h], got {rect!r}")
+        image_ops.crop_geometry(box, size, offset)  # the IndexError of a zero-area box, as extended_crop raises it
+        st = self._device_frame_state()
+        dev = st["device"]
+        with torch.cuda.device(dev):
+            table = self._stage_device_inputs(st, image, kind, box.astype(np.int32), image_ops.padding_color(mean_color))
+            crop_fn = multi_tracker.ENTRY_POINTS[table][1]
+            stream = torch.cuda.current_stream(dev)
+            dp = st["dev_in"].data_ptr()
+            _lib.check(getattr(_lib.load(), crop_fn)(dp, 1, dp + _TARGET_OFFSET, 1, offset, size,
+                                                     st["tcrop"].data_ptr(), stream.cuda_stream), crop_fn)
+            features = self.net.get_features(st["tcrop"])
+            stream.synchronize()  # the pinned inputs are rewritten by the next call
+        return features
+
+    def _update_device_frame(self, image, kind: str) -> Dict[str, Any]:
+        st, cfg = self.tracking_state, self.tracking_config
+        search_bbox, context = image_ops.crop_geometry(st.bbox, cfg["instance_size"], cfg["search_context"])
+        st.mapping = context
+        st.prev_size = search_bbox[2:]
+        rec = self._track_record_device_frame(image, kind)
+        pred_bbox = np.array([rec["x"], rec["y"], rec["w"], rec["h"]])
+        pred_bbox = image_ops.clamp_bbox(self._rescale_bbox(pred_bbox, context), image.shape)
+        st.bbox = pred_bbox
+        st.paths.append(pred_bbox)
+        return dict(bbox=pred_bbox)
+
+    def _track_record_device_frame(self, image, kind: str):
+        """One update on a device frame: crop-targets (N = 1, search_context, 256) -> fear_track_u8 -> the plain decode,
+        or with smooth the maps -> fear_decode_smooth; one 48-byte record back.  The crop kernel reads the frame's record
+        when it runs, so the graph (captured on the second update) keys on the table kind, smooth, the input buffer and
+        net.generation(), not on the frame's address or shape: fresh decoder surfaces and a resolution change replay it."""
+        from . import _lib
+
+        st = self._device_frame_state()
+        dev, smooth, cfg = st["device"], st["smooth"], self.tracking_config
+        size = int(cfg["instance_size"])
+        with torch.cuda.device(dev):
+            trk = self.tracking_state
+            table = self._stage_device_inputs(st, image, kind, trk.bbox, image_ops.padding_color(trk.mean_color),
+                                              trk.prev_size if smooth else None)
+            if st["zf_src"] is not self._template_features:
+                st["zf"].copy_(self._template_features)
+                st["zf_src"] = self._template_features
+            lib = _lib.load()
+            crop_fn = multi_tracker.ENTRY_POINTS[table][1]
+
+            def step():
+                stream = torch.cuda.current_stream(dev).cuda_stream
+                dp = st["dev_in"].data_ptr()
+                _lib.check(getattr(lib, crop_fn)(dp, 1, dp + _TARGET_OFFSET, 1, float(cfg["search_context"]), size,
+                                                 st["crop"].data_ptr(), stream), crop_fn)
+                if not smooth:
+                    return self.net.track_boxes(st["crop"], st["zf"])
+                maps = self.net.track(st["crop"], st["zf"])
+                sp = dp + _SMOOTH_OFFSET
+                _lib.check(lib.fear_decode_smooth(maps[TARGET_REGRESSION_LABEL_KEY].data_ptr(),
+                                                  maps[TARGET_CLASSIFICATION_KEY].data_ptr(), 1, sp, sp + 16,
+                                                  st["smooth_boxes"].data_ptr(), stream), "fear_decode_smooth")
+                return st["smooth_boxes"]
+
+            key = (table, smooth, st["dev_in"].data_ptr(), self.net.generation())
+            if key != st["key"]:  # another entry point, or stale workspace / weight pointers: warm up and capture again
+                st["graph"], st["key"], st["calls"] = None, key, 0
+            use_graph = cfg.get("cuda_graph", True) and st["graph_ok"]
+            if use_graph and st["graph"] is None and st["calls"] >= 1:
+                try:
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        st["boxes"] = step()
+                    st["graph"] = g
+                except RuntimeError as exc:
+                    import warnings
+
+                    warnings.warn(f"FEARTracker: CUDA-graph capture of the device-frame step failed ({exc}); "
+                                  "using eager launches")
+                    st["graph_ok"] = False
+                    torch.cuda.synchronize(dev)
+            if use_graph and st["graph"] is not None and st["graph_ok"]:
+                st["graph"].replay()
+                boxes = st["boxes"]
+            else:
+                boxes = step()
+            st["calls"] += 1
+            st["box_pin"].copy_(boxes, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
         return st["box_pin"].numpy().view(_lib.BOX_DTYPE).reshape(-1)[0].copy()
 
     def track(self, search_crop: np.ndarray) -> Tuple[np.ndarray, float]:
