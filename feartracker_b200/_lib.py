@@ -44,6 +44,9 @@ assert YUV_DTYPE.itemsize == 80
 # FearFrameYCbCr: FearFrameYUV plus its chroma subsampling (4:2:0, 4:2:2, 4:4:4)
 YCBCR_DTYPE = np.dtype(YUV_DTYPE.descr + [("chroma_shift_x", "<i4"), ("chroma_shift_y", "<i4")])
 assert YCBCR_DTYPE.itemsize == 88
+# FearFrameYCbCrV210: FearFrameYCbCr plus whether the entry is a v210 surface (10-bit 4:2:2, three codes per word)
+YCBCR_V210_DTYPE = np.dtype(YCBCR_DTYPE.descr + [("v210", "<i4"), ("reserved", "<i4")])
+assert YCBCR_V210_DTYPE.itemsize == 96
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -79,6 +82,9 @@ _SIGNATURES = {
     "fear_crop_targets_ycbcr_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_ycbcr": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_ycbcr_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_ycbcr_v210_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_ycbcr_v210": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_ycbcr_v210_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_decode_smooth": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),

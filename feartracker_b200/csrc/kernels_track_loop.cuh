@@ -12,9 +12,10 @@
 // (PackedFrames) or a FearFrameView table of strided RGB frames anywhere in device memory (FrameViews), both read
 // through TrackFrame; or a table of YUV frames, FearFrameYUV420 (YUV420Frames, 4:2:0, 8-bit BT.601 limited range),
 // FearFrameYUV (YUVFrames, 4:2:0, the format named per entry) or FearFrameYCbCr (YCbCrFrames, 4:2:0, 4:2:2 or 4:4:4 and
-// the format named per entry), all read through YUVFrame, which converts each pixel it reads to RGB.  A frame type gives
-// H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables, interpolation, sums and
-// the colour conversion exist once.
+// the format named per entry), all read through YUVFrame, which converts each pixel it reads to RGB; or a table of
+// FearFrameYCbCrV210 records (YCbCrV210Frames), read through V210Frame, which also unpacks v210 surfaces.  A frame type
+// gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables, interpolation, sums
+// and the colour conversion exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
 // into an FMA by default, which rounds once instead of twice, so every multiply-add here is spelled with the explicitly
@@ -122,7 +123,10 @@ struct YUVFrame {
   }
   __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
     const long long c = (long long)(y >> csy) * uvrs + (long long)(x >> csx) * uvps;
-    const int Yc = sample(Y + (long long)y * yrs + (long long)x * yps), Uc = sample(U + c), Vc = sample(V + c);
+    convert(sample(Y + (long long)y * yrs + (long long)x * yps), sample(U + c), sample(V + c), p);
+  }
+  // the RGB triple of the codes (Yc, Uc, Vc) in this frame's format
+  __device__ __forceinline__ void convert(int Yc, int Uc, int Vc, int p[3]) const {
     if (!h273) {
       yuv_to_rgb_bt601(Yc, Uc, Vc, p);
       return;
@@ -196,10 +200,68 @@ struct YUVFrames {
 struct YCbCrFrames {
   const FearFrameYCbCr* views;
   __device__ __forceinline__ YUVFrame operator()(int i) const {
-    const int csx = views[i].chroma_shift_x, csy = views[i].chroma_shift_y;
-    YUVFrame f = yuv_frame_of(views + i, csx, csy);
+    return ycbcr_frame_of(views + i);
+  }
+  // also the v210 == 0 entries of a FearFrameYCbCrV210 table, whose leading fields are these
+  template <class Record>
+  static __device__ __forceinline__ YUVFrame ycbcr_frame_of(const Record* p) {
+    const int csx = p->chroma_shift_x, csy = p->chroma_shift_y;
+    YUVFrame f = yuv_frame_of(p, csx, csy);
     f.bad |= !(csx == 1 ? (csy == 0 || csy == 1) : (csx == 0 && csy == 0));
     return f;
+  }
+};
+
+// A frame of a FearFrameYCbCrV210 table: a YUVFrame read as it is (v210 false), or a v210 surface (v210 true) whose row
+// y starts at Y + y * yrs.  A row is a run of 16-byte groups of four little-endian 32-bit words, each word three 10-bit
+// codes at bits 0, 10 and 20; the twelve codes of group g are, in order, Cb0 Y0 Cr0 Y1 Cb1 Y2 Cr1 Y3 Cb2 Y4 Cr2 Y5
+// (pixels 6g .. 6g + 5, chroma pairs 3g .. 3g + 2), so pixel x's luma is code 2 (x % 6) + 1 and its chroma pair
+// k = (x % 6) / 2 is codes 4k (Cb) and 4k + 2 (Cr) of group x / 6.  The codes go through convert(); H, W and empty()
+// are the YUVFrame's, whose fields the source fills in for either kind.  A value-initialised V210Frame{} is empty.
+struct V210Frame : YUVFrame {
+  bool v210;
+  // code i (0 .. 11) of the group at g
+  static __device__ __forceinline__ int code(const uint8_t* g, unsigned i) {
+    const unsigned w = i / 3;
+    return (__ldg(reinterpret_cast<const uint32_t*>(g) + w) >> (10 * (i - 3 * w))) & 1023;
+  }
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    if (!v210) {
+      YUVFrame::rgb(y, x, p);
+      return;
+    }
+    const unsigned g = (unsigned)x / 6, r = (unsigned)x - 6 * g, k = r >> 1;
+    const uint8_t* q = Y + (long long)y * yrs + 16LL * g;
+    convert(code(q, 2 * r + 1), code(q, 4 * k), code(q, 4 * k + 2), p);
+  }
+};
+
+// Frame i of a FearFrameYCbCrV210 table (the *_ycbcr_v210 entry points): with v210 == 0 the entry's FearFrameYCbCr
+// fields, read exactly as YCbCrFrames reads them; with v210 == 1 a v210 surface at y with row pitch y_row_stride, 10-bit
+// 4:2:2 in the entry's matrix and range (u, v, y_pixel_stride, the uv strides and shift are not read).  A v210 entry
+// the kernels cannot read: a null or non-4-byte-aligned y, a pitch not a multiple of 4 or below 16 * ceil(W / 6), an
+// odd W, bits other than 10, shifts other than (1, 0), or FearFrameYUV's matrix / range / size rules; any other v210
+// value is unreadable too.
+struct YCbCrV210Frames {
+  const FearFrameYCbCrV210* views;
+  __device__ __forceinline__ V210Frame operator()(int i) const {
+    const FearFrameYCbCrV210* p = views + i;
+    const int v210 = p->v210;
+    if (v210 != 1) {
+      V210Frame f{YCbCrFrames::ycbcr_frame_of(p), false};
+      f.bad |= v210 != 0;
+      return f;
+    }
+    const FearFrameYCbCrV210 v = *p;
+    const uint8_t* y = static_cast<const uint8_t*>(v.y);
+    const long long pitch = v.y_row_stride;
+    const bool ok = !(((uintptr_t)y | (uintptr_t)pitch) & 3) && pitch >= 16LL * (((long long)v.W + 5) / 6) &&
+                    v.bits == 10 && v.chroma_shift_x == 1 && v.chroma_shift_y == 0 && v.matrix >= FEAR_YUV_BT601 &&
+                    v.matrix <= FEAR_YUV_BT2020 && (v.full_range == 0 || v.full_range == 1);
+    // U and V point at the surface too, so empty() refuses exactly a null y among the planes
+    return V210Frame{{y, y, y, pitch, 0, 0, 0, v.H, v.W, 1, 0, 10, 0, true, true, !ok,
+                      ok ? yuv_coefs(v.matrix, v.full_range, 10) : YUVCoefs{}},
+                     true};
   }
 };
 

@@ -222,3 +222,71 @@ def yuv_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601
     pr = (V.astype(np.float64) - c0) * cs
     rgb = [yn + cr * pr, (yn - gb * pb) - gr * pr, yn + cb * pb]
     return np.stack([np.clip(np.rint(255.0 * c), 0, 255) for c in rgb], -1).astype(np.uint8)
+
+
+def v210_row_bytes(width: int) -> int:
+    """The bytes a v210 row of ``width`` pixels needs: 16 per group of 6 pixels, the last group possibly partial."""
+    return 16 * -(-int(width) // 6)
+
+
+def v210_pitch(width: int) -> int:
+    """The row pitch capture cards and ffmpeg give a v210 row of ``width`` pixels: 128 * ceil(width / 48) bytes."""
+    return 128 * -(-int(width) // 48)
+
+
+def _v210_check_width(width, rows_bytes=None) -> int:
+    if isinstance(width, bool) or not isinstance(width, (int, np.integer)) or width < 2 or width % 2:
+        raise ValueError(f"a v210 width must be an even int >= 2, got {width!r}")
+    width = int(width)
+    if rows_bytes is not None and rows_bytes < v210_row_bytes(width):
+        raise ValueError(f"a v210 row of {width} pixels needs {v210_row_bytes(width)} bytes, got {rows_bytes}")
+    return width
+
+
+def v210_unpack(words_u8: np.ndarray, width: int):
+    """The (y, u, v) uint16 planes of a v210 frame: ``words_u8`` (H, pitch) uint8 are its rows as bytes, ``width`` the
+    picture width (even).  y is (H, width), u (Cb) and v (Cr) are (H, width / 2) of 10-bit codes, the planes of a 4:2:2
+    frame (``yuv_to_rgb(y, u, v, matrix, full_range, bits=10, chroma_shift=(1, 0))`` is the RGB frame the tracker sees
+    for it).  A row is a run of 16-byte groups of four little-endian 32-bit words, each holding three 10-bit codes at bits
+    0, 10 and 20 (bits 30-31 ignored); the twelve codes of a group are Cb0 Y0 Cr0 Y1 Cb1 Y2 Cr1 Y3 Cb2 Y4 Cr2 Y5 (ffmpeg's
+    v210 order), pixels past ``width`` in the last group are dropped.  A numpy restatement of the crop kernel's reads
+    (include/fear_b200.h, FearFrameYCbCrV210)."""
+    a = np.asarray(words_u8)
+    if a.dtype != np.uint8 or a.ndim != 2 or a.shape[0] < 1:
+        raise ValueError(f"v210 rows must be a 2-D uint8 (H, pitch) array with H >= 1, got {a.dtype} {a.shape}")
+    width = _v210_check_width(width, a.shape[1])
+    groups = -(-width // 6)
+    w = np.ascontiguousarray(a[:, :16 * groups]).view("<u4").reshape(a.shape[0], groups, 4)
+    codes = np.stack([(w >> s) & 1023 for s in (0, 10, 20)], -1).reshape(a.shape[0], groups, 12).astype(np.uint16)
+    y = codes[..., 1::2].reshape(a.shape[0], 6 * groups)[:, :width]
+    u = codes[..., 0::4].reshape(a.shape[0], 3 * groups)[:, :width // 2]
+    v = codes[..., 2::4].reshape(a.shape[0], 3 * groups)[:, :width // 2]
+    return y, u, v
+
+
+def v210_pack(y: np.ndarray, u: np.ndarray, v: np.ndarray, pitch: Optional[int] = None) -> np.ndarray:
+    """The (H, pitch) uint8 v210 rows of 10-bit 4:2:2 planes: the inverse of ``v210_unpack``.  y is (H, W) with W even,
+    u and v (H, W / 2), codes in [0, 1023]; ``pitch`` defaults to ``v210_pitch(W)``.  Codes of the pixels that fill out
+    the last group, bits 30-31 and the bytes past the last group are 0."""
+    Y, U, V = (np.asarray(p) for p in (y, u, v))
+    if Y.ndim != 2 or Y.shape[0] < 1:
+        raise ValueError(f"luma must be a 2-D (H, W) array with H >= 1, got shape {Y.shape}")
+    h, width = Y.shape[0], _v210_check_width(Y.shape[1])
+    if U.shape != (h, width // 2) or V.shape != (h, width // 2):
+        raise ValueError(f"chroma must be ({h}, {width // 2}), got {U.shape} and {V.shape}")
+    if any(p.size and (p.min() < 0 or p.max() > 1023) for p in (Y, U, V)):
+        raise ValueError("v210 codes must be in [0, 1023]")
+    pitch = v210_pitch(width) if pitch is None else int(pitch)
+    if pitch < v210_row_bytes(width):
+        raise ValueError(f"a v210 row of {width} pixels needs {v210_row_bytes(width)} bytes, got pitch {pitch}")
+    groups = -(-width // 6)
+    codes = np.zeros((h, groups, 12), dtype=np.uint32)
+    for plane, first, step, n in ((Y, 1, 2, 6), (U, 0, 4, 3), (V, 2, 4, 3)):
+        full = np.zeros((h, n * groups), dtype=np.uint32)
+        full[:, :plane.shape[1]] = plane
+        codes[..., first::step] = full.reshape(h, groups, n)
+    c = codes.reshape(h, groups, 4, 3)
+    words = (c[..., 0] | c[..., 1] << 10 | c[..., 2] << 20).astype("<u4")
+    out = np.zeros((h, pitch), dtype=np.uint8)
+    out[:, :16 * groups] = words.reshape(h, 4 * groups).view(np.uint8)
+    return out

@@ -10,7 +10,8 @@ included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y
 device as a video decoder, webcam or capture card writes them: YUV420Frame (NV12 / I420, P010 / P016 / yuv420p10le),
 YUV422Frame (YUYV / UYVY / YVYU, Y210, NV16 / P210, yuv422p) and YUV444Frame (yuv444p, NVDEC's 4:4:4 surfaces), in
 BT.601, BT.709 or BT.2020, limited or full range, 8, 10 or 12 bits, converted to RGB inside the crop (8-bit BT.601
-limited range exactly as cv2.cvtColor converts it).  Tensors and YUV planes are read where they are, without a copy.
+limited range exactly as cv2.cvtColor converts it), and V210Frame (SDI capture cards' packed 10-bit 4:2:2, unpacked
+inside the crop).  Tensors, YUV planes and v210 surfaces are read where they are, without a copy.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -25,7 +26,9 @@ FearFrameView records (address, byte strides, H, W) in a fixed device buffer, wr
 are packed into one pinned buffer and sent with one copy, and their views point into the packed device buffer; CUDA
 tensors' views point at the tensors.  YUV420Frames go into a second fixed table of FearFrameYUV records (planes and colour
 format), read by the *_yuv entry points; a call with any 4:2:2 or 4:4:4 frame puts all its frames into a third, of
-FearFrameYCbCr records (the same plus the chroma subsampling), read by the *_ycbcr entry points.  The host then reads
+FearFrameYCbCr records (the same plus the chroma subsampling), read by the *_ycbcr entry points; a call with any
+V210Frame puts all its frames into a fourth, of FearFrameYCbCrV210 records (a FearFrameYCbCr or a v210 surface), read
+by the *_ycbcr_v210 entry points.  The host then reads
 back the boxes and scores.  The launch count of a step depends neither on N nor on the kind of frames.
 """
 import math
@@ -44,8 +47,11 @@ ENTRY_POINTS = {
     "views": ("fear_frame_sums_u8", "fear_crop_targets_view_u8", "fear_advance_targets_view"),
     "yuv": ("fear_frame_sums_yuv_u8", "fear_crop_targets_yuv_u8", "fear_advance_targets_yuv"),
     "ycbcr": ("fear_frame_sums_ycbcr_u8", "fear_crop_targets_ycbcr_u8", "fear_advance_targets_ycbcr"),
+    "ycbcr_v210": ("fear_frame_sums_ycbcr_v210_u8", "fear_crop_targets_ycbcr_v210_u8",
+                   "fear_advance_targets_ycbcr_v210"),
 }
-TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE}
+TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE,
+                "ycbcr_v210": _lib.YCBCR_V210_DTYPE}
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -125,6 +131,10 @@ class _YUVFrame:
         return (self.y.data_ptr(), self.u.data_ptr(), self.v.data_ptr(), yrs * es, yps * es, uvrs * es, uvps * es,
                 *self.shape[:2], image_ops.YUV_MATRICES[self.matrix][0], int(self.full_range), self.bits, self.shift,
                 *self.CHROMA_SHIFT)
+
+    def ycbcr_v210_record(self) -> tuple:
+        """The FearFrameYCbCrV210 record of a planar frame: ``ycbcr_record``, then v210 = 0 and the reserved 0."""
+        return self.ycbcr_record() + (0, 0)
 
 
 class YUV420Frame(_YUVFrame):
@@ -279,10 +289,57 @@ class YUV444Frame(_YUVFrame):
         return cls(t[:h], t[h:2 * h], t[2 * h:], matrix=matrix, full_range=full_range, bits=bits, msb=msb)
 
 
+class V210Frame:
+    """A v210 frame (10-bit 4:2:2 packed three codes to a 32-bit word) as SDI capture cards (Blackmagic DeckLink's
+    ``bmdFormat10BitYUV``, AJA, Magewell), ffmpeg's v210 decoder and QuickTime uncompressed 10-bit write it.  ``t`` is
+    the capture buffer as bytes: a CUDA uint8 (H, row bytes) tensor whose rows are contiguous, any row pitch (a view
+    ``surface[:, :n]`` of a pitched surface is fine); ``width`` is the picture width W (even).  A row needs
+    ``16 * ceil(W / 6)`` bytes; capture cards pitch rows to ``128 * ceil(W / 48)``.  The buffer address and the row pitch
+    must be multiples of 4 bytes.  ``matrix`` and ``full_range`` are those of YUV420Frame; the depth is 10 bits.
+
+    FEARMultiTracker and FEARTracker read the words where they are and unpack and convert every pixel they read, so no
+    planes and no RGB copy are made: the RGB frame the tracker sees is ``image_ops.yuv_to_rgb(*image_ops.v210_unpack(
+    rows, W), matrix, full_range, bits=10, chroma_shift=(1, 0))`` of the same bytes.  The constructor raises ValueError
+    on a malformed buffer or format.  ``shape`` is (H, W, 3)."""
+    CHROMA_SHIFT = (1, 0)
+    bits = 10
+
+    def __init__(self, t: torch.Tensor, width: int, *, matrix: str = "bt601", full_range: bool = False) -> None:
+        if matrix not in image_ops.YUV_MATRICES:
+            raise ValueError(f"V210Frame matrix must be one of {sorted(image_ops.YUV_MATRICES)}, got {matrix!r}")
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.ndim != 2 or t.device.type != "cuda":
+            what = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"V210Frame takes a 2-D CUDA uint8 (H, row bytes) tensor, got {what}")
+        if isinstance(width, bool) or not isinstance(width, (int, np.integer)) or not (2 <= width <= _MAX_SIDE) \
+                or width % 2:
+            raise ValueError(f"V210Frame width must be an even int in [2, {_MAX_SIDE}], got {width!r}")
+        h, need = t.shape[0], image_ops.v210_row_bytes(width)
+        if not 1 <= h <= _MAX_SIDE:
+            raise ValueError(f"V210Frame needs 1 to {_MAX_SIDE} rows, got {h}")
+        if t.shape[1] < need:
+            raise ValueError(f"a v210 row of {width} pixels needs {need} bytes, the tensor's rows have {t.shape[1]}")
+        pitch = t.stride(0) if h > 1 else need  # one row: the pitch is never stepped
+        if t.stride(1) != 1 or pitch < need:
+            raise ValueError(f"V210Frame rows must be contiguous bytes at a pitch >= {need}, got strides {t.stride()}")
+        if pitch % 4 or t.data_ptr() % 4:
+            raise ValueError(f"V210Frame rows must start on 4-byte boundaries: pitch {pitch}, address offset "
+                             f"{t.data_ptr() % 4}")
+        self.t, self.width, self.pitch = t, int(width), int(pitch)
+        self.shape = (h, self.width, 3)
+        self.matrix, self.full_range = matrix, bool(full_range)
+
+    def ycbcr_v210_record(self) -> tuple:
+        """The FearFrameYCbCrV210 record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W,
+        matrix, full_range, bits, shift, chroma_shift_x, chroma_shift_y, v210, reserved) of the surface: its address and
+        row pitch, the size and format, v210 = 1; the fields a v210 entry does not read are 0."""
+        return (self.t.data_ptr(), 0, 0, self.pitch, 0, 0, 0, *self.shape[:2], image_ops.YUV_MATRICES[self.matrix][0],
+                int(self.full_range), self.bits, 0, *self.CHROMA_SHIFT, 1, 0)
+
+
 def frame_kind(frame) -> str:
-    """"yuv" for a YUV420Frame, YUV422Frame or YUV444Frame, "cuda" for a torch tensor (checked by
+    """"yuv" for a YUV420Frame, YUV422Frame, YUV444Frame or V210Frame, "cuda" for a torch tensor (checked by
     ``check_device_frame``), "numpy" for anything else."""
-    if isinstance(frame, _YUVFrame):
+    if isinstance(frame, (_YUVFrame, V210Frame)):
         return "yuv"
     return "cuda" if isinstance(frame, torch.Tensor) else "numpy"
 
@@ -312,19 +369,22 @@ def check_tensor_frame(i: int, f: torch.Tensor, device) -> None:
 def check_device_frame(i: int, f, kind: str, device) -> None:
     """The checks of a frame of kind "cuda" or "yuv" (``frame_kind``): ValueError before any device call."""
     if kind == "yuv":
-        check_device(i, device, f.y, f.u, f.v)
+        check_device(i, device, *((f.t,) if isinstance(f, V210Frame) else (f.y, f.u, f.v)))
     else:
         check_tensor_frame(i, f, device)
 
 
 def write_records(table: np.ndarray, frames, name: str) -> None:
     """Write the records of device frames into rows of ``table`` (a numpy view of ``TABLE_DTYPES[name]``):
-    FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr"."""
+    FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr",
+    FearFrameYCbCrV210 for "ycbcr_v210"."""
     for i, f in enumerate(frames):
         if name == "yuv":
             table[i] = f.yuv_record()
         elif name == "ycbcr":
             table[i] = f.ycbcr_record()
+        elif name == "ycbcr_v210":
+            table[i] = f.ycbcr_v210_record()
         else:
             table[i] = frame_view(f)
 
@@ -380,8 +440,8 @@ class FEARMultiTracker:
         """Start tracking ``rects`` ((n, 4) [x, y, w, h]); target i lives in stream ``streams[i]`` (default 0), whose
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
-        ``frames`` are all numpy arrays, all CUDA tensors or all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame;
-        see ``update``).  A target's padding colour is the mean colour of its frame (of the converted RGB frame for a
+        ``frames`` are all numpy arrays, all CUDA tensors or all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame,
+        V210Frame; see ``update``).  A target's padding colour is the mean colour of its frame (of the converted RGB frame for a
         YUV frame), from exact
         per-channel sums computed on the device."""
         frames, kind = self._check_frames(frames)
@@ -463,8 +523,9 @@ class FEARMultiTracker:
         the tracker's CUDA device; they are read in place too, and every target fed YUV frames gives exactly the ids,
         boxes and scores of the same tracker fed ``image_ops.yuv_to_rgb`` of the planes (with the frame's
         ``CHROMA_SHIFT``) as numpy arrays (for the default format that is ``cv2.cvtColor(frame,
-        cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420 / COLOR_YUV2RGB_YUY2 / COLOR_YUV2RGB_UYVY)``).  Frames of one call
-        may have different colour formats and subsamplings.  Device frames must be
+        cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420 / COLOR_YUV2RGB_YUY2 / COLOR_YUV2RGB_UYVY)``).  A ``V210Frame``'s
+        words are read in place as well and give what its ``image_ops.v210_unpack`` planes give at 10 bits, 4:2:2.
+        Frames of one call may have different colour formats and subsamplings.  Device frames must be
         ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
@@ -500,7 +561,8 @@ class FEARMultiTracker:
 
     def _check_frames(self, frames):
         """-> (list of frames, their kind: "numpy", "cuda" or "yuv").  Raises ValueError before any device call."""
-        if isinstance(frames, _YUVFrame) or (isinstance(frames, (np.ndarray, torch.Tensor)) and frames.ndim == 3):
+        if isinstance(frames, (_YUVFrame, V210Frame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
+                                                          and frames.ndim == 3):
             frames = [frames]
         frames = list(frames)
         if not frames:
@@ -508,7 +570,7 @@ class FEARMultiTracker:
         kind = frame_kind(frames[0])
         if any(frame_kind(f) != kind for f in frames):
             raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV frames "
-                             "(YUV420Frame, YUV422Frame, YUV444Frame), not a mix")
+                             "(YUV420Frame, YUV422Frame, YUV444Frame, V210Frame), not a mix")
         for i, f in enumerate(frames):
             if kind != "numpy":
                 check_device_frame(i, f, kind, self._device)
@@ -545,19 +607,22 @@ class FEARMultiTracker:
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
             frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, ycbcr_pin=None,
-            ycbcr=None, sums_pin=None, sums=None)
+            ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, sums_pin=None, sums=None)
         return b
 
     def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
         """Write the frame table of ``frames`` into the fixed device table the kernels read, and return its name:
-        "yuv" (FearFrameYUV records) when every frame is a YUV420Frame, "ycbcr" (FearFrameYCbCr records) for YUV frames
-        of which any is 4:2:2 or 4:4:4, "views" (FearFrameView records) otherwise.  Numpy frames are
+        "yuv" (FearFrameYUV records) when every frame is a YUV420Frame, "ycbcr_v210" (FearFrameYCbCrV210 records) for
+        YUV frames of which any is a V210Frame, "ycbcr" (FearFrameYCbCr records) for other YUV frames of which any is
+        4:2:2 or 4:4:4, "views" (FearFrameView records) otherwise.  Numpy frames are
         packed into the pinned staging buffer first and sent with one host-to-device copy (the packed layout is
-        recomputed only when their shapes change); CUDA tensors and YUV planes are used where they are."""
+        recomputed only when their shapes change); CUDA tensors, YUV planes and v210 surfaces are used where they are."""
         b, num_frames = self._buf, len(frames)
         name = "views"
         if kind == "yuv":
             name = "yuv" if all(isinstance(f, YUV420Frame) for f in frames) else "ycbcr"
+            if any(isinstance(f, V210Frame) for f in frames):
+                name = "ycbcr_v210"
         dtype = TABLE_DTYPES[name]
         nbytes = num_frames * dtype.itemsize
         if b[name] is None or b[name].numel() < nbytes:  # grows only: the step graph keys on it
@@ -607,8 +672,8 @@ class FEARMultiTracker:
     def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device) -> torch.Tensor:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
-        keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records or YCbCr
-        records of any subsampling) and
+        keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records, YCbCr
+        records of any subsampling or YCbCr / v210 records) and
         its buffer, and the net's generation.  ``cuda_graph=False`` in the tracking config keeps eager launches."""
         key = (n, num_frames, table, self._buf[table].data_ptr())
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):

@@ -7,10 +7,10 @@ API mirror of reference model_training/tracker/base_tracker.py:28-124 and fear_t
 of the reference's observable behaviour); network + decode run in libfear_b200 and only the
 48-byte box record comes back per frame.  With ``gpu_crop: true`` the numpy frame is uploaded and cropped on the device.
 
-Frames already in GPU memory -- uint8 (H, W, 3) CUDA tensors with any non-negative strides, and YUV420Frame /
-YUV422Frame / YUV444Frame decoder surfaces -- are read in place: the crop, the conversion to RGB, the network and the
-decode (plain or smoothed) run on the device, and the tracker returns exactly what it returns for the same pixels as a
-numpy array (``image_ops.yuv_to_rgb`` of a YUV frame's planes).
+Frames already in GPU memory -- uint8 (H, W, 3) CUDA tensors with any non-negative strides, YUV420Frame /
+YUV422Frame / YUV444Frame decoder surfaces and V210Frame capture buffers -- are read in place: the crop, the conversion
+to RGB, the network and the decode (plain or smoothed) run on the device, and the tracker returns exactly what it
+returns for the same pixels as a numpy array (``image_ops.yuv_to_rgb`` of a YUV frame's planes).
 """
 from collections import deque
 from typing import Any, Dict, Optional, Tuple, Union
@@ -24,9 +24,9 @@ from .box_coder import FEARBoxCoder, TrackerDecodeResult
 from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY
 
 
-# byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCr), a FearTarget,
-# then five float64 inputs of fear_decode_smooth
-_TARGET_OFFSET = 88
+# byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrV210), a
+# FearTarget, then five float64 inputs of fear_decode_smooth
+_TARGET_OFFSET = 96
 _SMOOTH_OFFSET = _TARGET_OFFSET + 64
 _DEVICE_INPUT_BYTES = _SMOOTH_OFFSET + 5 * 8
 
@@ -108,16 +108,18 @@ class Tracker:
 class FEARTracker(Tracker):
     """The reference's single-object tracker.  ``initialize``, ``update`` and ``get_template_features`` take a frame as
     a uint8 (H, W, 3) RGB numpy array, as a uint8 (H, W, 3) CUDA tensor on the tracker's device (any non-negative
-    strides: ``rgba[..., :3]``, ``chw.permute(1, 2, 0)``, a region of interest), or as a YUV420Frame, YUV422Frame or
-    YUV444Frame whose planes are on the tracker's device; the kind may change from one call to the next.
+    strides: ``rgba[..., :3]``, ``chw.permute(1, 2, 0)``, a region of interest), or as a YUV420Frame, YUV422Frame,
+    YUV444Frame or V210Frame whose planes or words are on the tracker's device; the kind may change from one call to
+    the next.
 
     Numpy frames take the host crop, or with ``gpu_crop: true`` an upload and the device crop.  Device frames always
     take the device step, whatever ``gpu_crop`` says, since the host crop could only read them after copying them back:
-    fear_crop_targets_view_u8 (tensors) or fear_crop_targets_ycbcr_u8 (YUV frames, converted to RGB inside the crop)
-    makes the search crop, then the network and the decode, plain or with ``smooth: true`` the smoothed one, run as one
-    CUDA graph and one 48-byte record comes back.  The results, ``tracking_state`` included, are those of the same
-    tracker fed the same pixels as numpy arrays (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its
-    ``CHROMA_SHIFT``).  Device frames must be ready on the current CUDA stream; every call synchronises it before it
+    fear_crop_targets_view_u8 (tensors), fear_crop_targets_ycbcr_u8 (YUV frames, converted to RGB inside the crop) or
+    fear_crop_targets_ycbcr_v210_u8 (v210 frames, unpacked and converted inside the crop) makes the search crop, then
+    the network and the decode, plain or with ``smooth: true`` the smoothed one, run as one CUDA graph and one 48-byte
+    record comes back.  The results, ``tracking_state`` included, are those of the same tracker fed the same pixels as
+    numpy arrays (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its ``CHROMA_SHIFT``, of a v210 frame's
+    ``image_ops.v210_unpack`` planes).  Device frames must be ready on the current CUDA stream; every call synchronises it before it
     returns, so they only need to live for the call.  ``host_normalize: true`` takes numpy frames only."""
 
     def get_box_coder(self, tracking_config, cuda_id: int = 0):
@@ -279,9 +281,10 @@ class FEARTracker(Tracker):
 
     def _device_frame_state(self) -> dict:
         """Buffers of the device-frame step, separate from the gpu_crop path's.  ``inputs`` (pinned) and ``dev_in``
-        share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView or a
-        FearFrameYCbCr) at byte 0, the FearTarget at byte 88, fear_decode_smooth's prev_size (w, h), penalty_k,
-        window_influence and lr as float64 at byte 152; then, on the device only, the 16 x 16 window."""
+        share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView, a
+        FearFrameYCbCr or a FearFrameYCbCrV210) at byte 0, the FearTarget at byte 96, fear_decode_smooth's prev_size
+        (w, h), penalty_k, window_influence and lr as float64 at byte 160; then, on the device only, the 16 x 16
+        window."""
         from . import _lib
 
         dev = self._device()
@@ -309,8 +312,10 @@ class FEARTracker(Tracker):
     def _stage_device_inputs(self, st: dict, image, kind: str, bbox, pad, prev_size=None) -> str:
         """Write the frame's record, the target (frame 0, ``bbox``, padding colour ``pad``) and, given ``prev_size``,
         the smooth scalars into the pinned inputs and send them with one host-to-device copy.  Returns the table name:
-        "views" for a tensor, "ycbcr" for every YUV frame."""
-        table = "ycbcr" if kind == "yuv" else "views"
+        "views" for a tensor, "ycbcr_v210" for a V210Frame, "ycbcr" for every other YUV frame."""
+        table = "views"
+        if kind == "yuv":
+            table = "ycbcr_v210" if isinstance(image, multi_tracker.V210Frame) else "ycbcr"
         raw, dtype = st["inputs"].numpy(), multi_tracker.TABLE_DTYPES[table]
         multi_tracker.write_records(raw[:dtype.itemsize].view(dtype), [image], table)
         target = raw[_TARGET_OFFSET:_SMOOTH_OFFSET].view(np.int32)

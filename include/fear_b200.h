@@ -36,6 +36,9 @@
  *   fear_crop_targets_ycbcr_u8 / fear_advance_targets_ycbcr / fear_frame_sums_ycbcr_u8   the same three on YUV 4:2:0,
  *                         4:2:2 and 4:4:4 frames located by FearFrameYCbCr (YUYV / UYVY / Y210, NV16 / P210,
  *                         yuv422p, yuv444p, NVDEC's YUV444 surfaces), in every FearFrameYUV colour format
+ *   fear_crop_targets_ycbcr_v210_u8 / fear_advance_targets_ycbcr_v210 / fear_frame_sums_ycbcr_v210_u8   the same three
+ *                         on FearFrameYCbCrV210 tables: FearFrameYCbCr entries and v210 surfaces (10-bit 4:2:2 packed
+ *                         three codes to a 32-bit word, as SDI capture cards deliver it), unpacked inside the crop
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -168,6 +171,32 @@ typedef struct FearFrameYCbCr {            /* 88 bytes                          
   int32_t matrix, full_range, bits, shift; /* as in FearFrameYUV                                                */
   int32_t chroma_shift_x, chroma_shift_y;  /* (1, 1) 4:2:0, (1, 0) 4:2:2, (0, 0) 4:4:4                          */
 } FearFrameYCbCr;
+/* A FearFrameYCbCr or a v210 surface: 96 bytes, the fields of FearFrameYCbCr followed by `v210` and a reserved int32.
+ * With v210 == 0 the entry is read exactly as a FearFrameYCbCr, so v210 surfaces can share a table with every other YUV
+ * frame.  With v210 == 1 the entry is a v210 surface (10-bit 4:2:2 as SDI capture cards and ffmpeg's v210 codec write
+ * it): y is the address of row 0's first word, y_row_stride the row pitch in bytes; bits must be 10 and the chroma
+ * shifts (1, 0); matrix and full_range are read as in FearFrameYUV; u, v, y_pixel_stride, the uv strides and shift are
+ * not read.  A row is a run of 16-byte groups of four little-endian 32-bit words, each holding three 10-bit codes at
+ * bits 0-9, 10-19 and 20-29 (bits 30-31 are ignored).  Group g holds pixels 6g .. 6g + 5 and chroma pairs 3g .. 3g + 2:
+ *   w0 = Cb0 | Y0 << 10 | Cr0 << 20     w1 = Y1 | Cb1 << 10 | Y2 << 20
+ *   w2 = Cr1 | Y3 << 10 | Cb2 << 20     w3 = Y4 | Cr2 << 10 | Y5 << 20
+ * Pixel x takes chroma pair x / 2 (co-sited, nearest).  W must be even, H >= 1; a row needs 16 * ceil(W / 6) bytes, and
+ * capture cards and ffmpeg pitch rows to 128 * ceil(W / 48).  A W x H v210 surface with row pitch P at address b is
+ *   {b, 0, 0, P, 0, 0, 0, H, W, matrix, full_range, 10, 0, 1, 0, 1, 0}
+ * and converts exactly as FearFrameYUV's H.273 inverse at 10 bits does on the unpacked codes.  A v210 entry is treated
+ * like a frame index outside [0, F) when y is null or not 4-byte aligned, the pitch is not a multiple of 4 or below
+ * 16 * ceil(W / 6), W is odd or < 2, H < 1, bits is not 10, the shifts are not (1, 0), or matrix / full_range is not one
+ * FearFrameYUV allows; any v210 value other than 0 and 1 is too. */
+typedef struct FearFrameYCbCrV210 {        /* 96 bytes                                                          */
+  const void *y, *u, *v;                   /* device addresses (v210: y only, row 0's first word)               */
+  int64_t y_row_stride, y_pixel_stride;    /* bytes (v210: the row pitch, a multiple of 4; the pixel stride is   */
+  int64_t uv_row_stride, uv_pixel_stride;  /* not read, nor are the uv strides)                                  */
+  int32_t H, W;                            /* luma size                                                         */
+  int32_t matrix, full_range, bits, shift; /* as in FearFrameYUV (v210: bits 10, shift not read)                */
+  int32_t chroma_shift_x, chroma_shift_y;  /* as in FearFrameYCbCr (v210: 1, 0)                                 */
+  int32_t v210;                            /* 0: a FearFrameYCbCr entry; 1: a v210 surface                      */
+  int32_t reserved;                        /* not read                                                          */
+} FearFrameYCbCrV210;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -319,6 +348,16 @@ int fear_crop_targets_ycbcr_u8(const FearFrameYCbCr* d_views, int F, FearTarget*
 int fear_advance_targets_ycbcr(const FearBox* d_boxes, const FearFrameYCbCr* d_views, int F, FearTarget* d_targets,
                                int N, int instance_size, void* stream);
 int fear_frame_sums_ycbcr_u8(const FearFrameYCbCr* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* The same three on FearFrameYCbCrV210 tables, so v210 surfaces from SDI capture cards are unpacked and converted inside
+ * the crop and read where they are, alongside any other YUV frame.  A v210 == 0 entry gives exactly what the *_ycbcr
+ * entry points give on its FearFrameYCbCr fields.  Same semantics and FEAR_EINVAL rules as the *_ycbcr entry points; an
+ * entry the kernels cannot read (see FearFrameYCbCrV210) gets a padding-colour crop, keeps its box and sums to 0. */
+int fear_crop_targets_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, FearTarget* d_targets, int N,
+                                    double offset, int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_ycbcr_v210(const FearBox* d_boxes, const FearFrameYCbCrV210* d_views, int F,
+                                    FearTarget* d_targets, int N, int instance_size, void* stream);
+int fear_frame_sums_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
