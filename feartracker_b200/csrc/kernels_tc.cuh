@@ -358,6 +358,19 @@ inline bool pw_supported(int cin, int cout) { return available() && cin % 8 == 0
 
 #define FEAR_PW_FOR_NT(X) X(16) X(32) X(48) X(64) X(96) X(112) X(128)
 
+// A GEMM with one K chunk (K <= 32) does little work per CTA, and one CTA per SM runs its TMA load, MMAs and epilogue
+// stores strictly one after another.  Such layers are cut into tiles of at most kPwNarrowNT columns instead: the
+// kernel at NT = 32 needs 68 registers per thread (against 135 at NT = 96), so three CTAs share an SM and one CTA's
+// loads and stores overlap another's MMAs.  The A tile is then read once per n-tile, mostly from L2.  The tile width
+// does not change any output element's sequence of mma3 products, so results are the same bit for bit.
+constexpr int kPwNarrowNT = 32;
+inline int pw_tile_n_one_chunk(int N) {
+  const int Np = (N + 15) & ~15;
+  const int tiles = (Np + kPwNarrowNT - 1) / kPwNarrowNT;
+  const int need = (Np + tiles - 1) / tiles;
+  return need <= 16 ? 16 : 32;
+}
+
 inline int init_pw() {
   cudaError_t e = cudaSuccess;
 #define FEAR_PW_ATTR(NT_)                                                                                                  \
@@ -388,7 +401,7 @@ inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi,
   p.M = M;
   p.N = N;
   p.num_chunks = (K + 31) / 32;
-  const int NT = pw_tile_n(N);
+  const int NT = p.num_chunks == 1 ? pw_tile_n_one_chunk(N) : pw_tile_n(N);
   if (!NT) return -21;
   p.num_n_tiles = (((N + 15) & ~15) + NT - 1) / NT;
   p.last_ksteps = ((K - 32 * (p.num_chunks - 1)) + 7) / 8;
