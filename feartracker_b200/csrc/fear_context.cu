@@ -383,7 +383,7 @@ static int run_blocks(FearContext* c, cudaStream_t s, float* X, int B, int& h, i
     if (i == 1 && c->opt.fuse_irf && tc::available() && effective(c->opt.pw) == IMPL_TC && c->d_irf_image) {
       // xif2_0: expand 1x1 -> depthwise 3x3 s2 -> project 1x1 in ONE kernel; the expanded tensor stays on the SM
       LaunchScope scope(c, ST_BACKBONE_PW, s);
-      int r = tc::launch_irf_s2(s, X, Y, c->d_irf_image, B, h, w);
+      int r = tc::launch_irf_s2(s, X, Y, c->d_irf_image, B, h, w, tc::num_sms());
       if (r < 0) return set_err(FEAR_EINVAL, "fused IRF block launch failed (%d)", r);
       if (r == 1) scope.cancel();
       if (r == 0) {

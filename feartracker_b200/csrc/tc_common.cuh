@@ -126,15 +126,17 @@ inline int make_tmap_2d(CUtensorMap* m, const float* base, uint64_t rows, uint64
                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
-// 4-D fp32 channels-last activation tensor [B][H][W][C] (dims listed innermost first: C, W, H, B), no swizzle.
-// The box may start at negative / end at out-of-range coordinates: TMA zero-fills those elements, which is
-// exactly the zero padding of a "same" convolution (and it still counts the full box bytes on the mbarrier).
+// 4-D fp32 channels-last activation tensor [B][H][W][C] (dims listed innermost first: C, W, H, B), unswizzled
+// unless `sw` says otherwise.  The box may start at negative / end at out-of-range coordinates: TMA zero-fills those
+// elements, which is exactly the zero padding of a "same" convolution (and it still counts the full box bytes on the
+// mbarrier).
 inline int make_tmap_nhwc(CUtensorMap* m, const float* base, uint64_t B, uint64_t H, uint64_t W, uint64_t C,
-                          uint32_t box_c, uint32_t box_w, uint32_t box_h) {
+                          uint32_t box_c, uint32_t box_w, uint32_t box_h,
+                          CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_NONE) {
   cuuint64_t dims[4] = {C, W, H, B};
   cuuint64_t strides[3] = {C * sizeof(float), W * C * sizeof(float), H * W * C * sizeof(float)};
   cuuint32_t box[4] = {box_c, box_w, box_h, 1};
-  return encode_cached(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+  return encode_cached(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, dims, strides, box, sw,
                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 
