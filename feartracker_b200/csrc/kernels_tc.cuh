@@ -176,142 +176,81 @@ inline int launch_corr(cudaStream_t s, const float* zt, int Bz, float* cat, int 
 // ------------------------------------------------------------------------------------------
 // pw_tc_kernel -- 1x1 convolution as a GEMM on wgmma:  C[M][N] = act(A[M][K] * W[N][K]^T + bias (+ R))
 // A = channels-last activations (rows = pixels), W = BN-folded torch-native [Cout][Cin] weights,
-// pre-split on the host into tf32 (hi, lo) copies; A is split in registers.  One CTA per (m_tile, n_tile) pair,
-// n fastest; tile = 128 pixels x NT output channels.  TMA zero-fills the K tail (Cin not a multiple of 32),
-// rows >= M and weight rows >= N; the epilogue clips the M / N tails.
+// pre-split on the host into tf32 (hi, lo) copies; A is split in registers.  Tile = 128 pixels x NT output channels;
+// tile index = m_tile * num_n_tiles + n_tile (n fastest: the n-tiles of one m-tile run together and share A in L2).
+// TMA zero-fills the K tail (Cin not a multiple of 32), rows >= M and weight rows >= N; the epilogue clips the M / N tails.
 // ------------------------------------------------------------------------------------------
 struct PwParams {
   const float* bias;  // [N] or null
   const float* R;     // residual [M][ldr] or null
   float* C;
   int ldr, ldc;
-  int M, N, num_n_tiles, num_chunks, last_ksteps, relu, stages, stage_bytes;
+  int M, N, num_n_tiles, num_tiles, num_chunks, last_ksteps, relu, stages, stage_bytes;
   // --- fused depthwise producer (DWK = 3 | 5): the A operand is dw(X) computed on the fly ---
   int dw_relu, dw_bias;  // ReLU / bias of the depthwise stage
   int box_bytes;         // bytes of one (tile rows + DWK - 1) x (map width + DWK - 1) x 32-channel input box
 };
 
-// DWK = 0: plain 1x1 conv.  DWK = 3 | 5 (option "fuse_dwpw", on by default; MW x MW maps with MW = 16 | 32, stride 1): the
-// layer's input is the output of a DWK x DWK depthwise conv that is never materialised -- the producer TMA-loads the
-// depthwise INPUT box of each (128-pixel tile, 32-channel chunk) with its zero-filled halo (tmA is then the 4-D NHWC
-// map of X), the consumer warps run the depthwise conv out of shared memory (same FMA order as dw_tma_kernel => same
-// fp32 values as the unfused pair of kernels) and write the A tile in the SWIZZLE_128B layout the fragment loads expect.
-template <int NT, int DWK, int MW = 16>
-__global__ void __launch_bounds__(kTcThreads, 1)
-pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWh,
-             const __grid_constant__ CUtensorMap tmWl, const __grid_constant__ CUtensorMap tmDW,
-             const __grid_constant__ CUtensorMap tmDB, const PwParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int S = p.stages;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * p.stage_bytes);
-  uint64_t* empty = full + S;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int w_bytes = NT * 128;
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmWh);
-    prefetch_tmap(&tmWl);
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);
+// Warp-specialised CTA: warpgroup 0 is the TMA producer and keeps kPwProducerRegs registers per thread, warpgroups 1-2
+// are the consumers and take the rest: 128 * 40 + 256 * 232 = 64 512 of the SM's 65 536.  The consumers' budget holds
+// 128 accumulators (NT = 128) plus the A fragments of two chunks whose MMA groups are in flight at once.
+constexpr int kPwThreads = 384;
+constexpr int kPwProducerRegs = 40, kPwConsumerRegs = 232;
+
+// The 3xTF32 products of one 32-channel chunk, KS K steps in K order (KS < 4 only for the K tail, whose all-zero
+// K steps are skipped).  One straight-line issue sequence per KS: no wgmma sits behind a per-step branch.
+template <int NT, int KS>
+__device__ __forceinline__ void mma3_chunk(float* accm, float* accc, const uint32_t (&hi)[4][4], const uint32_t (&lo)[4][4],
+                                           uint32_t bh, uint32_t bl) {
+#pragma unroll
+  for (int j = 0; j < KS; ++j) mma3<NT>(accm, accc, hi[j], lo[j], bh + j * 32, bl + j * 32);
+}
+
+// Depthwise K x K conv (stride 1, MW x MW map) of one 32-channel chunk of a 128-pixel tile, from the landed input box
+// (halo included) into the A tile in the SWIZZLE_128B layout the fragment loads expect.  ct = consumer thread (0..255)
+// = (2-channel pair, 1 x 8 pixel strip); 16 strips cover the tile.  Same FMA order as dw_tma_kernel.
+template <int K, int MW>
+__device__ __forceinline__ void dw_chunk(const uint8_t* box, const uint8_t* wts, const uint8_t* bia, uint8_t* at, int ct,
+                                         int dw_bias, int dw_relu) {
+  constexpr int TX = 8, NIN = TX + K - 1, IW = MW + K - 1, PXN = MW / TX;
+  typedef unsigned long long U2;  // two packed fp32 channels
+  const int c2 = ct & 15, pos = ct >> 4;
+  const int x0 = (pos % PXN) * TX, y0 = pos / PXN;
+  const U2* in2 = reinterpret_cast<const U2*>(box) + (y0 * IW + x0) * 16 + c2;
+  const U2* w2 = reinterpret_cast<const U2*>(wts) + c2;
+  const U2 bias2 = dw_bias ? reinterpret_cast<const U2*>(bia)[c2] : 0ull;
+  U2 acc[TX];
+#pragma unroll
+  for (int i = 0; i < TX; ++i) acc[i] = bias2;
+#pragma unroll
+  for (int ky = 0; ky < K; ++ky) {
+    U2 v[NIN];
+#pragma unroll
+    for (int i = 0; i < NIN; ++i) v[i] = in2[(ky * IW + i) * 16];
+#pragma unroll
+    for (int kx = 0; kx < K; ++kx) {
+      const U2 k = w2[(ky * K + kx) * 16];
+#pragma unroll
+      for (int i = 0; i < TX; ++i) ffma2(acc[i], v[i + kx], k);
     }
-    fence_mbar_init();
   }
-  __syncthreads();
-  pdl_trigger();  // the next kernel may start its prologue on SMs we have left
-  pdl_wait();     // everything above overlapped the previous kernel's tail; its results are visible from here on
-
-  const int mt = blockIdx.x / p.num_n_tiles, nt = blockIdx.x - mt * p.num_n_tiles;
-  // stage: [A tile 16 KB][w_hi][w_lo] (+ fused depthwise: [input box][dw weights DWK*DWK x 32][dw bias 32])
-  auto a_tile = [&](int s) { return smem + s * p.stage_bytes; };
-  auto w_hi = [&](int s) { return smem + s * p.stage_bytes + kCorrABytes; };
-  auto w_lo = [&](int s) { return w_hi(s) + w_bytes; };
-  auto dw_box = [&](int s) { return w_lo(s) + w_bytes; };
-  auto dw_wts = [&](int s) { return dw_box(s) + p.box_bytes; };
-  auto dw_bia = [&](int s) { return dw_wts(s) + DWK * DWK * 128; };
-
-  if (warp == 8) {
-    if (lane == 0) {
-      constexpr int th = 128 / MW, tpf = MW / th;  // tile rows, tiles per frame
-      for (int c = 0; c < p.num_chunks; ++c) {
-        const int stage = c % S;
-        mbar_wait_backoff(&empty[stage], (uint32_t)(((c / S) & 1) ^ 1));
-        if constexpr (DWK > 0) {
-          mbar_arrive_expect_tx(&full[stage], 2 * w_bytes + p.box_bytes + DWK * DWK * 128 + (p.dw_bias ? 128 : 0));
-          tma_load_4d(dw_box(stage), &tmA, &full[stage], c * 32, -(DWK / 2), (mt % tpf) * th - DWK / 2, mt / tpf);
-          tma_load_2d(dw_wts(stage), &tmDW, &full[stage], c * 32, 0);
-          if (p.dw_bias) tma_load_2d(dw_bia(stage), &tmDB, &full[stage], c * 32, 0);
-        } else {
-          mbar_arrive_expect_tx(&full[stage], kCorrABytes + 2 * w_bytes);
-          tma_load_2d(a_tile(stage), &tmA, &full[stage], c * 32, mt * 128);
-        }
-        tma_load_2d(w_hi(stage), &tmWh, &full[stage], c * 32, nt * NT);
-        tma_load_2d(w_lo(stage), &tmWl, &full[stage], c * 32, nt * NT);
-      }
+#pragma unroll
+  for (int i = 0; i < TX; ++i) {
+    float2 v = make_float2(__uint_as_float((uint32_t)acc[i]), __uint_as_float((uint32_t)(acc[i] >> 32)));
+    if (dw_relu) {
+      v.x = fmaxf(v.x, 0.f);
+      v.y = fmaxf(v.y, 0.f);
     }
-    return;
+    const int R = y0 * MW + x0 + i;  // A-tile row = pixel inside the tile
+    *reinterpret_cast<float2*>(at + R * 128 + (((c2 >> 1) ^ (R & 7)) << 4) + ((c2 & 1) << 3)) = v;
   }
+}
 
-  const int wg = warp >> 2, r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), t = lane & 3;
-  float accm[NT / 2], accc[NT / 2];
-#pragma unroll
-  for (int i = 0; i < NT / 2; ++i) accm[i] = accc[i] = 0.f;
-  for (int c = 0; c < p.num_chunks; ++c) {
-    const int stage = c % S;
-    mbar_wait(&full[stage], (uint32_t)((c / S) & 1));
-    if constexpr (DWK > 0) {
-      // thread = (2-channel pair, 1 x 8 pixel strip); 16 strips cover the 128-pixel tile
-      constexpr int K = DWK, TX = 8, NIN = TX + K - 1, IW = MW + K - 1, PXN = MW / TX;
-      typedef unsigned long long U2;  // two packed fp32 channels
-      const int c2 = threadIdx.x & 15, pos = threadIdx.x >> 4;
-      const int x0 = (pos % PXN) * TX, y0 = pos / PXN;
-      const U2* in2 = reinterpret_cast<const U2*>(dw_box(stage)) + (y0 * IW + x0) * 16 + c2;
-      const U2* w2 = reinterpret_cast<const U2*>(dw_wts(stage)) + c2;
-      const U2 bias2 = p.dw_bias ? reinterpret_cast<const U2*>(dw_bia(stage))[c2] : 0ull;
-      U2 acc[TX];
-#pragma unroll
-      for (int i = 0; i < TX; ++i) acc[i] = bias2;
-#pragma unroll
-      for (int ky = 0; ky < K; ++ky) {
-        U2 v[NIN];
-#pragma unroll
-        for (int i = 0; i < NIN; ++i) v[i] = in2[(ky * IW + i) * 16];
-#pragma unroll
-        for (int kx = 0; kx < K; ++kx) {
-          const U2 k = w2[(ky * K + kx) * 16];
-#pragma unroll
-          for (int i = 0; i < TX; ++i) ffma2(acc[i], v[i + kx], k);
-        }
-      }
-      uint8_t* at = a_tile(stage);
-#pragma unroll
-      for (int i = 0; i < TX; ++i) {
-        float2 v = make_float2(__uint_as_float((uint32_t)acc[i]), __uint_as_float((uint32_t)(acc[i] >> 32)));
-        if (p.dw_relu) {
-          v.x = fmaxf(v.x, 0.f);
-          v.y = fmaxf(v.y, 0.f);
-        }
-        const int R = y0 * MW + x0 + i;  // A-tile row = pixel inside the tile
-        *reinterpret_cast<float2*>(at + R * 128 + (((c2 >> 1) ^ (R & 7)) << 4) + ((c2 & 1) << 3)) = v;
-      }
-      consumer_sync();  // the A tile of this chunk is complete (and every warp has left the previous chunk's)
-    }
-    uint32_t hi[4][4], lo[4][4];
-    load_a_frags(a_tile(stage), r0, t, hi, lo);
-    const uint32_t bh = smem_u32(w_hi(stage)), bl = smem_u32(w_lo(stage));
-    const int ksteps = (c == p.num_chunks - 1) ? p.last_ksteps : 4;  // K tail: skip all-zero K-steps
-    wg_fence();
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (j < ksteps) mma3<NT>(accm, accc, hi[j], lo[j], bh + j * 32, bl + j * 32);
-    wg_commit();
-    wg_wait();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[stage]);
-  }
-
-  // epilogue: (main + corr) + bias (+ residual), ReLU, 8-byte stores (4 lanes cover one 32-byte sector)
+// Epilogue of one tile: (main + corr) + bias (+ residual), ReLU, 8-byte stores straight from the accumulator registers
+// (4 lanes cover one 32-byte sector).
+template <int NT>
+__device__ __forceinline__ void pw_epilogue(const PwParams& p, const float* accm, const float* accc, int mt, int nt, int r0,
+                                            int t) {
   const int n0 = nt * NT + 2 * t;
 #pragma unroll
   for (int hrow = 0; hrow < 2; ++hrow) {
@@ -339,8 +278,224 @@ pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   }
 }
 
+// DWK = 0: plain 1x1 conv.  DWK = 3 | 5 (option "fuse_dwpw", on by default; MW x MW maps with MW = 16 | 32, stride 1): the
+// layer's input is the output of a DWK x DWK depthwise conv that is never materialised -- the producer TMA-loads the
+// depthwise INPUT box of each (128-pixel tile, 32-channel chunk) with its zero-filled halo (tmA is then the 4-D NHWC
+// map of X), the consumer warps run the depthwise conv out of shared memory (dw_chunk) and write the A tile.
+//
+// Persistent: min(tiles, SMs) CTAs, CTA c walks tiles c, c + G, c + 2G, ...  The producer streams the CTA's whole
+// chunk sequence through the mbarrier ring without regard to tile boundaries, so the next tile's first chunks land while
+// the consumers finish and store the current one; stage and parity advance over that sequence.  Both consumer
+// warpgroups share each tile (64 rows each, weights fetched once per 128 rows).  A consumer issues chunk c's MMA group
+// and then waits only for chunk c - 1's (wgmma.wait_group 1), which frees c - 1's stage and A fragments; in the fused
+// forms chunk c + 1's depthwise conv runs while chunk c's group is in flight.  wait_group 0 only before the epilogue.
+template <int NT, int DWK, int MW = 16>
+__global__ void __launch_bounds__(kPwThreads, 1)
+pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWh,
+             const __grid_constant__ CUtensorMap tmWl, const __grid_constant__ CUtensorMap tmDW,
+             const __grid_constant__ CUtensorMap tmDB, const PwParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const int S = p.stages;
+  constexpr int a_bufs = DWK > 0 ? 2 : 0;  // fused: the A tiles the consumers write live outside the ring
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * p.stage_bytes + a_bufs * kCorrABytes);  // [stages] TMA landed
+  uint64_t* empty = full + S;  // [stages] 8 consumer warps done
+  constexpr int w_bytes = NT * 128;
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmWh);
+    prefetch_tmap(&tmWl);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_trigger();  // the next kernel may start its prologue on SMs we have left
+  pdl_wait();     // everything above overlapped the previous kernel's tail; its results are visible from here on
+
+  // plain stage: [A tile 16 KB][w_hi][w_lo]; fused stage: [w_hi][w_lo][input box][dw weights DWK*DWK x 32][dw bias 32],
+  // then two A tiles after the ring.  A fused A tile is free once every consumer has loaded its fragments, long
+  // before the stage's weights are (their MMAs still run), so two of them serve any ring depth and the room they
+  // leave buys the ring a third stage.
+  auto a_tile = [&](int s) { return smem + s * p.stage_bytes; };
+  auto a_buf = [&](int b) { return smem + S * p.stage_bytes + b * kCorrABytes; };
+  auto w_hi = [&](int s) { return smem + s * p.stage_bytes + (DWK > 0 ? 0 : kCorrABytes); };
+  auto w_lo = [&](int s) { return w_hi(s) + w_bytes; };
+  auto dw_box = [&](int s) { return w_lo(s) + w_bytes; };
+  auto dw_wts = [&](int s) { return dw_box(s) + p.box_bytes; };
+  auto dw_bia = [&](int s) { return dw_wts(s) + DWK * DWK * 128; };
+
+  // Warpgroup index broadcast from lane 0: the compiler can prove it uniform, so no wgmma below is on a divergent path.
+  const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0);
+  if (wg == 0) {
+    setmaxnreg_dec<kPwProducerRegs>();
+    if (threadIdx.x == 0) {
+      constexpr int th = 128 / MW, tpf = MW / th;  // tile rows, tiles per frame
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
+        for (int c = 0; c < p.num_chunks; ++c) {
+          mbar_wait_backoff(&empty[stage], phase ^ 1);
+          if constexpr (DWK > 0) {
+            mbar_arrive_expect_tx(&full[stage], 2 * w_bytes + p.box_bytes + DWK * DWK * 128 + (p.dw_bias ? 128 : 0));
+            tma_load_4d(dw_box(stage), &tmA, &full[stage], c * 32, -(DWK / 2), (mt % tpf) * th - DWK / 2, mt / tpf);
+            tma_load_2d(dw_wts(stage), &tmDW, &full[stage], c * 32, 0);
+            if (p.dw_bias) tma_load_2d(dw_bia(stage), &tmDB, &full[stage], c * 32, 0);
+          } else {
+            mbar_arrive_expect_tx(&full[stage], kCorrABytes + 2 * w_bytes);
+            tma_load_2d(a_tile(stage), &tmA, &full[stage], c * 32, mt * 128);
+          }
+          tma_load_2d(w_hi(stage), &tmWh, &full[stage], c * 32, nt * NT);
+          tma_load_2d(w_lo(stage), &tmWl, &full[stage], c * 32, nt * NT);
+          if (++stage == S) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<kPwConsumerRegs>();
+
+  const int ct = threadIdx.x - 128, warp = ct >> 5, lane = ct & 31;  // consumer thread / warp (0..255 / 0..7)
+  const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), t = lane & 3;
+  int stage = 0, ab = 0;  // ring stage, fused A buffer of the current chunk
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
+    float accm[NT / 2], accc[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) accm[i] = accc[i] = 0.f;
+    if constexpr (DWK > 0) {
+      mbar_wait(&full[stage], phase);
+      dw_chunk<DWK, MW>(dw_box(stage), dw_wts(stage), dw_bia(stage), a_buf(ab), ct, p.dw_bias, p.dw_relu);
+      consumer_sync();  // the A tile of this chunk is complete
+    }
+    int prev = 0;
+    for (int c = 0; c < p.num_chunks; ++c) {
+      if constexpr (DWK == 0) mbar_wait(&full[stage], phase);
+      uint32_t hi[4][4], lo[4][4];
+      load_a_frags(DWK > 0 ? a_buf(ab) : a_tile(stage), r0, t, hi, lo);
+      const uint32_t bh = smem_u32(w_hi(stage)), bl = smem_u32(w_lo(stage));
+      const int ksteps = (c == p.num_chunks - 1) ? p.last_ksteps : 4;
+      wg_fence();
+      if (ksteps == 4) mma3_chunk<NT, 4>(accm, accc, hi, lo, bh, bl);
+      else if (ksteps == 3) mma3_chunk<NT, 3>(accm, accc, hi, lo, bh, bl);
+      else if (ksteps == 2) mma3_chunk<NT, 2>(accm, accc, hi, lo, bh, bl);
+      else mma3_chunk<NT, 1>(accm, accc, hi, lo, bh, bl);
+      wg_commit();
+      if (c > 0) {  // chunk c - 1's group is done: its stage may be refilled
+        wg_wait_n<1>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = stage;
+      if (++stage == S) {
+        stage = 0;
+        phase ^= 1;
+      }
+      if constexpr (DWK > 0) {
+        ab ^= 1;  // its last reader loaded chunk c - 1's fragments before the previous consumer_sync
+        if (c + 1 < p.num_chunks) {  // the next chunk's depthwise conv, while this chunk's MMAs run
+          mbar_wait(&full[stage], phase);
+          dw_chunk<DWK, MW>(dw_box(stage), dw_wts(stage), dw_bia(stage), a_buf(ab), ct, p.dw_bias, p.dw_relu);
+          consumer_sync();
+        }
+      }
+    }
+    wg_wait_n<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    pw_epilogue<NT>(p, accm, accc, mt, nt, r0, t);
+  }
+}
+
+// One-chunk GEMMs (K <= 32) on narrow tiles: one CTA per tile, 288 threads (two consumer warpgroups and one TMA
+// producer warp), no persistence.  Such a CTA loads its A and W tiles, issues one group of MMAs and stores its tile;
+// at NT <= 32 it needs 68 registers per thread, three CTAs share an SM and one CTA's loads and stores overlap another's
+// MMAs, which the persistent kernel (one CTA per SM, its consumers' epilogue between two tiles' MMAs) does not match at
+// these shapes.  Same mma3 sequence per output element and same epilogue as pw_tc_kernel.
+template <int NT>
+__global__ void __launch_bounds__(kTcThreads, 1)
+pw_tc_narrow_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWh,
+                    const __grid_constant__ CUtensorMap tmWl, const PwParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const int S = p.stages;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * p.stage_bytes);
+  uint64_t* empty = full + S;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int w_bytes = NT * 128;
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmWh);
+    prefetch_tmap(&tmWl);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_trigger();
+  pdl_wait();
+
+  const int mt = blockIdx.x / p.num_n_tiles, nt = blockIdx.x - mt * p.num_n_tiles;
+  auto a_tile = [&](int s) { return smem + s * p.stage_bytes; };
+  auto w_hi = [&](int s) { return smem + s * p.stage_bytes + kCorrABytes; };
+  auto w_lo = [&](int s) { return w_hi(s) + w_bytes; };
+
+  if (warp == 8) {
+    if (lane == 0) {
+      for (int c = 0; c < p.num_chunks; ++c) {
+        const int stage = c % S;
+        mbar_wait_backoff(&empty[stage], (uint32_t)(((c / S) & 1) ^ 1));
+        mbar_arrive_expect_tx(&full[stage], kCorrABytes + 2 * w_bytes);
+        tma_load_2d(a_tile(stage), &tmA, &full[stage], c * 32, mt * 128);
+        tma_load_2d(w_hi(stage), &tmWh, &full[stage], c * 32, nt * NT);
+        tma_load_2d(w_lo(stage), &tmWl, &full[stage], c * 32, nt * NT);
+      }
+    }
+    return;
+  }
+
+  const int wg = warp >> 2, r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), t = lane & 3;
+  float accm[NT / 2], accc[NT / 2];
+#pragma unroll
+  for (int i = 0; i < NT / 2; ++i) accm[i] = accc[i] = 0.f;
+  for (int c = 0; c < p.num_chunks; ++c) {
+    const int stage = c % S;
+    mbar_wait(&full[stage], (uint32_t)((c / S) & 1));
+    uint32_t hi[4][4], lo[4][4];
+    load_a_frags(a_tile(stage), r0, t, hi, lo);
+    const uint32_t bh = smem_u32(w_hi(stage)), bl = smem_u32(w_lo(stage));
+    const int ksteps = (c == p.num_chunks - 1) ? p.last_ksteps : 4;  // K tail: skip all-zero K-steps
+    wg_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (j < ksteps) mma3<NT>(accm, accc, hi[j], lo[j], bh + j * 32, bl + j * 32);
+    wg_commit();
+    wg_wait();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);
+  }
+  pw_epilogue<NT>(p, accm, accc, mt, nt, r0, t);
+}
+
 constexpr int kPwMaxSmem = 232448 - 1024;  // 227 KB opt-in limit minus static/driver slack
-constexpr int kPwMaxStages = 3;
+constexpr int kPwMaxStages = 4;
+constexpr int kPwSmemExtra = 1024 /*align*/ + 256 /*barriers*/;
+
+// Ring depth of the persistent kernel: as many stages of `stage_bytes` as fit next to `fixed_bytes`, at most
+// kPwMaxStages (the ring spans tile boundaries, so even a one- or two-chunk layer fills every stage).
+inline int pw_stages(int stage_bytes, int fixed_bytes) {
+  const int fit = (kPwMaxSmem - kPwSmemExtra - fixed_bytes) / stage_bytes;
+  return fit < kPwMaxStages ? fit : kPwMaxStages;
+}
 
 // Output-channel tile for a layer: the layer is cut into the fewest tiles of <= 128 columns (two accumulators of
 // NT / 2 registers per thread), each the narrowest instantiated width that covers its share; the last tile may hang
@@ -358,11 +513,10 @@ inline bool pw_supported(int cin, int cout) { return available() && cin % 8 == 0
 
 #define FEAR_PW_FOR_NT(X) X(16) X(32) X(48) X(64) X(96) X(112) X(128)
 
-// A GEMM with one K chunk (K <= 32) does little work per CTA, and one CTA per SM runs its TMA load, MMAs and epilogue
-// stores strictly one after another.  Such layers are cut into tiles of at most kPwNarrowNT columns instead: the
-// kernel at NT = 32 needs 68 registers per thread (against 135 at NT = 96), so three CTAs share an SM and one CTA's
-// loads and stores overlap another's MMAs.  The A tile is then read once per n-tile, mostly from L2.  The tile width
-// does not change any output element's sequence of mma3 products, so results are the same bit for bit.
+// A GEMM with one K chunk (K <= 32) does little work per tile.  Such layers are cut into tiles of at most kPwNarrowNT
+// columns and run on pw_tc_narrow_kernel, several CTAs per SM.  The A tile is then read once per n-tile, mostly from
+// L2.  The tile width does not change any output element's sequence of mma3 products, so results are the same bit
+// for bit.
 constexpr int kPwNarrowNT = 32;
 inline int pw_tile_n_one_chunk(int N) {
   const int Np = (N + 15) & ~15;
@@ -381,12 +535,17 @@ inline int init_pw() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_kernel<NT_, 5, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem);
   FEAR_PW_FOR_NT(FEAR_PW_ATTR)
 #undef FEAR_PW_ATTR
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_narrow_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(pw_tc_narrow_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwMaxSmem);
   if (e != cudaSuccess) {
     cudaGetLastError();
     return -1;
   }
   return 0;
 }
+
+// Persistent grid: one CTA per SM at most.
+inline dim3 pw_grid(int tiles) { return dim3(tiles < num_sms() ? tiles : num_sms()); }
 
 // w_hi / w_lo: tf32-split copies of the [N][K] weights (device).
 inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi, const float* w_lo, const float* bias,
@@ -401,14 +560,16 @@ inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi,
   p.M = M;
   p.N = N;
   p.num_chunks = (K + 31) / 32;
-  const int NT = p.num_chunks == 1 ? pw_tile_n_one_chunk(N) : pw_tile_n(N);
+  const bool narrow = p.num_chunks == 1;
+  const int NT = narrow ? pw_tile_n_one_chunk(N) : pw_tile_n(N);
   if (!NT) return -21;
   p.num_n_tiles = (((N + 15) & ~15) + NT - 1) / NT;
+  p.num_tiles = ((M + 127) / 128) * p.num_n_tiles;
   p.last_ksteps = ((K - 32 * (p.num_chunks - 1)) + 7) / 8;
   p.relu = relu;
   p.dw_relu = p.dw_bias = p.box_bytes = 0;
   p.stage_bytes = kCorrABytes + 2 * NT * 128;
-  p.stages = p.num_chunks < kPwMaxStages ? p.num_chunks : kPwMaxStages;
+  p.stages = narrow ? 1 : pw_stages(p.stage_bytes, 0);
   CUtensorMap tmA, tmWh, tmWl;
   int r = make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 128, 32);
   if (r) return r;
@@ -416,13 +577,17 @@ inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi,
   if (r) return r;
   r = make_tmap_2d(&tmWl, w_lo, (uint64_t)N, (uint64_t)K, (uint64_t)K, NT, 32);
   if (r) return r;
-  const int tiles = ((M + 127) / 128) * p.num_n_tiles;
-  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 1024 + 256;
+  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + kPwSmemExtra;
   cudaError_t e = cudaErrorInvalidValue;
+  if (narrow) {
+    if (NT == 16) e = launch_pdl(pw_tc_narrow_kernel<16>, dim3(p.num_tiles), dim3(kTcThreads), smem_bytes, s, tmA, tmWh, tmWl, p);
+    else e = launch_pdl(pw_tc_narrow_kernel<32>, dim3(p.num_tiles), dim3(kTcThreads), smem_bytes, s, tmA, tmWh, tmWl, p);
+    return e == cudaSuccess ? 0 : -23;
+  }
   switch (NT) {
-#define FEAR_PW_CASE(NT_)                                                                                                     \
-  case NT_:                                                                                                                   \
-    e = launch_pdl(pw_tc_kernel<NT_, 0>, dim3(tiles), dim3(kTcThreads), smem_bytes, s, tmA, tmWh, tmWl, tmA, tmA, p); \
+#define FEAR_PW_CASE(NT_)                                                                                               \
+  case NT_:                                                                                                             \
+    e = launch_pdl(pw_tc_kernel<NT_, 0>, pw_grid(p.num_tiles), dim3(kPwThreads), smem_bytes, s, tmA, tmWh, tmWl, tmA, tmA, p); \
     break;
     FEAR_PW_FOR_NT(FEAR_PW_CASE)
 #undef FEAR_PW_CASE
@@ -432,7 +597,9 @@ inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi,
 
 // Depthwise-fused GEMM (option "fuse_dwpw", default on; tests/test_gpu_parity.py): 1x1 conv whose input is dw_k x dw_k depthwise(X)
 // (+bias, ReLU), X = [B][map_w][map_w][K] channels-last, stride 1.  out = act(dw(X) * W^T + bias (+R)).
-// Returns 1 when the shape is not covered (caller runs the two kernels separately).
+// Returns 1 when the shape is not covered (caller runs the two kernels separately): the shape is taken when two stages
+// of [A tile | weights | box] (one for a one-chunk layer) fit in shared memory.  The kernel's ring of [weights | box]
+// stages next to two A tiles then has at least as many stages, up to kPwMaxStages.
 inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const float* dw_w, const float* dw_b, int dw_relu,
                         const float* w_hi, const float* w_lo, const float* bias, const float* R, int ldr, float* C,
                         int ldc, int N, int K, int relu, int map_w = 16) {
@@ -451,16 +618,17 @@ inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const f
   const int NT = pw_tile_n(N);
   if (!NT) return 1;
   p.num_n_tiles = (((N + 15) & ~15) + NT - 1) / NT;
+  p.num_tiles = (M / 128) * p.num_n_tiles;
   p.last_ksteps = ((K - 32 * (p.num_chunks - 1)) + 7) / 8;
   p.relu = relu;
   p.dw_relu = dw_relu;
   p.dw_bias = dw_b != nullptr;
   const int ih = 128 / map_w + dw_k - 1, iw = map_w + dw_k - 1;
   p.box_bytes = ih * iw * 128;
-  p.stage_bytes = (kCorrABytes + 2 * NT * 128 + p.box_bytes + dw_k * dw_k * 128 + 128 + 1023) & ~1023;
-  p.stages = p.num_chunks < 2 ? 1 : 2;
-  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 1024 + 256;
-  if ((int)smem_bytes > kPwMaxSmem) return 1;
+  p.stage_bytes = (2 * NT * 128 + p.box_bytes + dw_k * dw_k * 128 + 128 + 1023) & ~1023;
+  if ((p.num_chunks < 2 ? 1 : 2) * (kCorrABytes + p.stage_bytes) + kPwSmemExtra > kPwMaxSmem) return 1;
+  p.stages = pw_stages(p.stage_bytes, 2 * kCorrABytes);
+  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 2 * kCorrABytes + kPwSmemExtra;
   CUtensorMap tmX, tmWh, tmWl, tmDW, tmDB;
   int r = make_tmap_nhwc(&tmX, X, (uint64_t)B, (uint64_t)map_w, (uint64_t)map_w, (uint64_t)K, 32, iw, ih);
   if (r) return r;
@@ -476,10 +644,9 @@ inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const f
   } else {
     tmDB = tmDW;
   }
-  const int tiles = (M / 128) * p.num_n_tiles;
   cudaError_t e = cudaErrorInvalidValue;
 #define FEAR_PW_DW_LAUNCH(NT_, K_, MW_) \
-  e = launch_pdl(pw_tc_kernel<NT_, K_, MW_>, dim3(tiles), dim3(kTcThreads), smem_bytes, s, tmX, tmWh, tmWl, tmDW, tmDB, p)
+  e = launch_pdl(pw_tc_kernel<NT_, K_, MW_>, pw_grid(p.num_tiles), dim3(kPwThreads), smem_bytes, s, tmX, tmWh, tmWl, tmDW, tmDB, p)
   switch (NT) {
 #define FEAR_PW_CASE(NT_)                                \
   case NT_:                                              \
