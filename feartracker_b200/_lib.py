@@ -47,6 +47,10 @@ assert YCBCR_DTYPE.itemsize == 88
 # FearFrameYCbCrV210: FearFrameYCbCr plus whether the entry is a v210 surface (10-bit 4:2:2, three codes per word)
 YCBCR_V210_DTYPE = np.dtype(YCBCR_DTYPE.descr + [("v210", "<i4"), ("reserved", "<i4")])
 assert YCBCR_V210_DTYPE.itemsize == 96
+# FearFrameBayer: a raw Bayer mosaic (unpacked 8 to 16 bits, MIPI RAW10 / RAW12) with its row pitch and CFA pattern
+BAYER_DTYPE = np.dtype([("data", "<u8"), ("row_stride", "<i8"), ("H", "<i4"), ("W", "<i4"), ("pattern", "<i4"),
+                        ("bits", "<i4"), ("shift", "<i4"), ("packing", "<i4")])
+assert BAYER_DTYPE.itemsize == 40
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -85,6 +89,9 @@ _SIGNATURES = {
     "fear_crop_targets_ycbcr_v210_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_ycbcr_v210": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_ycbcr_v210_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_bayer_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_bayer": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_bayer_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_decode_smooth": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),

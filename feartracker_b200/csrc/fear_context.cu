@@ -1050,6 +1050,8 @@ static_assert(sizeof(FearFrameYUV) == 80, "FearFrameYUV layout is part of the AB
 static_assert(sizeof(FearFrameYCbCr) == 88, "FearFrameYCbCr layout is part of the ABI");
 static_assert(sizeof(FearFrameYCbCrV210) == 96 && offsetof(FearFrameYCbCrV210, v210) == 88,
               "FearFrameYCbCrV210 layout is part of the ABI");
+static_assert(sizeof(FearFrameBayer) == 40 && offsetof(FearFrameBayer, packing) == 36,
+              "FearFrameBayer layout is part of the ABI");
 
 static int check_crop_targets_args(int F, int N, double offset, int out_size) {
   if (N < 1 || N > 65535) return set_err(FEAR_EINVAL, "target count must be in [1, 65535] (got %d)", N);
@@ -1208,6 +1210,25 @@ extern "C" int fear_advance_targets_ycbcr_v210(const FearBox* d_boxes, const Fea
 extern "C" int fear_frame_sums_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, uint64_t* d_sums,
                                              void* stream) {
   return launch_frame_sums(d_views, YCbCrV210Frames{d_views}, F, d_sums, stream);
+}
+
+// Raw Bayer mosaics: the same kernels, reading through BayerFrames (each tap demosaiced as cv2.cvtColor does).
+extern "C" int fear_crop_targets_bayer_u8(const FearFrameBayer* d_views, int F, FearTarget* d_targets, int N,
+                                          double offset, int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_views || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(BayerFrames{d_views}, F, d_targets, N, offset, out_size, d_crops, stream);
+}
+
+extern "C" int fear_advance_targets_bayer(const FearBox* d_boxes, const FearFrameBayer* d_views, int F,
+                                          FearTarget* d_targets, int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_views || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return launch_advance_targets(d_boxes, BayerFrames{d_views}, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_frame_sums_bayer_u8(const FearFrameBayer* d_views, int F, uint64_t* d_sums, void* stream) {
+  return launch_frame_sums(d_views, BayerFrames{d_views}, F, d_sums, stream);
 }
 
 extern "C" int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,

@@ -13,9 +13,10 @@
 // through TrackFrame; or a table of YUV frames, FearFrameYUV420 (YUV420Frames, 4:2:0, 8-bit BT.601 limited range),
 // FearFrameYUV (YUVFrames, 4:2:0, the format named per entry) or FearFrameYCbCr (YCbCrFrames, 4:2:0, 4:2:2 or 4:4:4 and
 // the format named per entry), all read through YUVFrame, which converts each pixel it reads to RGB; or a table of
-// FearFrameYCbCrV210 records (YCbCrV210Frames), read through V210Frame, which also unpacks v210 surfaces.  A frame type
-// gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables, interpolation, sums
-// and the colour conversion exist once.
+// FearFrameYCbCrV210 records (YCbCrV210Frames), read through V210Frame, which also unpacks v210 surfaces; or a table of
+// FearFrameBayer records (BayerFrames), read through BayerFrame, which demosaics raw Bayer mosaics.  A frame type gives
+// H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables, interpolation, sums and
+// the colour conversion exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
 // into an FMA by default, which rounds once instead of twice, so every multiply-add here is spelled with the explicitly
@@ -262,6 +263,88 @@ struct YCbCrV210Frames {
     return V210Frame{{y, y, y, pitch, 0, 0, 0, v.H, v.W, 1, 0, 10, 0, true, true, !ok,
                       ok ? yuv_coefs(v.matrix, v.full_range, 10) : YUVCoefs{}},
                      true};
+  }
+};
+
+// A raw Bayer mosaic (FearFrameBayer): rgb(y, x) demosaics the pixel as cv2.cvtColor(COLOR_Bayer*2RGB) does, from the
+// codes of its 3 x 3 neighbourhood in int32, with (y, x) clamped into [1, H - 2] x [1, W - 2] (cv2 copies the second and
+// second-last rows and columns over the border ones).  (ry, rx) is the R site of the 2 x 2 block at (0, 0), so pixel
+// (y, x) is on an R row when (y ^ ry) is even and in an R column when (x ^ rx) is; R and B sites read all nine codes, G
+// sites five.  Codes above 8 bits are mapped to 8 bits per channel with ys = 1 / (2^bits - 1), the full-range luma step
+// of YUVFrame.  `bad` marks an entry the kernels cannot read.  A value-initialised BayerFrame{} is empty.
+struct BayerFrame {
+  const uint8_t* data;
+  long long rs;
+  int H, W;
+  int ry, rx, packing, bits, shift;
+  bool bad;
+  double ys;
+  __device__ __forceinline__ bool empty() const { return bad || data == nullptr || H < 3 || W < 3; }
+  // the code of pixel (y, x): a byte, a masked uint16, or a MIPI RAW10 / RAW12 group's high byte and low bits
+  __device__ __forceinline__ int code(int y, int x) const {
+    const uint8_t* row = data + (long long)y * rs;
+    if (packing == FEAR_BAYER_RAW10) {
+      const uint8_t* g = row + 5LL * (x >> 2);
+      const int i = x & 3;
+      return (__ldg(g + i) << 2) | ((__ldg(g + 4) >> (2 * i)) & 3);
+    }
+    if (packing == FEAR_BAYER_RAW12) {
+      const uint8_t* g = row + 3LL * (x >> 1);
+      const int i = x & 1;
+      return (__ldg(g + i) << 4) | ((__ldg(g + 2) >> (4 * i)) & 15);
+    }
+    if (bits == 8) return __ldg(row + x);
+    return (__ldg(reinterpret_cast<const uint16_t*>(row) + x) >> shift) & ((1 << bits) - 1);
+  }
+  __device__ __forceinline__ int to_u8(int v) const {
+    return bits == 8 ? v : yuv_unit_to_u8(__dmul_rn((double)v, ys));
+  }
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    y = min(max(y, 1), H - 2);
+    x = min(max(x, 1), W - 2);
+    const int c = code(y, x), n = code(y - 1, x), s = code(y + 1, x), w = code(y, x - 1), e = code(y, x + 1);
+    const bool r_row = !((y ^ ry) & 1), r_col = !((x ^ rx) & 1);
+    int r, g, b;
+    if (r_row == r_col) {  // an R site (both) or a B site (neither)
+      const int cross = (n + s + w + e + 2) >> 2;
+      const int diag = (code(y - 1, x - 1) + code(y - 1, x + 1) + code(y + 1, x - 1) + code(y + 1, x + 1) + 2) >> 2;
+      r = r_row ? c : diag;
+      g = cross;
+      b = r_row ? diag : c;
+    } else {  // a G site: its row's other colour is horizontal, its column's vertical
+      const int hor = (w + e + 1) >> 1, ver = (n + s + 1) >> 1;
+      r = r_row ? hor : ver;
+      g = c;
+      b = r_row ? ver : hor;
+    }
+    p[0] = to_u8(r);
+    p[1] = to_u8(g);
+    p[2] = to_u8(b);
+  }
+};
+
+// Frame i of a FearFrameBayer table (the *_bayer entry points), checked per entry against FearFrameBayer's rules.
+struct BayerFrames {
+  const FearFrameBayer* views;
+  __device__ __forceinline__ BayerFrame operator()(int i) const {
+    const FearFrameBayer v = views[i];
+    const long long W = v.W;
+    const bool wide = v.packing == FEAR_BAYER_UNPACKED && v.bits != 8;
+    const long long row_bytes = v.packing == FEAR_BAYER_RAW10   ? 5 * ((W + 3) / 4)
+                                : v.packing == FEAR_BAYER_RAW12 ? 3 * ((W + 1) / 2)
+                                                                : (wide ? 2 : 1) * W;
+    bool ok;
+    if (v.packing == FEAR_BAYER_RAW10) ok = v.bits == 10;
+    else if (v.packing == FEAR_BAYER_RAW12) ok = v.bits == 12;
+    else if (v.packing == FEAR_BAYER_UNPACKED)
+      ok = v.bits == 8 ? v.shift == 0
+                       : (v.bits == 10 || v.bits == 12 || v.bits == 14 || v.bits == 16) && v.shift >= 0 &&
+                             v.shift <= 16 - v.bits && !(((uintptr_t)v.data | (uintptr_t)v.row_stride) & 1);
+    else ok = false;
+    ok = ok && v.pattern >= FEAR_BAYER_RGGB && v.pattern <= FEAR_BAYER_BGGR && v.row_stride >= row_bytes;
+    return BayerFrame{static_cast<const uint8_t*>(v.data), v.row_stride, v.H, v.W, v.pattern >> 1, v.pattern & 1,
+                      v.packing, v.bits, v.shift, !ok,
+                      ok && v.bits != 8 ? __ddiv_rn(1.0, (double)((1 << v.bits) - 1)) : 0.0};
   }
 };
 

@@ -290,3 +290,124 @@ def v210_pack(y: np.ndarray, u: np.ndarray, v: np.ndarray, pitch: Optional[int] 
     out = np.zeros((h, pitch), dtype=np.uint8)
     out[:, :16 * groups] = words.reshape(h, 4 * groups).view(np.uint8)
     return out
+
+
+# Bayer colour filter arrays: the colours of the 2 x 2 block at pixel (0, 0), row by row (OpenCV 4.x's sensor-order
+# COLOR_Bayer{RGGB,GRBG,GBRG,BGGR}2RGB) -> FearFrameBayer's pattern; pattern p has its R site at (p >> 1, p & 1)
+BAYER_PATTERNS = {"RGGB": 0, "GRBG": 1, "GBRG": 2, "BGGR": 3}
+# MIPI CSI-2 packings of FearFrameBayer: bits -> (pixels, bytes) per group
+MIPI_GROUPS = {10: (4, 5), 12: (2, 3)}
+
+
+def _bayer_pattern(pattern) -> int:
+    if pattern not in BAYER_PATTERNS:
+        raise ValueError(f"a Bayer pattern must be one of {sorted(BAYER_PATTERNS)}, got {pattern!r}")
+    return BAYER_PATTERNS[pattern]
+
+
+def bayer_demosaic(raw: np.ndarray, pattern: str = "RGGB") -> np.ndarray:
+    """The (H, W, 3) RGB frame of a (H, W) Bayer mosaic at its own depth (uint8 or uint16 codes), as
+    ``cv2.cvtColor(raw, cv2.COLOR_Bayer{pattern}2RGB)`` gives it for H, W >= 3.  A numpy restatement of the crop
+    kernel's demosaic (include/fear_b200.h, FearFrameBayer): with N, S, W, E the neighbours and NW .. SE the diagonals,
+    an R site takes G = (N + S + W + E + 2) >> 2 and B = (NW + NE + SW + SE + 2) >> 2, a B site alike with R and B
+    swapped, a G site on an R row R = (W + E + 1) >> 1 and B = (N + S + 1) >> 1, on a B row the reverse; pixel (y, x) of
+    the border takes the values of pixel (clamp(y, 1, H - 2), clamp(x, 1, W - 2))."""
+    a = np.asarray(raw)
+    if a.ndim != 2 or a.dtype not in (np.uint8, np.uint16) or a.shape[0] < 3 or a.shape[1] < 3:
+        raise ValueError(f"a Bayer mosaic must be a 2-D uint8 or uint16 (H, W) array with H, W >= 3, got "
+                         f"{a.dtype} {a.shape}")
+    p = _bayer_pattern(pattern)
+    ry, rx = p >> 1, p & 1
+    h, w = a.shape
+    s = a.astype(np.int64)
+    c = s[1:-1, 1:-1]
+    n, so, we, e = s[:-2, 1:-1], s[2:, 1:-1], s[1:-1, :-2], s[1:-1, 2:]
+    cross = (n + so + we + e + 2) >> 2
+    diag = (s[:-2, :-2] + s[:-2, 2:] + s[2:, :-2] + s[2:, 2:] + 2) >> 2
+    hor, ver = (we + e + 1) >> 1, (n + so + 1) >> 1
+    yy, xx = np.meshgrid(np.arange(1, h - 1), np.arange(1, w - 1), indexing="ij")
+    r_row, r_col = ((yy ^ ry) & 1) == 0, ((xx ^ rx) & 1) == 0
+    rb = r_row == r_col
+    r = np.where(rb, np.where(r_row, c, diag), np.where(r_row, hor, ver))
+    g = np.where(rb, cross, c)
+    b = np.where(rb, np.where(r_row, diag, c), np.where(r_row, ver, hor))
+    inner = np.stack([r, g, b], -1)
+    rows = np.clip(np.arange(h), 1, h - 2) - 1
+    cols = np.clip(np.arange(w), 1, w - 2) - 1
+    return inner[rows][:, cols].astype(a.dtype)
+
+
+def bayer_to_rgb(codes: np.ndarray, pattern: str = "RGGB", bits: int = 8) -> np.ndarray:
+    """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for a Bayer mosaic of ``bits``-bit codes (uint8 at 8 bits,
+    else uint16 codes in [0, 2^bits - 1], already unpacked and masked): ``bayer_demosaic`` at the codes' depth, then,
+    above 8 bits, each channel value v mapped as full-range luma is, min(max(rint(255 * (v * (1 / (2^bits - 1)))), 0),
+    255) in float64 (``yuv_to_rgb(v, c, c, full_range=True, bits=bits)`` at neutral chroma c = 2^(bits - 1))."""
+    if isinstance(bits, bool) or bits not in (8, 10, 12, 14, 16):
+        raise ValueError(f"Bayer bits must be 8, 10, 12, 14 or 16, got {bits!r}")
+    a = np.asarray(codes)
+    if a.dtype != (np.uint8 if bits == 8 else np.uint16):
+        raise ValueError(f"{bits}-bit Bayer codes must be {'uint8' if bits == 8 else 'uint16'}, got {a.dtype}")
+    if bits < 16 and a.size and int(a.max()) >= 1 << bits:
+        raise ValueError(f"{bits}-bit Bayer codes must be below {1 << bits}, got {int(a.max())}")
+    rgb = bayer_demosaic(a, pattern)
+    if bits == 8:
+        return rgb
+    ys = 1.0 / float((1 << bits) - 1)
+    return np.clip(np.rint(255.0 * (rgb.astype(np.float64) * ys)), 0, 255).astype(np.uint8)
+
+
+def mipi_row_bytes(width: int, bits: int) -> int:
+    """The bytes a MIPI CSI-2 RAW10 (4 pixels in 5 bytes) or RAW12 (2 pixels in 3 bytes) row of ``width`` pixels
+    needs, the last group possibly partial."""
+    if bits not in MIPI_GROUPS:
+        raise ValueError(f"MIPI packing is RAW10 or RAW12, got bits {bits!r}")
+    px, nb = MIPI_GROUPS[bits]
+    return nb * -(-int(width) // px)
+
+
+def mipi_unpack(buf: np.ndarray, width: int, bits: int) -> np.ndarray:
+    """The (H, width) uint16 codes of MIPI CSI-2 RAW10 / RAW12 rows ``buf`` ((H, pitch) uint8, pitch >= the row bytes;
+    bytes past the last group are not read).  RAW10: bytes 0-3 of a group are bits 9..2 of pixels 0..3, byte 4 is
+    P3[1:0] << 6 | P2[1:0] << 4 | P1[1:0] << 2 | P0[1:0]; RAW12: bytes 0-1 are bits 11..4 of pixels 0, 1, byte 2 is
+    P1[3:0] << 4 | P0[3:0].  A numpy restatement of the crop kernel's reads (include/fear_b200.h, FearFrameBayer)."""
+    a = np.asarray(buf)
+    if a.dtype != np.uint8 or a.ndim != 2 or a.shape[0] < 1:
+        raise ValueError(f"MIPI rows must be a 2-D uint8 (H, pitch) array, got {a.dtype} {a.shape}")
+    if isinstance(width, bool) or not isinstance(width, (int, np.integer)) or width < 1:
+        raise ValueError(f"a MIPI row width must be an int >= 1, got {width!r}")
+    need = mipi_row_bytes(width, bits)
+    if a.shape[1] < need:
+        raise ValueError(f"a RAW{bits} row of {width} pixels needs {need} bytes, got {a.shape[1]}")
+    px, nb = MIPI_GROUPS[bits]
+    g = a[:, :need].reshape(a.shape[0], -1, nb).astype(np.uint16)
+    lo_bits = bits - 8
+    lo = np.stack([(g[..., px] >> (lo_bits * i)) & ((1 << lo_bits) - 1) for i in range(px)], -1)
+    codes = (g[..., :px] << lo_bits) | lo
+    return codes.reshape(a.shape[0], -1)[:, :int(width)]
+
+
+def mipi_pack(codes: np.ndarray, bits: int, pitch: Optional[int] = None) -> np.ndarray:
+    """The (H, pitch) uint8 MIPI CSI-2 RAW10 / RAW12 rows of (H, W) codes in [0, 2^bits): the inverse of
+    ``mipi_unpack``.  ``pitch`` defaults to the row bytes; the pixels that fill out the last group and the bytes past
+    it are 0."""
+    c = np.asarray(codes)
+    if c.ndim != 2 or c.shape[0] < 1 or c.shape[1] < 1:
+        raise ValueError(f"codes must be a 2-D (H, W) array, got shape {c.shape}")
+    need = mipi_row_bytes(c.shape[1], bits)
+    if c.size and (c.min() < 0 or c.max() >= 1 << bits):
+        raise ValueError(f"RAW{bits} codes must be in [0, {(1 << bits) - 1}]")
+    pitch = need if pitch is None else int(pitch)
+    if pitch < need:
+        raise ValueError(f"a RAW{bits} row of {c.shape[1]} pixels needs {need} bytes, got pitch {pitch}")
+    px, nb = MIPI_GROUPS[bits]
+    h, groups, lo_bits = c.shape[0], need // nb, bits - 8
+    full = np.zeros((h, groups * px), dtype=np.uint32)
+    full[:, :c.shape[1]] = c
+    full = full.reshape(h, groups, px)
+    g = np.zeros((h, groups, nb), dtype=np.uint32)
+    g[..., :px] = full >> lo_bits
+    for i in range(px):
+        g[..., px] |= (full[..., i] & ((1 << lo_bits) - 1)) << (lo_bits * i)
+    out = np.zeros((h, pitch), dtype=np.uint8)
+    out[:, :need] = g.reshape(h, need)
+    return out

@@ -11,7 +11,9 @@ device as a video decoder, webcam or capture card writes them: YUV420Frame (NV12
 YUV422Frame (YUYV / UYVY / YVYU, Y210, NV16 / P210, yuv422p) and YUV444Frame (yuv444p, NVDEC's 4:4:4 surfaces), in
 BT.601, BT.709 or BT.2020, limited or full range, 8, 10 or 12 bits, converted to RGB inside the crop (8-bit BT.601
 limited range exactly as cv2.cvtColor converts it), and V210Frame (SDI capture cards' packed 10-bit 4:2:2, unpacked
-inside the crop).  Tensors, YUV planes and v210 surfaces are read where they are, without a copy.
+inside the crop); or raw Bayer mosaics as machine-vision and CSI-2 cameras send them: BayerFrame (RGGB / GRBG / GBRG /
+BGGR at 8 to 16 bits, MIPI RAW10 / RAW12), demosaiced inside the crop exactly as cv2.cvtColor(COLOR_Bayer*2RGB)
+demosaics them.  Tensors, YUV planes, v210 surfaces and Bayer mosaics are read where they are, without a copy.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -28,8 +30,9 @@ tensors' views point at the tensors.  YUV420Frames go into a second fixed table 
 format), read by the *_yuv entry points; a call with any 4:2:2 or 4:4:4 frame puts all its frames into a third, of
 FearFrameYCbCr records (the same plus the chroma subsampling), read by the *_ycbcr entry points; a call with any
 V210Frame puts all its frames into a fourth, of FearFrameYCbCrV210 records (a FearFrameYCbCr or a v210 surface), read
-by the *_ycbcr_v210 entry points.  The host then reads
-back the boxes and scores.  The launch count of a step depends neither on N nor on the kind of frames.
+by the *_ycbcr_v210 entry points.  BayerFrames go into a fifth, of FearFrameBayer records, read by the *_bayer entry
+points; they cannot share a call with other kinds of frames.  The host then reads back the boxes and scores.  The
+launch count of a step depends neither on N nor on the kind of frames.
 """
 import math
 import warnings
@@ -49,9 +52,10 @@ ENTRY_POINTS = {
     "ycbcr": ("fear_frame_sums_ycbcr_u8", "fear_crop_targets_ycbcr_u8", "fear_advance_targets_ycbcr"),
     "ycbcr_v210": ("fear_frame_sums_ycbcr_v210_u8", "fear_crop_targets_ycbcr_v210_u8",
                    "fear_advance_targets_ycbcr_v210"),
+    "bayer": ("fear_frame_sums_bayer_u8", "fear_crop_targets_bayer_u8", "fear_advance_targets_bayer"),
 }
 TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE,
-                "ycbcr_v210": _lib.YCBCR_V210_DTYPE}
+                "ycbcr_v210": _lib.YCBCR_V210_DTYPE, "bayer": _lib.BAYER_DTYPE}
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -336,11 +340,98 @@ class V210Frame:
                 int(self.full_range), self.bits, 0, *self.CHROMA_SHIFT, 1, 0)
 
 
+class BayerFrame:
+    """A raw Bayer mosaic as machine-vision cameras (GigE Vision / USB3 Vision PFNC ``BayerRG8``, ``BayerGR12`` ...),
+    CSI-2 sensors under V4L2 or libcamera (``SRGGB10P`` / ``SRGGB12P``) and raw recorders deliver it.  ``pattern`` is
+    the colours of the 2 x 2 block at pixel (0, 0), row by row: "RGGB", "GRBG", "GBRG" or "BGGR" (OpenCV 4.x's
+    ``COLOR_Bayer{pattern}2RGB``; a region of interest at an odd offset names its own pattern).
+
+        BayerFrame(t, pattern, bits=8, msb=False)   t a CUDA (H, W) tensor: uint8 at 8 bits, torch.uint16 at 10, 12,
+                                                    14 or 16 bits, the code in the low bits (``msb=False``) or the
+                                                    high bits (``msb=True``) of each sample; any row stride, column
+                                                    stride 1 (a view ``surface[:, :W]`` of a pitched surface is fine)
+        BayerFrame.raw10(t, width, pattern)         t a CUDA uint8 (H, row bytes) tensor of MIPI CSI-2 RAW10 rows
+        BayerFrame.raw12(t, width, pattern)         t a CUDA uint8 (H, row bytes) tensor of MIPI CSI-2 RAW12 rows
+
+    H and W must be at least 3.  FEARMultiTracker and FEARTracker read the samples where they are and demosaic every
+    pixel they read, so no RGB copy is made: the RGB frame the tracker sees is ``image_ops.bayer_to_rgb(codes,
+    pattern, bits)`` of the frame's codes (``image_ops.mipi_unpack`` for packed rows), which is ``cv2.cvtColor(raw,
+    cv2.COLOR_Bayer{pattern}2RGB)`` at 8 bits.  The constructors raise ValueError on a malformed tensor or format.
+    ``shape`` is (H, W, 3)."""
+
+    def __init__(self, t: torch.Tensor, pattern: str = "RGGB", bits: int = 8, msb: bool = False) -> None:
+        self._check_pattern(pattern)
+        if isinstance(bits, bool) or bits not in (8, 10, 12, 14, 16):
+            raise ValueError(f"BayerFrame bits must be 8, 10, 12, 14 or 16, got {bits!r}")
+        if bits == 8 and msb:
+            raise ValueError("BayerFrame msb applies to samples wider than 8 bits, not 8-bit ones")
+        dtype = torch.uint8 if bits == 8 else torch.uint16
+        self._check_tensor(t, dtype, f"(H, W) tensor at {bits} bits")
+        self._init(t, pattern, int(bits), 16 - int(bits) if msb else 0, 0, t.shape[1], t.shape[1] * t.element_size())
+
+    @classmethod
+    def raw10(cls, t: torch.Tensor, width: int, pattern: str = "RGGB") -> "BayerFrame":
+        return cls._packed(t, width, pattern, 10, 1)
+
+    @classmethod
+    def raw12(cls, t: torch.Tensor, width: int, pattern: str = "RGGB") -> "BayerFrame":
+        return cls._packed(t, width, pattern, 12, 2)
+
+    @classmethod
+    def _packed(cls, t, width, pattern, bits: int, packing: int) -> "BayerFrame":
+        cls._check_pattern(pattern)
+        cls._check_tensor(t, torch.uint8, f"(H, row bytes) tensor of RAW{bits} rows")
+        if isinstance(width, bool) or not isinstance(width, (int, np.integer)) or not (3 <= width <= _MAX_SIDE):
+            raise ValueError(f"BayerFrame width must be an int in [3, {_MAX_SIDE}], got {width!r}")
+        need = image_ops.mipi_row_bytes(width, bits)
+        if t.shape[1] < need:
+            raise ValueError(f"a RAW{bits} row of {width} pixels needs {need} bytes, the tensor's rows have "
+                             f"{t.shape[1]}")
+        f = cls.__new__(cls)
+        f._init(t, pattern, bits, 0, packing, int(width), need)
+        return f
+
+    @staticmethod
+    def _check_pattern(pattern) -> None:
+        if pattern not in image_ops.BAYER_PATTERNS:
+            raise ValueError(f"BayerFrame pattern must be one of {sorted(image_ops.BAYER_PATTERNS)}, got {pattern!r}")
+
+    @staticmethod
+    def _check_tensor(t, dtype: torch.dtype, what: str) -> None:
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.ndim != 2 or t.device.type != "cuda":
+            got = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"BayerFrame takes a 2-D CUDA {dtype} {what}, got {got}")
+        if not (3 <= t.shape[0] <= _MAX_SIDE and 3 <= t.shape[1] <= _MAX_SIDE):
+            raise ValueError(f"a Bayer mosaic needs at least 3 rows and 3 columns, got {tuple(t.shape)}")
+
+    def _init(self, t: torch.Tensor, pattern: str, bits: int, shift: int, packing: int, width: int,
+              row_bytes: int) -> None:
+        es = t.element_size()
+        pitch = t.stride(0) * es
+        if t.stride(1) != 1 or pitch < row_bytes:
+            raise ValueError(f"BayerFrame rows must be contiguous samples at a pitch of at least {row_bytes} bytes, "
+                             f"got strides {t.stride()}")
+        if es == 2 and (pitch % 2 or t.data_ptr() % 2):
+            raise ValueError(f"BayerFrame uint16 rows must start on 2-byte boundaries: pitch {pitch}, address offset "
+                             f"{t.data_ptr() % 2}")
+        self.t, self.pattern, self.bits, self.shift, self.packing = t, pattern, bits, shift, packing
+        self.pitch = int(pitch)
+        self.shape = (t.shape[0], width, 3)
+
+    def bayer_record(self) -> tuple:
+        """The FearFrameBayer record (data, row_stride, H, W, pattern, bits, shift, packing): the address of sample
+        (0, 0) (packed: of row 0's first byte), the row pitch in bytes, the size and the format."""
+        return (self.t.data_ptr(), self.pitch, *self.shape[:2], image_ops.BAYER_PATTERNS[self.pattern], self.bits,
+                self.shift, self.packing)
+
+
 def frame_kind(frame) -> str:
-    """"yuv" for a YUV420Frame, YUV422Frame, YUV444Frame or V210Frame, "cuda" for a torch tensor (checked by
-    ``check_device_frame``), "numpy" for anything else."""
+    """"yuv" for a YUV420Frame, YUV422Frame, YUV444Frame or V210Frame, "bayer" for a BayerFrame, "cuda" for a torch
+    tensor (checked by ``check_device_frame``), "numpy" for anything else."""
     if isinstance(frame, (_YUVFrame, V210Frame)):
         return "yuv"
+    if isinstance(frame, BayerFrame):
+        return "bayer"
     return "cuda" if isinstance(frame, torch.Tensor) else "numpy"
 
 
@@ -367,8 +458,10 @@ def check_tensor_frame(i: int, f: torch.Tensor, device) -> None:
 
 
 def check_device_frame(i: int, f, kind: str, device) -> None:
-    """The checks of a frame of kind "cuda" or "yuv" (``frame_kind``): ValueError before any device call."""
-    if kind == "yuv":
+    """The checks of a frame of kind "cuda", "yuv" or "bayer" (``frame_kind``): ValueError before any device call."""
+    if kind == "bayer":
+        check_device(i, device, f.t)
+    elif kind == "yuv":
         check_device(i, device, *((f.t,) if isinstance(f, V210Frame) else (f.y, f.u, f.v)))
     else:
         check_tensor_frame(i, f, device)
@@ -377,7 +470,7 @@ def check_device_frame(i: int, f, kind: str, device) -> None:
 def write_records(table: np.ndarray, frames, name: str) -> None:
     """Write the records of device frames into rows of ``table`` (a numpy view of ``TABLE_DTYPES[name]``):
     FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr",
-    FearFrameYCbCrV210 for "ycbcr_v210"."""
+    FearFrameYCbCrV210 for "ycbcr_v210", FearFrameBayer for "bayer"."""
     for i, f in enumerate(frames):
         if name == "yuv":
             table[i] = f.yuv_record()
@@ -385,6 +478,8 @@ def write_records(table: np.ndarray, frames, name: str) -> None:
             table[i] = f.ycbcr_record()
         elif name == "ycbcr_v210":
             table[i] = f.ycbcr_v210_record()
+        elif name == "bayer":
+            table[i] = f.bayer_record()
         else:
             table[i] = frame_view(f)
 
@@ -440,9 +535,9 @@ class FEARMultiTracker:
         """Start tracking ``rects`` ((n, 4) [x, y, w, h]); target i lives in stream ``streams[i]`` (default 0), whose
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
-        ``frames`` are all numpy arrays, all CUDA tensors or all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame,
-        V210Frame; see ``update``).  A target's padding colour is the mean colour of its frame (of the converted RGB frame for a
-        YUV frame), from exact
+        ``frames`` are all numpy arrays, all CUDA tensors, all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame,
+        V210Frame) or all BayerFrames (see ``update``).  A target's padding colour is the mean colour of its frame (of
+        the converted RGB frame for a YUV frame, of the demosaiced 8-bit frame for a Bayer frame), from exact
         per-channel sums computed on the device."""
         frames, kind = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
@@ -525,8 +620,10 @@ class FEARMultiTracker:
         ``CHROMA_SHIFT``) as numpy arrays (for the default format that is ``cv2.cvtColor(frame,
         cv2.COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420 / COLOR_YUV2RGB_YUY2 / COLOR_YUV2RGB_UYVY)``).  A ``V210Frame``'s
         words are read in place as well and give what its ``image_ops.v210_unpack`` planes give at 10 bits, 4:2:2.
-        Frames of one call may have different colour formats and subsamplings.  Device frames must be
-        ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
+        Frames of one call may have different colour formats and subsamplings.  ``frames`` may also be all
+        ``BayerFrame``s (any patterns, depths and packings), never mixed with other kinds; their samples are read in
+        place and give exactly what ``image_ops.bayer_to_rgb`` of their codes gives as numpy arrays.  Device frames must
+        be ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
         frames, kind = self._check_frames(frames)
@@ -560,8 +657,9 @@ class FEARMultiTracker:
         return torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
 
     def _check_frames(self, frames):
-        """-> (list of frames, their kind: "numpy", "cuda" or "yuv").  Raises ValueError before any device call."""
-        if isinstance(frames, (_YUVFrame, V210Frame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
+        """-> (list of frames, their kind: "numpy", "cuda", "yuv" or "bayer").  Raises ValueError before any device
+        call."""
+        if isinstance(frames, (_YUVFrame, V210Frame, BayerFrame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
                                                           and frames.ndim == 3):
             frames = [frames]
         frames = list(frames)
@@ -569,6 +667,9 @@ class FEARMultiTracker:
             raise ValueError("no frames given")
         kind = frame_kind(frames[0])
         if any(frame_kind(f) != kind for f in frames):
+            if any(frame_kind(f) == "bayer" for f in frames):
+                raise ValueError("BayerFrames cannot share a call with other kinds of frames (numpy arrays, CUDA "
+                                 "tensors, YUV frames): pass all of a call's frames as BayerFrames")
             raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV frames "
                              "(YUV420Frame, YUV422Frame, YUV444Frame, V210Frame), not a mix")
         for i, f in enumerate(frames):
@@ -607,22 +708,25 @@ class FEARMultiTracker:
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
             frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, ycbcr_pin=None,
-            ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, sums_pin=None, sums=None)
+            ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, bayer_pin=None, bayer=None, sums_pin=None, sums=None)
         return b
 
     def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
         """Write the frame table of ``frames`` into the fixed device table the kernels read, and return its name:
         "yuv" (FearFrameYUV records) when every frame is a YUV420Frame, "ycbcr_v210" (FearFrameYCbCrV210 records) for
         YUV frames of which any is a V210Frame, "ycbcr" (FearFrameYCbCr records) for other YUV frames of which any is
-        4:2:2 or 4:4:4, "views" (FearFrameView records) otherwise.  Numpy frames are
-        packed into the pinned staging buffer first and sent with one host-to-device copy (the packed layout is
-        recomputed only when their shapes change); CUDA tensors, YUV planes and v210 surfaces are used where they are."""
+        4:2:2 or 4:4:4, "bayer" (FearFrameBayer records) for BayerFrames, "views" (FearFrameView records) otherwise.
+        Numpy frames are packed into the pinned staging buffer first and sent with one host-to-device copy (the packed
+        layout is recomputed only when their shapes change); CUDA tensors, YUV planes, v210 surfaces and Bayer mosaics
+        are used where they are."""
         b, num_frames = self._buf, len(frames)
         name = "views"
         if kind == "yuv":
             name = "yuv" if all(isinstance(f, YUV420Frame) for f in frames) else "ycbcr"
             if any(isinstance(f, V210Frame) for f in frames):
                 name = "ycbcr_v210"
+        elif kind == "bayer":
+            name = "bayer"
         dtype = TABLE_DTYPES[name]
         nbytes = num_frames * dtype.itemsize
         if b[name] is None or b[name].numel() < nbytes:  # grows only: the step graph keys on it
@@ -673,7 +777,7 @@ class FEARMultiTracker:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
         keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records, YCbCr
-        records of any subsampling or YCbCr / v210 records) and
+        records of any subsampling, YCbCr / v210 records or Bayer records) and
         its buffer, and the net's generation.  ``cuda_graph=False`` in the tracking config keeps eager launches."""
         key = (n, num_frames, table, self._buf[table].data_ptr())
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):

@@ -8,9 +8,10 @@ of the reference's observable behaviour); network + decode run in libfear_b200 a
 48-byte box record comes back per frame.  With ``gpu_crop: true`` the numpy frame is uploaded and cropped on the device.
 
 Frames already in GPU memory -- uint8 (H, W, 3) CUDA tensors with any non-negative strides, YUV420Frame /
-YUV422Frame / YUV444Frame decoder surfaces and V210Frame capture buffers -- are read in place: the crop, the conversion
-to RGB, the network and the decode (plain or smoothed) run on the device, and the tracker returns exactly what it
-returns for the same pixels as a numpy array (``image_ops.yuv_to_rgb`` of a YUV frame's planes).
+YUV422Frame / YUV444Frame decoder surfaces, V210Frame capture buffers and BayerFrame raw mosaics -- are read in place:
+the crop, the conversion to RGB (or the demosaic), the network and the decode (plain or smoothed) run on the device, and
+the tracker returns exactly what it returns for the same pixels as a numpy array (``image_ops.yuv_to_rgb`` of a YUV
+frame's planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes).
 """
 from collections import deque
 from typing import Any, Dict, Optional, Tuple, Union
@@ -24,8 +25,8 @@ from .box_coder import FEARBoxCoder, TrackerDecodeResult
 from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY
 
 
-# byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrV210), a
-# FearTarget, then five float64 inputs of fear_decode_smooth
+# byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrV210; a
+# FearFrameBayer is 40 bytes), a FearTarget, then five float64 inputs of fear_decode_smooth
 _TARGET_OFFSET = 96
 _SMOOTH_OFFSET = _TARGET_OFFSET + 64
 _DEVICE_INPUT_BYTES = _SMOOTH_OFFSET + 5 * 8
@@ -109,18 +110,20 @@ class FEARTracker(Tracker):
     """The reference's single-object tracker.  ``initialize``, ``update`` and ``get_template_features`` take a frame as
     a uint8 (H, W, 3) RGB numpy array, as a uint8 (H, W, 3) CUDA tensor on the tracker's device (any non-negative
     strides: ``rgba[..., :3]``, ``chw.permute(1, 2, 0)``, a region of interest), or as a YUV420Frame, YUV422Frame,
-    YUV444Frame or V210Frame whose planes or words are on the tracker's device; the kind may change from one call to
-    the next.
+    YUV444Frame, V210Frame or BayerFrame whose planes, words or samples are on the tracker's device; the kind may
+    change from one call to the next.
 
     Numpy frames take the host crop, or with ``gpu_crop: true`` an upload and the device crop.  Device frames always
     take the device step, whatever ``gpu_crop`` says, since the host crop could only read them after copying them back:
     fear_crop_targets_view_u8 (tensors), fear_crop_targets_ycbcr_u8 (YUV frames, converted to RGB inside the crop) or
-    fear_crop_targets_ycbcr_v210_u8 (v210 frames, unpacked and converted inside the crop) makes the search crop, then
-    the network and the decode, plain or with ``smooth: true`` the smoothed one, run as one CUDA graph and one 48-byte
-    record comes back.  The results, ``tracking_state`` included, are those of the same tracker fed the same pixels as
-    numpy arrays (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its ``CHROMA_SHIFT``, of a v210 frame's
-    ``image_ops.v210_unpack`` planes).  Device frames must be ready on the current CUDA stream; every call synchronises it before it
-    returns, so they only need to live for the call.  ``host_normalize: true`` takes numpy frames only."""
+    fear_crop_targets_ycbcr_v210_u8 (v210 frames, unpacked and converted inside the crop) or fear_crop_targets_bayer_u8
+    (Bayer frames, demosaiced inside the crop) makes the search crop, then the network and the decode, plain or with
+    ``smooth: true`` the smoothed one, run as one CUDA graph and one 48-byte record comes back.  The results,
+    ``tracking_state`` included, are those of the same tracker fed the same pixels as numpy arrays
+    (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its ``CHROMA_SHIFT``, of a v210 frame's
+    ``image_ops.v210_unpack`` planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes).  Device frames must be ready
+    on the current CUDA stream; every call synchronises it before it returns, so they only need to live for the call.
+    ``host_normalize: true`` takes numpy frames only."""
 
     def get_box_coder(self, tracking_config, cuda_id: int = 0):
         return FEARBoxCoder(tracker_config=tracking_config)
@@ -268,8 +271,8 @@ class FEARTracker(Tracker):
 
     # -- device frames: CUDA tensors and YUV frames, read in place by the crop-targets entry points (one target) --
     def _frame_kind(self, image) -> str:
-        """"numpy", "cuda" or "yuv" (multi_tracker.frame_kind).  A device frame is checked here, before any device call
-        or state change: NotImplementedError with ``host_normalize``, ValueError when malformed."""
+        """"numpy", "cuda", "yuv" or "bayer" (multi_tracker.frame_kind).  A device frame is checked here, before any
+        device call or state change: NotImplementedError with ``host_normalize``, ValueError when malformed."""
         kind = multi_tracker.frame_kind(image)
         if kind == "numpy":
             return kind
@@ -282,9 +285,9 @@ class FEARTracker(Tracker):
     def _device_frame_state(self) -> dict:
         """Buffers of the device-frame step, separate from the gpu_crop path's.  ``inputs`` (pinned) and ``dev_in``
         share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView, a
-        FearFrameYCbCr or a FearFrameYCbCrV210) at byte 0, the FearTarget at byte 96, fear_decode_smooth's prev_size
-        (w, h), penalty_k, window_influence and lr as float64 at byte 160; then, on the device only, the 16 x 16
-        window."""
+        FearFrameYCbCr, a FearFrameYCbCrV210 or a FearFrameBayer) at byte 0, the FearTarget at byte 96,
+        fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr as float64 at byte 160; then, on the
+        device only, the 16 x 16 window."""
         from . import _lib
 
         dev = self._device()
@@ -312,8 +315,9 @@ class FEARTracker(Tracker):
     def _stage_device_inputs(self, st: dict, image, kind: str, bbox, pad, prev_size=None) -> str:
         """Write the frame's record, the target (frame 0, ``bbox``, padding colour ``pad``) and, given ``prev_size``,
         the smooth scalars into the pinned inputs and send them with one host-to-device copy.  Returns the table name:
-        "views" for a tensor, "ycbcr_v210" for a V210Frame, "ycbcr" for every other YUV frame."""
-        table = "views"
+        "views" for a tensor, "ycbcr_v210" for a V210Frame, "ycbcr" for every other YUV frame, "bayer" for a
+        BayerFrame."""
+        table = "bayer" if kind == "bayer" else "views"
         if kind == "yuv":
             table = "ycbcr_v210" if isinstance(image, multi_tracker.V210Frame) else "ycbcr"
         raw, dtype = st["inputs"].numpy(), multi_tracker.TABLE_DTYPES[table]

@@ -39,6 +39,9 @@
  *   fear_crop_targets_ycbcr_v210_u8 / fear_advance_targets_ycbcr_v210 / fear_frame_sums_ycbcr_v210_u8   the same three
  *                         on FearFrameYCbCrV210 tables: FearFrameYCbCr entries and v210 surfaces (10-bit 4:2:2 packed
  *                         three codes to a 32-bit word, as SDI capture cards deliver it), unpacked inside the crop
+ *   fear_crop_targets_bayer_u8 / fear_advance_targets_bayer / fear_frame_sums_bayer_u8   the same three on raw Bayer
+ *                         mosaics located by FearFrameBayer (8 to 16 bits, MIPI RAW10 / RAW12), demosaiced inside the
+ *                         crop as cv2.cvtColor(COLOR_Bayer*2RGB) demosaics them
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -197,6 +200,40 @@ typedef struct FearFrameYCbCrV210 {        /* 96 bytes                          
   int32_t v210;                            /* 0: a FearFrameYCbCr entry; 1: a v210 surface                      */
   int32_t reserved;                        /* not read                                                          */
 } FearFrameYCbCrV210;
+/* A raw Bayer mosaic (machine-vision cameras' PFNC BayerRG8 / BayerGR12 ..., CSI-2 sensors' SRGGB10P / SRGGB12P):
+ * 40 bytes.  `pattern` names the colours of the 2 x 2 block at pixel (0, 0), row by row (OpenCV 4.x's sensor-order
+ * COLOR_Bayer{RGGB,GRBG,GBRG,BGGR}2RGB).  `packing` is how a row holds its samples:
+ *   FEAR_BAYER_UNPACKED  one sample per pixel: a byte at 8 bits (shift 0), a uint16 at 10, 12, 14 or 16 bits whose code
+ *                        is (s >> shift) & (2^bits - 1), 0 <= shift <= 16 - bits (LSB-aligned: 0, MSB: 16 - bits); a
+ *                        uint16 row needs an even address and an even row_stride
+ *   FEAR_BAYER_RAW10     MIPI CSI-2 RAW10 (bits 10): 4 pixels in 5 bytes, bytes 0-3 bits 9..2 of P0..P3, byte 4
+ *                        P3[1:0] << 6 | P2[1:0] << 4 | P1[1:0] << 2 | P0[1:0]; a row needs 5 * ceil(W / 4) bytes
+ *   FEAR_BAYER_RAW12     MIPI CSI-2 RAW12 (bits 12): 2 pixels in 3 bytes, bytes 0-1 bits 11..4 of P0, P1, byte 2
+ *                        P1[3:0] << 4 | P0[3:0]; a row needs 3 * ceil(W / 2) bytes
+ * `data` is sample (0, 0) (packed: the first byte of row 0) and row_stride the row pitch in bytes (shift is not read for
+ * packed rows).  Every pixel is demosaiced as cv2.cvtColor(raw, COLOR_Bayer{pattern}2RGB) does (bilinear, integer): with
+ * (y, x) clamped into [1, H - 2] x [1, W - 2], the pixel's own colour is its code, and with N, S, W, E the codes next to
+ * it and NW, NE, SW, SE the diagonal ones, cross = (N + S + W + E + 2) >> 2, diag = (NW + NE + SW + SE + 2) >> 2,
+ * hor = (W + E + 1) >> 1, ver = (N + S + 1) >> 1: an R site takes G = cross, B = diag; a B site G = cross, R = diag; a G
+ * site on an R row R = hor, B = ver; a G site on a B row B = hor, R = ver.  Above 8 bits each channel value v is mapped
+ * to 8 bits as FearFrameYUV's full-range luma is: min(max(rint(255 * (v * (1 / (2^bits - 1)))), 0), 255) in float64.
+ * An entry is treated like a frame index outside [0, F) when data is null, H or W is below 3 (cv2 accepts smaller
+ * frames; the kernels do not), pattern is not 0..3, packing is not 0..2, an unpacked entry has bits not in {8, 10, 12, 14,
+ * 16}, a shift other than 0 at 8 bits, a negative shift or shift + bits > 16, or (uint16) an odd address or row_stride,
+ * a RAW10 entry has bits other than 10 or a RAW12 entry bits other than 12, or row_stride is below the bytes of a row. */
+#define FEAR_BAYER_RGGB 0
+#define FEAR_BAYER_GRBG 1
+#define FEAR_BAYER_GBRG 2
+#define FEAR_BAYER_BGGR 3
+#define FEAR_BAYER_UNPACKED 0
+#define FEAR_BAYER_RAW10 1
+#define FEAR_BAYER_RAW12 2
+typedef struct FearFrameBayer {               /* 40 bytes                                                       */
+  const void* data;                           /* device address of sample (0, 0) / of row 0's first byte        */
+  int64_t row_stride;                         /* bytes                                                          */
+  int32_t H, W;                               /* size in pixels, both >= 3                                      */
+  int32_t pattern, bits, shift, packing;      /* FEAR_BAYER_*, code depth, uint16 alignment, FEAR_BAYER_* packing */
+} FearFrameBayer;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -358,6 +395,16 @@ int fear_crop_targets_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, Fe
 int fear_advance_targets_ycbcr_v210(const FearBox* d_boxes, const FearFrameYCbCrV210* d_views, int F,
                                     FearTarget* d_targets, int N, int instance_size, void* stream);
 int fear_frame_sums_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* The same three on FearFrameBayer tables: raw Bayer mosaics read where they are, each tap demosaiced (and above 8 bits
+ * mapped to 8 bits) inside the crop, so the kernels see cv2.cvtColor(raw, COLOR_Bayer{pattern}2RGB).  Same semantics
+ * and FEAR_EINVAL rules as the *_ycbcr entry points; an entry the kernels cannot read (see FearFrameBayer) gets a
+ * padding-colour crop, keeps its box and sums to 0. */
+int fear_crop_targets_bayer_u8(const FearFrameBayer* d_views, int F, FearTarget* d_targets, int N, double offset,
+                               int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_bayer(const FearBox* d_boxes, const FearFrameBayer* d_views, int F, FearTarget* d_targets,
+                               int N, int instance_size, void* stream);
+int fear_frame_sums_bayer_u8(const FearFrameBayer* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
