@@ -189,6 +189,7 @@ struct PwParams {
   // --- fused depthwise producer (DWK = 3 | 5): the A operand is dw(X) computed on the fly ---
   int dw_relu, dw_bias;  // ReLU / bias of the depthwise stage
   int box_bytes;         // bytes of one (tile rows + DWK - 1) x (map width + DWK - 1) x 32-channel input box
+  int tma_store;         // pw_tc_kernel stores C by TMA (tmC); 0 when C or ldc is not 16-byte aligned
 };
 
 // Warp-specialised CTA: warpgroup 0 is the TMA producer and keeps kPwProducerRegs registers per thread, warpgroups 1-2
@@ -278,6 +279,79 @@ __device__ __forceinline__ void pw_epilogue(const PwParams& p, const float* accm
   }
 }
 
+// Epilogue of one consumer warpgroup's 64 rows through shared memory, for pw_tc_kernel.  First the same arithmetic as
+// pw_epilogue, in place in accm, so every bias and residual load is issued before the first barrier.  Then slabs of 32
+// columns (two [64 rows][16 columns] boxes, SWIZZLE_64B, so the 8-byte writes of a warp take the minimum two wavefronts),
+// each stored by TMA from one elected thread.  Slabs alternate between two buffers and the tile's last slab goes to
+// `last`; a buffer is rewritten only once the store issued from it two slabs ago has read it (wait_group.read 1).
+// Nothing waits for the global writes: the warpgroup goes on to the next tile's MMAs.  TMA clips the M and N tails at
+// the tensor's bounds.
+constexpr int kPwSlabBytes = 64 * 128;  // one warpgroup's 64 rows x 32 columns
+constexpr int kPwBoxBytes = 64 * 64;    // one TMA store box: 64 rows x 16 columns
+template <int NT>
+__host__ __device__ constexpr int pw_slabs() { return (NT + 31) / 32; }  // staging slabs per tile
+
+// Named barrier of one consumer warpgroup (ids 2 and 3; consumer_sync is id 1).
+__device__ __forceinline__ void wg_sync(int wgc) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wgc) : "memory"); }
+
+template <int NT>
+__device__ __forceinline__ void pw_epilogue_tma(const PwParams& p, const CUtensorMap* tmC, float* accm, const float* accc,
+                                                int mt, int nt, int wgc, int wr, int t, uint8_t* last, uint8_t* other,
+                                                bool leader) {
+  const long long row0 = (long long)mt * 128 + wgc * 64;  // first output row of this warpgroup
+#pragma unroll
+  for (int i = 0; i < NT / 8; ++i) {
+    const int col = nt * NT + 8 * i + 2 * t;
+#pragma unroll
+    for (int hrow = 0; hrow < 2; ++hrow) {
+      const long long grow = row0 + wr + hrow * 8;
+      float2 o = make_float2(accm[4 * i + 2 * hrow] + accc[4 * i + 2 * hrow], accm[4 * i + 2 * hrow + 1] + accc[4 * i + 2 * hrow + 1]);
+      if (grow < p.M && col < p.N) {  // TMA drops what lies outside C; bias and R are not read there
+        float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+        if (p.R) {
+          const float2 rr = __ldg(reinterpret_cast<const float2*>(p.R + grow * p.ldr + col));
+          b.x += rr.x;
+          b.y += rr.y;
+        }
+        o.x += b.x;
+        o.y += b.y;
+      }
+      if (p.relu) {
+        o.x = fmaxf(o.x, 0.f);
+        o.y = fmaxf(o.y, 0.f);
+      }
+      accm[4 * i + 2 * hrow] = o.x;
+      accm[4 * i + 2 * hrow + 1] = o.y;
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < pw_slabs<NT>(); ++s) {
+    uint8_t* buf = (pw_slabs<NT>() - 1 - s) & 1 ? other : last;
+    if (leader) tma_store_wait_read<1>();
+    wg_sync(wgc);
+#pragma unroll
+    for (int i = 4 * s; i < 4 * s + 4 && i < NT / 8; ++i) {
+      const int cc = 8 * (i & 1) + 2 * t;  // column inside the 16-column box
+#pragma unroll
+      for (int hrow = 0; hrow < 2; ++hrow) {
+        const int r = wr + hrow * 8;
+        *reinterpret_cast<float2*>(buf + ((i >> 1) & 1) * kPwBoxBytes + r * 64 + (((cc >> 2) ^ ((r >> 1) & 3)) << 4) +
+                                   (cc & 3) * 4) = make_float2(accm[4 * i + 2 * hrow], accm[4 * i + 2 * hrow + 1]);
+      }
+    }
+    fence_proxy_async_smem();  // generic-proxy writes -> visible to the TMA engine
+    wg_sync(wgc);
+    if (leader) {
+#pragma unroll
+      for (int b = 0; b < 2 && 32 * s + 16 * b < NT; ++b) {
+        const int col0 = nt * NT + 32 * s + 16 * b;
+        if (col0 < p.N && row0 < p.M) tma_store_2d(tmC, buf + b * kPwBoxBytes, col0, (int)row0);
+      }
+      tma_store_commit();
+    }
+  }
+}
+
 // DWK = 0: plain 1x1 conv.  DWK = 3 | 5 (option "fuse_dwpw", on by default; MW x MW maps with MW = 16 | 32, stride 1): the
 // layer's input is the output of a DWK x DWK depthwise conv that is never materialised -- the producer TMA-loads the
 // depthwise INPUT box of each (128-pixel tile, 32-channel chunk) with its zero-filled halo (tmA is then the 4-D NHWC
@@ -289,22 +363,25 @@ __device__ __forceinline__ void pw_epilogue(const PwParams& p, const float* accm
 // warpgroups share each tile (64 rows each, weights fetched once per 128 rows).  A consumer issues chunk c's MMA group
 // and then waits only for chunk c - 1's (wgmma.wait_group 1), which frees c - 1's stage and A fragments; in the fused
 // forms chunk c + 1's depthwise conv runs while chunk c's group is in flight.  wait_group 0 only before the epilogue.
+// Each consumer warpgroup then stores its 64 rows by TMA from shared memory (pw_epilogue_tma) and goes straight on to
+// the next tile; with p.tma_store == 0 it stores from registers (pw_epilogue).
 template <int NT, int DWK, int MW = 16>
 __global__ void __launch_bounds__(kPwThreads, 1)
 pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWh,
              const __grid_constant__ CUtensorMap tmWl, const __grid_constant__ CUtensorMap tmDW,
-             const __grid_constant__ CUtensorMap tmDB, const PwParams p) {
+             const __grid_constant__ CUtensorMap tmDB, const __grid_constant__ CUtensorMap tmC, const PwParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int S = p.stages;
-  constexpr int a_bufs = DWK > 0 ? 2 : 0;  // fused: the A tiles the consumers write live outside the ring
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * p.stage_bytes + a_bufs * kCorrABytes);  // [stages] TMA landed
+  // two 16 KB buffers after the ring: the epilogue's staging slabs and, in the fused forms, the A tiles
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * p.stage_bytes + 2 * kCorrABytes);  // [stages] TMA landed
   uint64_t* empty = full + S;  // [stages] 8 consumer warps done
   constexpr int w_bytes = NT * 128;
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmWh);
     prefetch_tmap(&tmWl);
+    if (p.tma_store) prefetch_tmap(&tmC);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 8);
@@ -316,9 +393,13 @@ pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   pdl_wait();     // everything above overlapped the previous kernel's tail; its results are visible from here on
 
   // plain stage: [A tile 16 KB][w_hi][w_lo]; fused stage: [w_hi][w_lo][input box][dw weights DWK*DWK x 32][dw bias 32],
-  // then two A tiles after the ring.  A fused A tile is free once every consumer has loaded its fragments, long
-  // before the stage's weights are (their MMAs still run), so two of them serve any ring depth and the room they
-  // leave buys the ring a third stage.
+  // then two 16 KB buffers after the ring.  Each holds one staging slab of each consumer warpgroup (warpgroup w's 8 KB
+  // at offset 8 KB * w).  In the fused forms the buffers are also the A tiles: an A tile is free once every consumer has
+  // loaded its fragments, long before the stage's weights are (their MMAs still run), so two of them serve any ring
+  // depth and the room they leave buys the ring a third stage.  A warpgroup stages only its own rows of an A tile,
+  // which only it reads, once its last MMA group is done.  The tile's last slab goes to the last chunk's A tile, so the
+  // next tile's first depthwise conv, which writes the other A tile, waits only for the slabs before it (wait_group.read
+  // 1, then consumer_sync), and the last slab need only be read before the barrier that follows that conv.
   auto a_tile = [&](int s) { return smem + s * p.stage_bytes; };
   auto a_buf = [&](int b) { return smem + S * p.stage_bytes + b * kCorrABytes; };
   auto w_hi = [&](int s) { return smem + s * p.stage_bytes + (DWK > 0 ? 0 : kCorrABytes); };
@@ -362,17 +443,26 @@ pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   setmaxnreg_inc<kPwConsumerRegs>();
 
   const int ct = threadIdx.x - 128, warp = ct >> 5, lane = ct & 31;  // consumer thread / warp (0..255 / 0..7)
-  const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), t = lane & 3;
+  const int wgc = warp >> 2, wr = (warp & 3) * 16 + (lane >> 2), t = lane & 3;  // consumer warpgroup, row inside it
+  const int r0 = wgc * 64 + wr;
+  const bool leader = (ct & 127) == 0;  // issues the warpgroup's TMA stores
   int stage = 0, ab = 0;  // ring stage, fused A buffer of the current chunk
   uint32_t phase = 0;
+  int slab = 0;  // staging slabs written so far (plain form: the buffers alternate over the CTA's slabs)
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     const int mt = tile / p.num_n_tiles, nt = tile - mt * p.num_n_tiles;
     float accm[NT / 2], accc[NT / 2];
 #pragma unroll
     for (int i = 0; i < NT / 2; ++i) accm[i] = accc[i] = 0.f;
     if constexpr (DWK > 0) {
+      const bool drain = p.tma_store && tile != blockIdx.x;  // the previous tile's slabs lie in the A tiles
+      if (drain) {
+        if (leader) tma_store_wait_read<1>();
+        consumer_sync();
+      }
       mbar_wait(&full[stage], phase);
       dw_chunk<DWK, MW>(dw_box(stage), dw_wts(stage), dw_bia(stage), a_buf(ab), ct, p.dw_bias, p.dw_relu);
+      if (drain && leader) tma_store_wait_read<0>();  // before the next depthwise conv writes the last slab's A tile
       consumer_sync();  // the A tile of this chunk is complete
     }
     int prev = 0;
@@ -410,8 +500,15 @@ pw_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     wg_wait_n<0>();
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev]);
-    pw_epilogue<NT>(p, accm, accc, mt, nt, r0, t);
+    if (p.tma_store) {
+      const int lb = DWK > 0 ? ab ^ 1 : (slab + pw_slabs<NT>() - 1) & 1;  // fused: the last chunk's A tile
+      slab += pw_slabs<NT>();
+      pw_epilogue_tma<NT>(p, &tmC, accm, accc, mt, nt, wgc, wr, t, a_buf(lb) + wgc * kPwSlabBytes,
+                          a_buf(lb ^ 1) + wgc * kPwSlabBytes, leader);
+    } else
+      pw_epilogue<NT>(p, accm, accc, mt, nt, r0, t);
   }
+  if (leader && p.tma_store) tma_store_wait<0>();  // the stores are complete before the CTA exits
 }
 
 // One-chunk GEMMs (K <= 32) on narrow tiles: one CTA per tile, 288 threads (two consumer warpgroups and one TMA
@@ -497,6 +594,20 @@ inline int pw_stages(int stage_bytes, int fixed_bytes) {
   return fit < kPwMaxStages ? fit : kPwMaxStages;
 }
 
+// The plain persistent kernel keeps its two staging buffers next to a full ring at the widest tile.
+constexpr int kPwStagingBytes = 2 * kCorrABytes;
+static_assert(kPwMaxStages * (kCorrABytes + 2 * 128 * 128) + kPwStagingBytes + kPwSmemExtra <= kPwMaxSmem,
+              "pw_tc_kernel<128, 0>: four ring stages and the staging buffers fit in shared memory");
+
+// Output map of pw_tc_kernel's TMA stores: C = [M][N] at row pitch ldc, boxes of 64 rows x 16 columns.  16 divides every
+// tile width, so a box never reaches into a neighbouring n-tile, and the N extent keeps the stores out of columns >= N of
+// a wider buffer (the head's 320-column concat buffer).  TMA needs a 16-byte aligned base and pitch: returns 1 when
+// either is not, and the kernel then stores from registers.
+inline int make_tmap_out(CUtensorMap* m, float* C, int ldc, int M, int N) {
+  if ((reinterpret_cast<uintptr_t>(C) & 15) || (ldc & 3)) return 1;
+  return make_tmap_2d(m, C, (uint64_t)M, (uint64_t)N, (uint64_t)ldc, 64, 16);
+}
+
 // Output-channel tile for a layer: the layer is cut into the fewest tiles of <= 128 columns (two accumulators of
 // NT / 2 registers per thread), each the narrowest instantiated width that covers its share; the last tile may hang
 // over N (weight rows >= N are zero-filled by TMA, the store is clipped).
@@ -567,9 +678,9 @@ inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi,
   p.num_tiles = ((M + 127) / 128) * p.num_n_tiles;
   p.last_ksteps = ((K - 32 * (p.num_chunks - 1)) + 7) / 8;
   p.relu = relu;
-  p.dw_relu = p.dw_bias = p.box_bytes = 0;
+  p.dw_relu = p.dw_bias = p.box_bytes = p.tma_store = 0;
   p.stage_bytes = kCorrABytes + 2 * NT * 128;
-  p.stages = narrow ? 1 : pw_stages(p.stage_bytes, 0);
+  p.stages = narrow ? 1 : pw_stages(p.stage_bytes, kPwStagingBytes);
   CUtensorMap tmA, tmWh, tmWl;
   int r = make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 128, 32);
   if (r) return r;
@@ -577,17 +688,23 @@ inline int launch_pw(cudaStream_t s, const float* A, int lda, const float* w_hi,
   if (r) return r;
   r = make_tmap_2d(&tmWl, w_lo, (uint64_t)N, (uint64_t)K, (uint64_t)K, NT, 32);
   if (r) return r;
-  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + kPwSmemExtra;
   cudaError_t e = cudaErrorInvalidValue;
   if (narrow) {
+    const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + kPwSmemExtra;
     if (NT == 16) e = launch_pdl(pw_tc_narrow_kernel<16>, dim3(p.num_tiles), dim3(kTcThreads), smem_bytes, s, tmA, tmWh, tmWl, p);
     else e = launch_pdl(pw_tc_narrow_kernel<32>, dim3(p.num_tiles), dim3(kTcThreads), smem_bytes, s, tmA, tmWh, tmWl, p);
     return e == cudaSuccess ? 0 : -23;
   }
+  CUtensorMap tmC = tmA;
+  r = make_tmap_out(&tmC, C, ldc, M, N);
+  if (r < 0) return r;
+  p.tma_store = r == 0;
+  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + kPwStagingBytes + kPwSmemExtra;
   switch (NT) {
 #define FEAR_PW_CASE(NT_)                                                                                               \
   case NT_:                                                                                                             \
-    e = launch_pdl(pw_tc_kernel<NT_, 0>, pw_grid(p.num_tiles), dim3(kPwThreads), smem_bytes, s, tmA, tmWh, tmWl, tmA, tmA, p); \
+    e = launch_pdl(pw_tc_kernel<NT_, 0>, pw_grid(p.num_tiles), dim3(kPwThreads), smem_bytes, s, tmA, tmWh, tmWl, tmA, tmA, \
+                   tmC, p);                                                                                             \
     break;
     FEAR_PW_FOR_NT(FEAR_PW_CASE)
 #undef FEAR_PW_CASE
@@ -627,9 +744,9 @@ inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const f
   p.box_bytes = ih * iw * 128;
   p.stage_bytes = (2 * NT * 128 + p.box_bytes + dw_k * dw_k * 128 + 128 + 1023) & ~1023;
   if ((p.num_chunks < 2 ? 1 : 2) * (kCorrABytes + p.stage_bytes) + kPwSmemExtra > kPwMaxSmem) return 1;
-  p.stages = pw_stages(p.stage_bytes, 2 * kCorrABytes);
+  p.stages = pw_stages(p.stage_bytes, 2 * kCorrABytes);  // the two A tiles double as the epilogue's staging
   const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 2 * kCorrABytes + kPwSmemExtra;
-  CUtensorMap tmX, tmWh, tmWl, tmDW, tmDB;
+  CUtensorMap tmX, tmWh, tmWl, tmDW, tmDB, tmC;
   int r = make_tmap_nhwc(&tmX, X, (uint64_t)B, (uint64_t)map_w, (uint64_t)map_w, (uint64_t)K, 32, iw, ih);
   if (r) return r;
   r = make_tmap_2d(&tmWh, w_hi, (uint64_t)N, (uint64_t)K, (uint64_t)K, NT, 32);
@@ -644,9 +761,16 @@ inline int launch_pw_dw(cudaStream_t s, const float* X, int B, int dw_k, const f
   } else {
     tmDB = tmDW;
   }
+  // At NT <= 32 a tile is one staging slab, whose barriers and drain cost more next to the depthwise conv than the TMA
+  // store saves (xif3_1 .. xif3_3, DESIGN.md 4.1): those tiles keep the stores from registers.
+  tmC = tmX;
+  r = NT > 32 ? make_tmap_out(&tmC, C, ldc, M, N) : 1;
+  if (r < 0) return r;
+  p.tma_store = r == 0;
   cudaError_t e = cudaErrorInvalidValue;
-#define FEAR_PW_DW_LAUNCH(NT_, K_, MW_) \
-  e = launch_pdl(pw_tc_kernel<NT_, K_, MW_>, pw_grid(p.num_tiles), dim3(kPwThreads), smem_bytes, s, tmX, tmWh, tmWl, tmDW, tmDB, p)
+#define FEAR_PW_DW_LAUNCH(NT_, K_, MW_)                                                                              \
+  e = launch_pdl(pw_tc_kernel<NT_, K_, MW_>, pw_grid(p.num_tiles), dim3(kPwThreads), smem_bytes, s, tmX, tmWh, tmWl, \
+                 tmDW, tmDB, tmC, p)
   switch (NT) {
 #define FEAR_PW_CASE(NT_)                                \
   case NT_:                                              \
