@@ -47,6 +47,9 @@ assert YCBCR_DTYPE.itemsize == 88
 # FearFrameYCbCrV210: FearFrameYCbCr plus whether the entry is a v210 surface (10-bit 4:2:2, three codes per word)
 YCBCR_V210_DTYPE = np.dtype(YCBCR_DTYPE.descr + [("v210", "<i4"), ("reserved", "<i4")])
 assert YCBCR_V210_DTYPE.itemsize == 96
+# FearFrameYCbCrHDR: FearFrameYCbCrV210 plus the H.273 transfer characteristics (0, PQ 16, HLG 18)
+YCBCR_HDR_DTYPE = np.dtype(YCBCR_V210_DTYPE.descr + [("transfer", "<i4"), ("reserved_hdr", "<i4")])
+assert YCBCR_HDR_DTYPE.itemsize == 104
 # FearFrameBayer: a raw Bayer mosaic (unpacked 8 to 16 bits, MIPI RAW10 / RAW12) with its row pitch and CFA pattern
 BAYER_DTYPE = np.dtype([("data", "<u8"), ("row_stride", "<i8"), ("H", "<i4"), ("W", "<i4"), ("pattern", "<i4"),
                         ("bits", "<i4"), ("shift", "<i4"), ("packing", "<i4")])
@@ -89,6 +92,9 @@ _SIGNATURES = {
     "fear_crop_targets_ycbcr_v210_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_ycbcr_v210": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_ycbcr_v210_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_ycbcr_hdr_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_ycbcr_hdr": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_ycbcr_hdr_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_crop_targets_bayer_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_bayer": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_bayer_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),

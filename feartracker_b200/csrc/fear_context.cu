@@ -1050,6 +1050,9 @@ static_assert(sizeof(FearFrameYUV) == 80, "FearFrameYUV layout is part of the AB
 static_assert(sizeof(FearFrameYCbCr) == 88, "FearFrameYCbCr layout is part of the ABI");
 static_assert(sizeof(FearFrameYCbCrV210) == 96 && offsetof(FearFrameYCbCrV210, v210) == 88,
               "FearFrameYCbCrV210 layout is part of the ABI");
+static_assert(sizeof(FearFrameYCbCrHDR) == 104 && offsetof(FearFrameYCbCrHDR, v210) == 88 &&
+                  offsetof(FearFrameYCbCrHDR, transfer) == 96,
+              "FearFrameYCbCrHDR layout is part of the ABI");
 static_assert(sizeof(FearFrameBayer) == 40 && offsetof(FearFrameBayer, packing) == 36,
               "FearFrameBayer layout is part of the ABI");
 
@@ -1210,6 +1213,26 @@ extern "C" int fear_advance_targets_ycbcr_v210(const FearBox* d_boxes, const Fea
 extern "C" int fear_frame_sums_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, uint64_t* d_sums,
                                              void* stream) {
   return launch_frame_sums(d_views, YCbCrV210Frames{d_views}, F, d_sums, stream);
+}
+
+// FearFrameYCbCrV210 entries with a transfer function (PQ, HLG tone-mapped to SDR in each tap): the same kernels,
+// reading through YCbCrHDRFrames.
+extern "C" int fear_crop_targets_ycbcr_hdr_u8(const FearFrameYCbCrHDR* d_views, int F, FearTarget* d_targets, int N,
+                                              double offset, int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_views || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(YCbCrHDRFrames{d_views}, F, d_targets, N, offset, out_size, d_crops, stream);
+}
+
+extern "C" int fear_advance_targets_ycbcr_hdr(const FearBox* d_boxes, const FearFrameYCbCrHDR* d_views, int F,
+                                              FearTarget* d_targets, int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_views || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return launch_advance_targets(d_boxes, YCbCrHDRFrames{d_views}, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_frame_sums_ycbcr_hdr_u8(const FearFrameYCbCrHDR* d_views, int F, uint64_t* d_sums, void* stream) {
+  return launch_frame_sums(d_views, YCbCrHDRFrames{d_views}, F, d_sums, stream);
 }
 
 // Raw Bayer mosaics: the same kernels, reading through BayerFrames (each tap demosaiced as cv2.cvtColor does).

@@ -14,9 +14,10 @@
 // FearFrameYUV (YUVFrames, 4:2:0, the format named per entry) or FearFrameYCbCr (YCbCrFrames, 4:2:0, 4:2:2 or 4:4:4 and
 // the format named per entry), all read through YUVFrame, which converts each pixel it reads to RGB; or a table of
 // FearFrameYCbCrV210 records (YCbCrV210Frames), read through V210Frame, which also unpacks v210 surfaces; or a table of
-// FearFrameBayer records (BayerFrames), read through BayerFrame, which demosaics raw Bayer mosaics.  A frame type gives
-// H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables, interpolation, sums and
-// the colour conversion exist once.
+// FearFrameYCbCrHDR records (YCbCrHDRFrames), read through HDRFrame, which also tone-maps PQ and HLG video to SDR; or a
+// table of FearFrameBayer records (BayerFrames), read through BayerFrame, which demosaics raw Bayer mosaics.  A frame
+// type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables,
+// interpolation, sums and the colour conversion exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
 // into an FMA by default, which rounds once instead of twice, so every multiply-add here is spelled with the explicitly
@@ -126,6 +127,13 @@ struct YUVFrame {
     const long long c = (long long)(y >> csy) * uvrs + (long long)(x >> csx) * uvps;
     convert(sample(Y + (long long)y * yrs + (long long)x * yps), sample(U + c), sample(V + c), p);
   }
+  // the codes (Y, Cb, Cr) of pixel (y, x), as rgb() reads them
+  __device__ __forceinline__ void codes(int y, int x, int c[3]) const {
+    const long long o = (long long)(y >> csy) * uvrs + (long long)(x >> csx) * uvps;
+    c[0] = sample(Y + (long long)y * yrs + (long long)x * yps);
+    c[1] = sample(U + o);
+    c[2] = sample(V + o);
+  }
   // the RGB triple of the codes (Yc, Uc, Vc) in this frame's format
   __device__ __forceinline__ void convert(int Yc, int Uc, int Vc, int p[3]) const {
     if (!h273) {
@@ -138,6 +146,16 @@ struct YUVFrame {
     p[0] = yuv_unit_to_u8(__dadd_rn(yn, __dmul_rn(k.cR, pr)));
     p[1] = yuv_unit_to_u8(__dsub_rn(__dsub_rn(yn, __dmul_rn(k.gB, pb)), __dmul_rn(k.gR, pr)));
     p[2] = yuv_unit_to_u8(__dadd_rn(yn, __dmul_rn(k.cB, pb)));
+  }
+  // the unclamped R'G'B' of the H.273 inverse of the codes (Yc, Uc, Vc), before the rounding to 8 bits: convert()'s
+  // arithmetic, kept apart so the SDR conversion compiles as it always has
+  __device__ __forceinline__ void h273_rgb(int Yc, int Uc, int Vc, double e[3]) const {
+    const double yn = __dmul_rn(__dsub_rn((double)Yc, k.y0), k.ys);
+    const double pb = __dmul_rn(__dsub_rn((double)Uc, k.c0), k.cs);
+    const double pr = __dmul_rn(__dsub_rn((double)Vc, k.c0), k.cs);
+    e[0] = __dadd_rn(yn, __dmul_rn(k.cR, pr));
+    e[1] = __dsub_rn(__dsub_rn(yn, __dmul_rn(k.gB, pb)), __dmul_rn(k.gR, pr));
+    e[2] = __dadd_rn(yn, __dmul_rn(k.cB, pb));
   }
 };
 
@@ -231,9 +249,21 @@ struct V210Frame : YUVFrame {
       YUVFrame::rgb(y, x, p);
       return;
     }
+    int c[3];
+    codes(y, x, c);
+    convert(c[0], c[1], c[2], p);
+  }
+  // the codes (Y, Cb, Cr) of pixel (y, x), of either kind
+  __device__ __forceinline__ void codes(int y, int x, int c[3]) const {
+    if (!v210) {
+      YUVFrame::codes(y, x, c);
+      return;
+    }
     const unsigned g = (unsigned)x / 6, r = (unsigned)x - 6 * g, k = r >> 1;
     const uint8_t* q = Y + (long long)y * yrs + 16LL * g;
-    convert(code(q, 2 * r + 1), code(q, 4 * k), code(q, 4 * k + 2), p);
+    c[0] = code(q, 2 * r + 1);
+    c[1] = code(q, 4 * k);
+    c[2] = code(q, 4 * k + 2);
   }
 };
 
@@ -246,14 +276,18 @@ struct V210Frame : YUVFrame {
 struct YCbCrV210Frames {
   const FearFrameYCbCrV210* views;
   __device__ __forceinline__ V210Frame operator()(int i) const {
-    const FearFrameYCbCrV210* p = views + i;
+    return v210_frame_of(views + i);
+  }
+  // also the FearFrameYCbCrV210 fields that lead a FearFrameYCbCrHDR record
+  template <class Record>
+  static __device__ __forceinline__ V210Frame v210_frame_of(const Record* p) {
     const int v210 = p->v210;
     if (v210 != 1) {
       V210Frame f{YCbCrFrames::ycbcr_frame_of(p), false};
       f.bad |= v210 != 0;
       return f;
     }
-    const FearFrameYCbCrV210 v = *p;
+    const Record v = *p;
     const uint8_t* y = static_cast<const uint8_t*>(v.y);
     const long long pitch = v.y_row_stride;
     const bool ok = !(((uintptr_t)y | (uintptr_t)pitch) & 3) && pitch >= 16LL * (((long long)v.W + 5) / 6) &&
@@ -263,6 +297,125 @@ struct YCbCrV210Frames {
     return V210Frame{{y, y, y, pitch, 0, 0, 0, v.H, v.W, 1, 0, 10, 0, true, true, !ok,
                       ok ? yuv_coefs(v.matrix, v.full_range, 10) : YUVCoefs{}},
                      true};
+  }
+};
+
+// The HDR chain of FearFrameYCbCrHDR (include/fear_b200.h), restating image_ops.hdr_to_sdr step by step: every float64
+// operation is a rounded intrinsic (no FMA contraction), exp / log / pow come from CUDA's double library.  The derived
+// constants are folded rather than derived per thread: each is the hex literal of the float64 that
+// image_ops.HDR_CONSTANTS names by the same hex string (tests/test_hdr_cpu.py checks the two agree and that each is its
+// derivation), so no libm or constant folding on either side can change a bit.  The BT.2020 -> BT.709 matrix is
+// image_ops.bt2020_to_bt709_matrix(), derived once in Python floats from the primaries and D65 and held here the same way.
+constexpr double kPqC1 = 3424.0 / 4096.0, kPqC2 = 2413.0 / 4096.0 * 32.0, kPqC3 = 2392.0 / 4096.0 * 32.0;  // exact
+constexpr double kHdrPqInvM1 = 0x1.91c0d56e7162bp+2;  // 1 / m1, m1 = 2610 / 16384
+constexpr double kHdrPqInvM2 = 0x1.9f9b5860989b1p-7;  // 1 / m2, m2 = 2523 / 4096 * 128
+constexpr double kHdrHlgA = 0.17883277;
+constexpr double kHdrHlgB = 0x1.23803fd659be6p-2;     // 1 - 4a
+constexpr double kHdrHlgC = 0x1.1eac9e800497cp-1;     // 0.5 - a ln(4a)
+constexpr double kHdrInv24 = 0x1.aaaaaaaaaaaabp-2;    // 1 / 2.4
+constexpr double kHdrRhoHdrM1 = 0x1.885043b97c4bap+3; // rho_HDR - 1, rho_HDR = 1 + 32 (1000 / 10000)^(1 / 2.4)
+constexpr double kHdrLnRhoHdr = 0x1.4ad8a755a96c8p+1; // ln(rho_HDR)
+constexpr double kHdrRhoSdr = 0x1.6c9af449393ffp+2;   // rho_SDR = 1 + 32 (100 / 10000)^(1 / 2.4)
+constexpr double kHdrRhoSdrM1 = 0x1.2c9af449393ffp+2; // rho_SDR - 1
+__device__ constexpr double kHdrGamut[3][3] = {       // linear BT.2020 -> linear BT.709
+    {0x1.a915f0355ba58p+0, -0x1.2cdf4ca1c314bp-1, -0x1.2a649e47a1b10p-4},
+    {-0x1.fe28a36c581d8p-4, 0x1.2205ba47cc3a2p+0, -0x1.119808835c29cp-7},
+    {-0x1.2961d1c06ea4dp-6, -0x1.9bf89e59cb351p-4, 0x1.1e65112c9e6dep+0}};
+
+__device__ __forceinline__ double hdr_clamp01(double v) { return fmin(fmax(v, 0.0), 1.0); }
+
+// SMPTE ST 2084 EOTF: E' in [0, 1] -> cd/m2
+__device__ __forceinline__ double hdr_pq_light(double e) {
+  const double p = pow(e, kHdrPqInvM2);
+  const double r = __ddiv_rn(fmax(__dsub_rn(p, kPqC1), 0.0), __dsub_rn(kPqC2, __dmul_rn(kPqC3, p)));
+  return __dmul_rn(10000.0, pow(r, kHdrPqInvM1));
+}
+
+// BT.2100 HLG inverse OETF: E' in [0, 1] -> scene light in [0, 1]
+__device__ __forceinline__ double hdr_hlg_scene(double e) {
+  if (e <= 0.5) return __ddiv_rn(__dmul_rn(e, e), 3.0);
+  return __ddiv_rn(__dadd_rn(exp(__ddiv_rn(__dsub_rn(e, kHdrHlgC), kHdrHlgA)), kHdrHlgB), 12.0);
+}
+
+// Y' = 0.2627 R' + 0.6780 G' + 0.0593 B' (also HLG's Ys), left to right
+__device__ __forceinline__ double hdr_luma(const double c[3]) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(0.2627, c[0]), __dmul_rn(0.6780, c[1])), __dmul_rn(0.0593, c[2]));
+}
+
+// BT.2446-1 Method A's tone curve Y'p -> Y'c
+__device__ __forceinline__ double hdr_method_a_curve(double yp) {
+  if (yp <= 0.7399) return __dmul_rn(1.077, yp);
+  if (yp < 0.9909) return __dsub_rn(__dadd_rn(__dmul_rn(-1.1510, __dmul_rn(yp, yp)), __dmul_rn(2.7811, yp)), 0.6302);
+  return __dadd_rn(__dmul_rn(0.5, yp), 0.5);
+}
+
+// The 8-bit SDR BT.709 triple of the unclamped BT.2020 R'G'B' e under transfer FEAR_TRC_PQ or FEAR_TRC_HLG.
+__device__ __forceinline__ void hdr_to_sdr(int transfer, const double e[3], int p[3]) {
+  double c[3];
+  if (transfer == FEAR_TRC_PQ) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) c[i] = hdr_pq_light(hdr_clamp01(e[i]));
+  } else {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) c[i] = hdr_hlg_scene(hdr_clamp01(e[i]));
+    const double scale = __dmul_rn(1000.0, pow(hdr_luma(c), 0.2));
+#pragma unroll
+    for (int i = 0; i < 3; ++i) c[i] = __dmul_rn(scale, c[i]);
+  }
+  // normalise to the 1000 cd/m2 peak, then BT.2446-1 Method A on L^(1 / 2.4)
+#pragma unroll
+  for (int i = 0; i < 3; ++i) c[i] = pow(fmin(__ddiv_rn(c[i], 1000.0), 1.0), kHdrInv24);
+  const double y = hdr_luma(c);
+  const double yp = __ddiv_rn(log(__dadd_rn(1.0, __dmul_rn(kHdrRhoHdrM1, y))), kHdrLnRhoHdr);
+  const double ysdr = __ddiv_rn(__dsub_rn(pow(kHdrRhoSdr, hdr_method_a_curve(yp)), 1.0), kHdrRhoSdrM1);
+  const double f = y == 0.0 ? 0.0 : __ddiv_rn(ysdr, __dmul_rn(1.1, y));
+  const double cb = __ddiv_rn(__dmul_rn(f, __dsub_rn(c[2], y)), 1.8814);
+  const double cr = __ddiv_rn(__dmul_rn(f, __dsub_rn(c[0], y)), 1.4746);
+  const double ytmo = __dsub_rn(ysdr, fmax(__dmul_rn(0.1, cr), 0.0));
+  // the BT.2020 inverse, back to linear light, the gamut matrix, then BT.709 R'G'B'
+  const double r2 = __dadd_rn(ytmo, __dmul_rn(1.4746, cr));
+  const double b2 = __dadd_rn(ytmo, __dmul_rn(1.8814, cb));
+  const double g2 = __ddiv_rn(__dsub_rn(__dsub_rn(ytmo, __dmul_rn(0.2627, r2)), __dmul_rn(0.0593, b2)), 0.6780);
+  const double lin[3] = {pow(hdr_clamp01(r2), 2.4), pow(hdr_clamp01(g2), 2.4), pow(hdr_clamp01(b2), 2.4)};
+  // one output channel at a time: fully unrolled, the frame-sums instantiation spills a register around the library
+  // calls (ptxas -v)
+#pragma unroll 1
+  for (int i = 0; i < 3; ++i) {
+    const double v = __dadd_rn(__dadd_rn(__dmul_rn(kHdrGamut[i][0], lin[0]), __dmul_rn(kHdrGamut[i][1], lin[1])),
+                               __dmul_rn(kHdrGamut[i][2], lin[2]));
+    p[i] = yuv_unit_to_u8(pow(hdr_clamp01(v), kHdrInv24));
+  }
+}
+
+// A frame of a FearFrameYCbCrHDR table: a V210Frame read as it is (transfer 0), or its codes through the H.273 inverse
+// and the HDR chain (transfer FEAR_TRC_PQ or FEAR_TRC_HLG).  A value-initialised HDRFrame{} is empty.
+struct HDRFrame : V210Frame {
+  int transfer;
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    if (transfer == 0) {
+      V210Frame::rgb(y, x, p);
+      return;
+    }
+    int c[3];
+    double e[3];
+    codes(y, x, c);
+    h273_rgb(c[0], c[1], c[2], e);
+    hdr_to_sdr(transfer, e, p);
+  }
+};
+
+// Frame i of a FearFrameYCbCrHDR table (the *_ycbcr_hdr entry points): its FearFrameYCbCrV210 fields read exactly as
+// YCbCrV210Frames reads them, and the transfer.  Unreadable besides: a transfer other than 0, FEAR_TRC_PQ and
+// FEAR_TRC_HLG, or an HDR transfer with a matrix other than BT.2020 or 8-bit samples.
+struct YCbCrHDRFrames {
+  const FearFrameYCbCrHDR* views;
+  __device__ __forceinline__ HDRFrame operator()(int i) const {
+    const FearFrameYCbCrHDR* p = views + i;
+    const int t = p->transfer;
+    HDRFrame f{YCbCrV210Frames::v210_frame_of(p), t};
+    const bool hdr = (t == FEAR_TRC_PQ || t == FEAR_TRC_HLG) && p->matrix == FEAR_YUV_BT2020 && p->bits != 8;
+    f.bad |= !(t == 0 || hdr);
+    return f;
   }
 };
 

@@ -6,6 +6,7 @@ boxes, constant-colour padding, cv2 bilinear resize, ImageNet normalisation in f
 ``albumentations`` is not required: its Resize is ``cv2.resize(INTER_LINEAR)`` and its Normalize
 is ``(img - mean*255) * (1/(std*255))`` in float32.
 """
+import math
 from typing import Optional, Sequence, Tuple
 
 import cv2
@@ -168,11 +169,164 @@ YUV_MATRICES = {"bt601": (0, 0.299, 0.114), "bt709": (1, 0.2126, 0.0722), "bt202
 
 
 def yuv420_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601", full_range: bool = False,
-                  bits: int = 8, shift: int = 0) -> np.ndarray:
+                  bits: int = 8, shift: int = 0, transfer: Optional[str] = None) -> np.ndarray:
     """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for a YUV 4:2:0 frame: luma ``y`` (H, W), chroma ``u`` (Cb)
     and ``v`` (Cr) (H/2, W/2) of raw samples, pixel (r, c) taking chroma sample (r // 2, c // 2).  ``yuv_to_rgb`` with
     ``chroma_shift=(1, 1)``."""
-    return yuv_to_rgb(y, u, v, matrix, full_range, bits, shift, (1, 1))
+    return yuv_to_rgb(y, u, v, matrix, full_range, bits, shift, (1, 1), transfer)
+
+
+# HDR transfers of yuv_to_rgb and FearFrameYCbCrHDR: name -> ITU-T H.273 TransferCharacteristics code (None: 0, the
+# matrix only)
+HDR_TRANSFERS = {"pq": 16, "hlg": 18}
+
+# SMPTE ST 2084 (PQ) constants; every one is exact in float64
+PQ_M1, PQ_M2 = 2610.0 / 16384.0, 2523.0 / 4096.0 * 128.0
+PQ_C1, PQ_C2, PQ_C3 = 3424.0 / 4096.0, 2413.0 / 4096.0 * 32.0, 2392.0 / 4096.0 * 32.0
+HLG_A = 0.17883277
+# The HDR chain's derived constants, folded: each is the float64 named by its hex string, which the crop kernel spells
+# with the same hex literal (csrc/kernels_track_loop.cuh, kHdr*), so numpy and CUDA start from identical bits whatever
+# either side's libm or constant folding would give.  HDR_CONSTANT_DERIVATIONS states how each was derived.
+HDR_CONSTANTS = {
+    "pq_inv_m1": float.fromhex("0x1.91c0d56e7162bp+2"),      # 1 / m1
+    "pq_inv_m2": float.fromhex("0x1.9f9b5860989b1p-7"),      # 1 / m2
+    "hlg_b": float.fromhex("0x1.23803fd659be6p-2"),          # 1 - 4a
+    "hlg_c": float.fromhex("0x1.1eac9e800497cp-1"),          # 0.5 - a ln(4a)
+    "inv_2_4": float.fromhex("0x1.aaaaaaaaaaaabp-2"),        # 1 / 2.4
+    "rho_hdr_m1": float.fromhex("0x1.885043b97c4bap+3"),     # rho_HDR - 1, rho_HDR = 1 + 32 (1000 / 10000)^(1 / 2.4)
+    "ln_rho_hdr": float.fromhex("0x1.4ad8a755a96c8p+1"),     # ln(rho_HDR)
+    "rho_sdr": float.fromhex("0x1.6c9af449393ffp+2"),        # rho_SDR = 1 + 32 (100 / 10000)^(1 / 2.4)
+    "rho_sdr_m1": float.fromhex("0x1.2c9af449393ffp+2"),     # rho_SDR - 1
+}
+HDR_CONSTANT_DERIVATIONS = {
+    "pq_inv_m1": lambda: 1.0 / PQ_M1,
+    "pq_inv_m2": lambda: 1.0 / PQ_M2,
+    "hlg_b": lambda: 1.0 - 4.0 * HLG_A,
+    "hlg_c": lambda: 0.5 - HLG_A * math.log(4.0 * HLG_A),
+    "inv_2_4": lambda: 1.0 / 2.4,
+    "rho_hdr_m1": lambda: (1.0 + 32.0 * (1000.0 / 10000.0) ** (1.0 / 2.4)) - 1.0,
+    "ln_rho_hdr": lambda: math.log(1.0 + 32.0 * (1000.0 / 10000.0) ** (1.0 / 2.4)),
+    "rho_sdr": lambda: 1.0 + 32.0 * (100.0 / 10000.0) ** (1.0 / 2.4),
+    "rho_sdr_m1": lambda: (1.0 + 32.0 * (100.0 / 10000.0) ** (1.0 / 2.4)) - 1.0,
+}
+
+# CIE 1931 xy of the BT.2020 and BT.709 primaries (R, G, B) and of D65
+BT2020_PRIMARIES = ((0.708, 0.292), (0.170, 0.797), (0.131, 0.046))
+BT709_PRIMARIES = ((0.64, 0.33), (0.30, 0.60), (0.15, 0.06))
+D65_WHITE = (0.3127, 0.3290)
+
+
+def _inverse3(m):
+    """The inverse of a 3 x 3 matrix (nested lists of Python floats) by the adjugate, each operation rounded on its
+    own: no LAPACK, so every platform derives the same bits."""
+    (a, b, c), (d, e, f), (g, h, i) = m
+    adj = [[e * i - f * h, c * h - b * i, b * f - c * e],
+           [f * g - d * i, a * i - c * g, c * d - a * f],
+           [d * h - e * g, b * g - a * h, a * e - b * d]]
+    det = (a * adj[0][0] + b * adj[1][0]) + c * adj[2][0]
+    return [[v / det for v in row] for row in adj]
+
+
+def _matmul3(p, q):
+    return [[(p[r][0] * q[0][c] + p[r][1] * q[1][c]) + p[r][2] * q[2][c] for c in range(3)] for r in range(3)]
+
+
+def _rgb_to_xyz(primaries, white):
+    """The normalised primary matrix (SMPTE RP 177): linear RGB -> CIE XYZ for the primaries' xy and the white's xy."""
+    cols = [[x / y, 1.0, ((1.0 - x) - y) / y] for x, y in primaries]
+    p = [[cols[c][r] for c in range(3)] for r in range(3)]
+    wx, wy = white
+    w = [wx / wy, 1.0, ((1.0 - wx) - wy) / wy]
+    s = [(pi[0] * w[0] + pi[1] * w[1]) + pi[2] * w[2] for pi in _inverse3(p)]
+    return [[p[r][c] * s[c] for c in range(3)] for r in range(3)]
+
+
+def bt2020_to_bt709_matrix() -> np.ndarray:
+    """The (3, 3) float64 matrix taking linear BT.2020 RGB to linear BT.709 RGB (both D65):
+    NPM(BT.709)^-1 NPM(BT.2020), derived from the primaries in Python floats in a fixed order (BT.2087's
+    [[1.6605, -0.5876, -0.0728], [-0.1246, 1.1329, -0.0083], [-0.0182, -0.1006, 1.1187]] to 4 digits).  The crop
+    kernel holds these nine values as hex literals (kHdrGamut)."""
+    return np.array(_matmul3(_inverse3(_rgb_to_xyz(BT709_PRIMARIES, D65_WHITE)),
+                             _rgb_to_xyz(BT2020_PRIMARIES, D65_WHITE)), dtype=np.float64)
+
+
+def pq_eotf(e: np.ndarray) -> np.ndarray:
+    """SMPTE ST 2084 EOTF: non-linear E' in [0, 1] -> display light in cd/m², each step rounded on its own."""
+    k = HDR_CONSTANTS
+    p = np.asarray(e, dtype=np.float64) ** k["pq_inv_m2"]
+    return 10000.0 * (np.maximum(p - PQ_C1, 0.0) / (PQ_C2 - PQ_C3 * p)) ** k["pq_inv_m1"]
+
+
+def hlg_inverse_oetf(e: np.ndarray) -> np.ndarray:
+    """BT.2100 HLG inverse OETF: non-linear E' in [0, 1] -> normalised scene light E in [0, 1]."""
+    e = np.asarray(e, dtype=np.float64)
+    k = HDR_CONSTANTS
+    with np.errstate(over="ignore"):  # the exp branch of codes below 1/2 is computed, then discarded
+        hi = (np.exp((e - k["hlg_c"]) / HLG_A) + k["hlg_b"]) / 12.0
+    return np.where(e <= 0.5, (e * e) / 3.0, hi)
+
+
+def hlg_display_light(e_rgb) -> list:
+    """BT.2100 HLG at Lw = 1000 cd/m², Lb = 0, system gamma 1.2: the three non-linear components -> display light in
+    cd/m² per component, Fd = 1000 * Ys^0.2 * E."""
+    er, eg, eb = (hlg_inverse_oetf(c) for c in e_rgb)
+    ys = (0.2627 * er + 0.6780 * eg) + 0.0593 * eb
+    scale = 1000.0 * ys ** 0.2
+    return [scale * c for c in (er, eg, eb)]
+
+
+def method_a_curve(yp: np.ndarray) -> np.ndarray:
+    """BT.2446-1 Method A's tone curve Y'p -> Y'c (knots at 0.7399 and 0.9909)."""
+    yp = np.asarray(yp, dtype=np.float64)
+    mid = (-1.1510 * (yp * yp) + 2.7811 * yp) - 0.6302
+    return np.where(yp <= 0.7399, 1.077 * yp, np.where(yp < 0.9909, mid, 0.5 * yp + 0.5))
+
+
+def hdr_to_sdr(rgb, transfer: str) -> np.ndarray:
+    """The (..., 3) uint8 SDR BT.709 pixels of unclamped float64 BT.2020 R'G'B' components ``rgb`` (three arrays, the
+    H.273 inverse before rounding) under the HDR ``transfer`` ("pq" or "hlg"), each step rounded on its own:
+    clamp to [0, 1]; display light (PQ EOTF, or HLG inverse OETF + OOTF at 1000 cd/m²); L = min(Fd / 1000, 1); BT.2446-1
+    Method A tone mapping (L_HDR 1000, L_SDR 100) on L^(1/2.4); the BT.2020 inverse; clamp, ^2.4, the BT.2020 -> BT.709
+    matrix, clamp, ^(1/2.4) (``hdr_to_sdr_unit``), then min(max(rint(255 v), 0), 255).  include/fear_b200.h
+    (FearFrameYCbCrHDR) states the chain; the crop kernel restates this function."""
+    return np.stack([np.clip(np.rint(255.0 * v), 0, 255) for v in hdr_to_sdr_unit(rgb, transfer)], -1).astype(np.uint8)
+
+
+def hdr_to_sdr_unit(rgb, transfer: str) -> list:
+    """``hdr_to_sdr`` before its last step: the three BT.709 R'G'B' components in [0, 1], float64."""
+    k = HDR_CONSTANTS
+    e = [np.clip(np.asarray(c, dtype=np.float64), 0.0, 1.0) for c in rgb]
+    fd = [pq_eotf(c) for c in e] if transfer == "pq" else hlg_display_light(e)
+    lin = [np.minimum(c / 1000.0, 1.0) for c in fd]
+    r, g, b = (c ** k["inv_2_4"] for c in lin)
+    y = (0.2627 * r + 0.6780 * g) + 0.0593 * b
+    yp = np.log(1.0 + k["rho_hdr_m1"] * y) / k["ln_rho_hdr"]
+    ysdr = (k["rho_sdr"] ** method_a_curve(yp) - 1.0) / k["rho_sdr_m1"]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        f = np.where(y == 0.0, 0.0, ysdr / (1.1 * y))
+    cb = (f * (b - y)) / 1.8814
+    cr = (f * (r - y)) / 1.4746
+    ytmo = ysdr - np.maximum(0.1 * cr, 0.0)
+    r2 = ytmo + 1.4746 * cr
+    b2 = ytmo + 1.8814 * cb
+    g2 = ((ytmo - 0.2627 * r2) - 0.0593 * b2) / 0.6780
+    lin = [np.clip(c, 0.0, 1.0) ** 2.4 for c in (r2, g2, b2)]
+    m = bt2020_to_bt709_matrix()
+    out = [(m[i, 0] * lin[0] + m[i, 1] * lin[1]) + m[i, 2] * lin[2] for i in range(3)]
+    return [np.clip(c, 0.0, 1.0) ** k["inv_2_4"] for c in out]
+
+
+def check_transfer(transfer, matrix: str, bits: int, what: str = "transfer") -> None:
+    """ValueError unless ``transfer`` is None, "pq" or "hlg", and an HDR transfer comes with the BT.2020 matrix at 10
+    or 12 bits."""
+    if transfer is None:
+        return
+    if not isinstance(transfer, str) or transfer not in HDR_TRANSFERS:
+        raise ValueError(f"{what} must be None, 'pq' or 'hlg', got {transfer!r}")
+    if matrix != "bt2020":
+        raise ValueError(f"{what} {transfer!r} needs the bt2020 matrix (BT.2100), got {matrix!r}")
+    if bits == 8:
+        raise ValueError(f"{what} {transfer!r} needs 10- or 12-bit samples, not 8-bit ones")
 
 
 # (chroma_shift_x, chroma_shift_y) of the subsamplings FearFrameYCbCr describes: 4:2:0, 4:2:2, 4:4:4
@@ -180,18 +334,23 @@ CHROMA_SHIFTS = ((1, 1), (1, 0), (0, 0))
 
 
 def yuv_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601", full_range: bool = False,
-               bits: int = 8, shift: int = 0, chroma_shift=(1, 1)) -> np.ndarray:
+               bits: int = 8, shift: int = 0, chroma_shift=(1, 1), transfer: Optional[str] = None) -> np.ndarray:
     """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for a YUV frame: luma ``y`` (H, W), chroma ``u`` (Cb) and
     ``v`` (Cr) of (H >> sy, W >> sx) raw samples (uint8, or uint16 at 10 / 12 bits, code = (sample >> shift) &
     (2^bits - 1)), where ``chroma_shift`` = (sx, sy) is (1, 1) for 4:2:0, (1, 0) for 4:2:2 and (0, 0) for 4:4:4, and
     pixel (r, c) takes chroma sample (r >> sy, c >> sx).  A numpy restatement of the crop kernel's conversion
     (include/fear_b200.h, FearFrameYUV and FearFrameYCbCr): for (bt601, limited, 8) cv2.cvtColor's fixed point, bit for
     bit; otherwise the ITU-T H.273 inverse in float64 with the same constants, derived in the same order, each
-    operation rounded on its own, then rint (half to even) and saturation to [0, 255]."""
+    operation rounded on its own, then rint (half to even) and saturation to [0, 255].
+
+    ``transfer`` "pq" or "hlg" (BT.2020 at 10 or 12 bits only) reads the frame as HDR video: the unclamped R'G'B' of
+    the H.273 inverse go through ``hdr_to_sdr`` instead of being rounded, giving the SDR BT.709 frame of BT.2446-1
+    Method A tone mapping (include/fear_b200.h, FearFrameYCbCrHDR).  ``None`` is the matrix alone."""
     if matrix not in YUV_MATRICES:
         raise ValueError(f"matrix must be one of {sorted(YUV_MATRICES)}, got {matrix!r}")
     if bits not in (8, 10, 12) or not (0 <= shift <= 16 - bits) or (bits == 8 and shift):
         raise ValueError(f"bits must be 8, 10 or 12 with 0 <= shift <= 16 - bits (0 at 8 bits), got {bits}, {shift}")
+    check_transfer(transfer, matrix, bits)
     sx, sy = chroma_shift
     if (sx, sy) not in CHROMA_SHIFTS:
         raise ValueError(f"chroma_shift must be one of {CHROMA_SHIFTS} (4:2:0, 4:2:2, 4:4:4), got {chroma_shift!r}")
@@ -207,6 +366,15 @@ def yuv_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601
         U, V = U - 128, V - 128
         rgb = [(yy + 1673527 * V) >> 20, (yy - 852492 * V - 409993 * U) >> 20, (yy + 2116026 * U) >> 20]
         return np.clip(np.stack(rgb, -1), 0, 255).astype(np.uint8)
+    rgb = h273_rgb(Y, U, V, matrix, full_range, bits)
+    if transfer is not None:
+        return hdr_to_sdr(rgb, transfer)
+    return np.stack([np.clip(np.rint(255.0 * c), 0, 255) for c in rgb], -1).astype(np.uint8)
+
+
+def h273_rgb(Y: np.ndarray, U: np.ndarray, V: np.ndarray, matrix: str, full_range: bool, bits: int) -> list:
+    """The unclamped float64 R', G', B' of the ITU-T H.273 inverse of integer codes (Y, U, V of one shape), before the
+    rounding to 8 bits: the conversion of ``yuv_to_rgb`` for every format but (bt601, limited, 8)."""
     _, kr, kb = YUV_MATRICES[matrix]
     m = float(1 << (bits - 8))
     if full_range:
@@ -217,11 +385,10 @@ def yuv_to_rgb(y: np.ndarray, u: np.ndarray, v: np.ndarray, matrix: str = "bt601
     kg = (1.0 - kr) - kb
     cr, cb = 2.0 * (1.0 - kr), 2.0 * (1.0 - kb)
     gb, gr = 2.0 * kb * (1.0 - kb) / kg, 2.0 * kr * (1.0 - kr) / kg
-    yn = (Y.astype(np.float64) - y0) * ys
-    pb = (U.astype(np.float64) - c0) * cs
-    pr = (V.astype(np.float64) - c0) * cs
-    rgb = [yn + cr * pr, (yn - gb * pb) - gr * pr, yn + cb * pb]
-    return np.stack([np.clip(np.rint(255.0 * c), 0, 255) for c in rgb], -1).astype(np.uint8)
+    yn = (np.asarray(Y).astype(np.float64) - y0) * ys
+    pb = (np.asarray(U).astype(np.float64) - c0) * cs
+    pr = (np.asarray(V).astype(np.float64) - c0) * cs
+    return [yn + cr * pr, (yn - gb * pb) - gr * pr, yn + cb * pb]
 
 
 def v210_row_bytes(width: int) -> int:

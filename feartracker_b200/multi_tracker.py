@@ -30,7 +30,9 @@ tensors' views point at the tensors.  YUV420Frames go into a second fixed table 
 format), read by the *_yuv entry points; a call with any 4:2:2 or 4:4:4 frame puts all its frames into a third, of
 FearFrameYCbCr records (the same plus the chroma subsampling), read by the *_ycbcr entry points; a call with any
 V210Frame puts all its frames into a fourth, of FearFrameYCbCrV210 records (a FearFrameYCbCr or a v210 surface), read
-by the *_ycbcr_v210 entry points.  BayerFrames go into a fifth, of FearFrameBayer records, read by the *_bayer entry
+by the *_ycbcr_v210 entry points; a call with any HDR frame (``transfer="pq"`` or ``"hlg"``) puts all its frames into
+a sixth, of FearFrameYCbCrHDR records (a FearFrameYCbCrV210 and its transfer), read by the *_ycbcr_hdr entry points,
+which tone-map HDR taps to SDR inside the crop.  BayerFrames go into a fifth, of FearFrameBayer records, read by the *_bayer entry
 points; they cannot share a call with other kinds of frames.  The host then reads back the boxes and scores.  The
 launch count of a step depends neither on N nor on the kind of frames.
 """
@@ -52,10 +54,11 @@ ENTRY_POINTS = {
     "ycbcr": ("fear_frame_sums_ycbcr_u8", "fear_crop_targets_ycbcr_u8", "fear_advance_targets_ycbcr"),
     "ycbcr_v210": ("fear_frame_sums_ycbcr_v210_u8", "fear_crop_targets_ycbcr_v210_u8",
                    "fear_advance_targets_ycbcr_v210"),
+    "ycbcr_hdr": ("fear_frame_sums_ycbcr_hdr_u8", "fear_crop_targets_ycbcr_hdr_u8", "fear_advance_targets_ycbcr_hdr"),
     "bayer": ("fear_frame_sums_bayer_u8", "fear_crop_targets_bayer_u8", "fear_advance_targets_bayer"),
 }
 TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE,
-                "ycbcr_v210": _lib.YCBCR_V210_DTYPE, "bayer": _lib.BAYER_DTYPE}
+                "ycbcr_v210": _lib.YCBCR_V210_DTYPE, "ycbcr_hdr": _lib.YCBCR_HDR_DTYPE, "bayer": _lib.BAYER_DTYPE}
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -74,9 +77,9 @@ class _YUVFrame:
     _SIZES = "H and W even and >= 2"  # the luma sizes the subsampling allows, for error messages
 
     def __init__(self, y: torch.Tensor, u: torch.Tensor, v: torch.Tensor, *, matrix: str = "bt601",
-                 full_range: bool = False, bits: int = 8, msb: bool = False) -> None:
+                 full_range: bool = False, bits: int = 8, msb: bool = False, transfer: Optional[str] = None) -> None:
         cls = type(self).__name__
-        self._check_format(matrix, full_range, bits, msb)
+        self._check_format(matrix, full_range, bits, msb, transfer)
         dtype = self._dtype(bits)
         for name, p in (("y", y), ("u", u), ("v", v)):
             if not isinstance(p, torch.Tensor) or p.dtype != dtype or p.ndim != 2:
@@ -98,15 +101,17 @@ class _YUVFrame:
         self.shape = (h, w, 3)
         self.matrix, self.full_range, self.bits = matrix, bool(full_range), int(bits)
         self.shift = 16 - self.bits if msb else 0
+        self.transfer = transfer
 
     @classmethod
-    def _check_format(cls, matrix, full_range, bits, msb) -> None:
+    def _check_format(cls, matrix, full_range, bits, msb, transfer=None) -> None:
         if matrix not in image_ops.YUV_MATRICES:
             raise ValueError(f"{cls.__name__} matrix must be one of {sorted(image_ops.YUV_MATRICES)}, got {matrix!r}")
         if isinstance(bits, bool) or bits not in (8, 10, 12):
             raise ValueError(f"{cls.__name__} bits must be 8, 10 or 12, got {bits!r}")
         if bits == 8 and msb:
             raise ValueError(f"{cls.__name__} msb applies to 10- and 12-bit samples, not 8-bit ones")
+        image_ops.check_transfer(transfer, matrix, bits, f"{cls.__name__} transfer")
 
     @staticmethod
     def _dtype(bits: int) -> torch.dtype:
@@ -140,6 +145,11 @@ class _YUVFrame:
         """The FearFrameYCbCrV210 record of a planar frame: ``ycbcr_record``, then v210 = 0 and the reserved 0."""
         return self.ycbcr_record() + (0, 0)
 
+    def hdr_record(self) -> tuple:
+        """The FearFrameYCbCrHDR record: ``ycbcr_v210_record``, then the H.273 transfer code (0 without a transfer,
+        16 for "pq", 18 for "hlg") and the reserved 0."""
+        return self.ycbcr_v210_record() + (image_ops.HDR_TRANSFERS.get(self.transfer, 0), 0)
+
 
 class YUV420Frame(_YUVFrame):
     """A YUV 4:2:0 frame as a video decoder writes it: a luma plane ``y`` (H, W) and chroma planes ``u`` (Cb) and
@@ -157,9 +167,13 @@ class YUV420Frame(_YUVFrame):
                      the low bits (yuv420p10le / yuv420p12le)
     The default (bt601, limited, 8 bits) is converted exactly as ``cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_NV12 /
     COLOR_YUV2RGB_I420)`` converts it; every other format by the ITU-T H.273 inverse in float64 (include/fear_b200.h,
-    FearFrameYUV).  ``image_ops.yuv420_to_rgb`` restates both in numpy: it gives the RGB frame the tracker sees.  Only
-    the matrix is applied: transfer functions (PQ, HLG) are not.  NV21 / YV12 are ``YUV420Frame(y, u, v)`` with the
-    planes in the right order.
+    FearFrameYUV).  ``image_ops.yuv420_to_rgb`` restates both in numpy: it gives the RGB frame the tracker sees.
+    NV21 / YV12 are ``YUV420Frame(y, u, v)`` with the planes in the right order.
+
+        transfer     None: the matrix only (SDR); "pq" or "hlg": HDR video (BT.2100 PQ as Android phones and HDR10
+                     streams record it, HLG as iPhones and UHD broadcast do), BT.2020 at 10 / 12 bits only, tone-mapped
+                     to SDR BT.709 inside the crop by ITU-R BT.2446-1 Method A at a 1000 cd/m² peak
+                     (``image_ops.yuv_to_rgb(..., transfer=...)``, include/fear_b200.h FearFrameYCbCrHDR)
 
         YUV420Frame.nv12(t)    t (3H/2, W): H luma rows, then H/2 rows of interleaved (U, V) pairs; the rows may be
                                pitched (t = surface[:, :W]), as NVDEC and cv2 lay out NV12; at 10 / 12 bits a uint16
@@ -170,24 +184,28 @@ class YUV420Frame(_YUVFrame):
 
     ``shape`` is (H, W, 3), the shape of the RGB frame it stands for.  The constructors raise ValueError on a malformed
     frame or format; they do not look at the device (the tracker checks that).  YUV422Frame and YUV444Frame take the
-    same colour formats."""
+    same colour formats and transfers."""
 
     @classmethod
-    def nv12(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV420Frame":
-        cls._check_format(matrix, full_range, bits, False)
+    def nv12(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8,
+             transfer: Optional[str] = None) -> "YUV420Frame":
+        cls._check_format(matrix, full_range, bits, False, transfer)
         h = cls._luma_rows(t, "nv12", bits)
         uv = t[h:]
-        return cls(t[:h], uv[:, 0::2], uv[:, 1::2], matrix=matrix, full_range=full_range, bits=bits, msb=bits > 8)
+        return cls(t[:h], uv[:, 0::2], uv[:, 1::2], matrix=matrix, full_range=full_range, bits=bits, msb=bits > 8,
+                   transfer=transfer)
 
     @classmethod
-    def i420(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV420Frame":
-        cls._check_format(matrix, full_range, bits, False)
+    def i420(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8,
+             transfer: Optional[str] = None) -> "YUV420Frame":
+        cls._check_format(matrix, full_range, bits, False, transfer)
         h, w = cls._luma_rows(t, "i420", bits), t.shape[1]
         if not t.is_contiguous():
             raise ValueError(f"YUV420Frame.i420 takes a contiguous tensor, got strides {t.stride()}")
         flat, luma, quarter = t.reshape(-1), h * w, h * w // 4
         return cls(flat[:luma].view(h, w), flat[luma:luma + quarter].view(h // 2, w // 2),
-                   flat[luma + quarter:].view(h // 2, w // 2), matrix=matrix, full_range=full_range, bits=bits)
+                   flat[luma + quarter:].view(h // 2, w // 2), matrix=matrix, full_range=full_range, bits=bits,
+                   transfer=transfer)
 
     @classmethod
     def _luma_rows(cls, t, layout: str, bits: int = 8) -> int:
@@ -231,43 +249,49 @@ class YUV422Frame(_YUVFrame):
     _SIZES = "W even and >= 2, H >= 1"
 
     @classmethod
-    def _packed(cls, t, layout: str, order: tuple, matrix, full_range, bits) -> "YUV422Frame":
-        cls._check_format(matrix, full_range, bits, False)
+    def _packed(cls, t, layout: str, order: tuple, matrix, full_range, bits, transfer) -> "YUV422Frame":
+        cls._check_format(matrix, full_range, bits, False, transfer)
         cls._surface(t, layout, bits, 1, 4, "(H, 2W) tensor with W even")
         y0, u0, v0 = order  # sample offsets of Y0, U and V in each 4-sample group
         return cls(t[:, y0::2], t[:, u0::4], t[:, v0::4], matrix=matrix, full_range=full_range, bits=bits,
-                   msb=bits > 8)
+                   msb=bits > 8, transfer=transfer)
 
     @classmethod
-    def yuyv(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
-        return cls._packed(t, "yuyv", (0, 1, 3), matrix, full_range, bits)
+    def yuyv(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8,
+             transfer: Optional[str] = None) -> "YUV422Frame":
+        return cls._packed(t, "yuyv", (0, 1, 3), matrix, full_range, bits, transfer)
 
     @classmethod
-    def uyvy(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
-        return cls._packed(t, "uyvy", (1, 0, 2), matrix, full_range, bits)
+    def uyvy(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8,
+             transfer: Optional[str] = None) -> "YUV422Frame":
+        return cls._packed(t, "uyvy", (1, 0, 2), matrix, full_range, bits, transfer)
 
     @classmethod
-    def yvyu(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
-        return cls._packed(t, "yvyu", (0, 3, 1), matrix, full_range, bits)
+    def yvyu(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8,
+             transfer: Optional[str] = None) -> "YUV422Frame":
+        return cls._packed(t, "yvyu", (0, 3, 1), matrix, full_range, bits, transfer)
 
     @classmethod
-    def nv16(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
-        cls._check_format(matrix, full_range, bits, False)
+    def nv16(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8,
+             transfer: Optional[str] = None) -> "YUV422Frame":
+        cls._check_format(matrix, full_range, bits, False, transfer)
         cls._surface(t, "nv16", bits, 2, 2, "(2H, W) tensor with W even")
         h = t.shape[0] // 2
         uv = t[h:]
-        return cls(t[:h], uv[:, 0::2], uv[:, 1::2], matrix=matrix, full_range=full_range, bits=bits, msb=bits > 8)
+        return cls(t[:h], uv[:, 0::2], uv[:, 1::2], matrix=matrix, full_range=full_range, bits=bits, msb=bits > 8,
+                   transfer=transfer)
 
     @classmethod
-    def i422(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8) -> "YUV422Frame":
-        cls._check_format(matrix, full_range, bits, False)
+    def i422(cls, t: torch.Tensor, *, matrix: str = "bt601", full_range: bool = False, bits: int = 8,
+             transfer: Optional[str] = None) -> "YUV422Frame":
+        cls._check_format(matrix, full_range, bits, False, transfer)
         cls._surface(t, "i422", bits, 2, 2, "(2H, W) tensor with W even")
         if not t.is_contiguous():
             raise ValueError(f"YUV422Frame.i422 takes a contiguous tensor, got strides {t.stride()}")
         h, w = t.shape[0] // 2, t.shape[1]
         flat, luma, half = t.reshape(-1), h * w, h * w // 2
         return cls(flat[:luma].view(h, w), flat[luma:luma + half].view(h, w // 2), flat[luma + half:].view(h, w // 2),
-                   matrix=matrix, full_range=full_range, bits=bits)
+                   matrix=matrix, full_range=full_range, bits=bits, transfer=transfer)
 
 
 class YUV444Frame(_YUVFrame):
@@ -286,11 +310,12 @@ class YUV444Frame(_YUVFrame):
 
     @classmethod
     def i444(cls, t: torch.Tensor, *, msb: bool = False, matrix: str = "bt601", full_range: bool = False,
-             bits: int = 8) -> "YUV444Frame":
-        cls._check_format(matrix, full_range, bits, msb)
+             bits: int = 8, transfer: Optional[str] = None) -> "YUV444Frame":
+        cls._check_format(matrix, full_range, bits, msb, transfer)
         cls._surface(t, "i444", bits, 3, 1, "(3H, W) tensor")
         h = t.shape[0] // 3
-        return cls(t[:h], t[h:2 * h], t[2 * h:], matrix=matrix, full_range=full_range, bits=bits, msb=msb)
+        return cls(t[:h], t[h:2 * h], t[2 * h:], matrix=matrix, full_range=full_range, bits=bits, msb=msb,
+                   transfer=transfer)
 
 
 class V210Frame:
@@ -299,7 +324,9 @@ class V210Frame:
     the capture buffer as bytes: a CUDA uint8 (H, row bytes) tensor whose rows are contiguous, any row pitch (a view
     ``surface[:, :n]`` of a pitched surface is fine); ``width`` is the picture width W (even).  A row needs
     ``16 * ceil(W / 6)`` bytes; capture cards pitch rows to ``128 * ceil(W / 48)``.  The buffer address and the row pitch
-    must be multiples of 4 bytes.  ``matrix`` and ``full_range`` are those of YUV420Frame; the depth is 10 bits.
+    must be multiples of 4 bytes.  ``matrix``, ``full_range`` and ``transfer`` are those of YUV420Frame; the depth is 10
+    bits (``transfer`` "pq" or "hlg" with ``matrix="bt2020"`` reads 10-bit HLG or PQ from SDI: the tracker sees
+    ``image_ops.yuv_to_rgb(..., bits=10, chroma_shift=(1, 0), transfer=...)`` of the unpacked planes).
 
     FEARMultiTracker and FEARTracker read the words where they are and unpack and convert every pixel they read, so no
     planes and no RGB copy are made: the RGB frame the tracker sees is ``image_ops.yuv_to_rgb(*image_ops.v210_unpack(
@@ -308,9 +335,11 @@ class V210Frame:
     CHROMA_SHIFT = (1, 0)
     bits = 10
 
-    def __init__(self, t: torch.Tensor, width: int, *, matrix: str = "bt601", full_range: bool = False) -> None:
+    def __init__(self, t: torch.Tensor, width: int, *, matrix: str = "bt601", full_range: bool = False,
+                 transfer: Optional[str] = None) -> None:
         if matrix not in image_ops.YUV_MATRICES:
             raise ValueError(f"V210Frame matrix must be one of {sorted(image_ops.YUV_MATRICES)}, got {matrix!r}")
+        image_ops.check_transfer(transfer, matrix, self.bits, "V210Frame transfer")
         if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.ndim != 2 or t.device.type != "cuda":
             what = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
             raise ValueError(f"V210Frame takes a 2-D CUDA uint8 (H, row bytes) tensor, got {what}")
@@ -331,6 +360,7 @@ class V210Frame:
         self.t, self.width, self.pitch = t, int(width), int(pitch)
         self.shape = (h, self.width, 3)
         self.matrix, self.full_range = matrix, bool(full_range)
+        self.transfer = transfer
 
     def ycbcr_v210_record(self) -> tuple:
         """The FearFrameYCbCrV210 record (y, u, v, y_row_stride, y_pixel_stride, uv_row_stride, uv_pixel_stride, H, W,
@@ -338,6 +368,11 @@ class V210Frame:
         row pitch, the size and format, v210 = 1; the fields a v210 entry does not read are 0."""
         return (self.t.data_ptr(), 0, 0, self.pitch, 0, 0, 0, *self.shape[:2], image_ops.YUV_MATRICES[self.matrix][0],
                 int(self.full_range), self.bits, 0, *self.CHROMA_SHIFT, 1, 0)
+
+    def hdr_record(self) -> tuple:
+        """The FearFrameYCbCrHDR record: ``ycbcr_v210_record``, then the H.273 transfer code (0, 16 for "pq", 18 for
+        "hlg") and the reserved 0."""
+        return self.ycbcr_v210_record() + (image_ops.HDR_TRANSFERS.get(self.transfer, 0), 0)
 
 
 class BayerFrame:
@@ -470,7 +505,7 @@ def check_device_frame(i: int, f, kind: str, device) -> None:
 def write_records(table: np.ndarray, frames, name: str) -> None:
     """Write the records of device frames into rows of ``table`` (a numpy view of ``TABLE_DTYPES[name]``):
     FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr",
-    FearFrameYCbCrV210 for "ycbcr_v210", FearFrameBayer for "bayer"."""
+    FearFrameYCbCrV210 for "ycbcr_v210", FearFrameYCbCrHDR for "ycbcr_hdr", FearFrameBayer for "bayer"."""
     for i, f in enumerate(frames):
         if name == "yuv":
             table[i] = f.yuv_record()
@@ -478,6 +513,8 @@ def write_records(table: np.ndarray, frames, name: str) -> None:
             table[i] = f.ycbcr_record()
         elif name == "ycbcr_v210":
             table[i] = f.ycbcr_v210_record()
+        elif name == "ycbcr_hdr":
+            table[i] = f.hdr_record()
         elif name == "bayer":
             table[i] = f.bayer_record()
         else:
@@ -708,13 +745,14 @@ class FEARMultiTracker:
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
             frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, ycbcr_pin=None,
-            ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, bayer_pin=None, bayer=None, sums_pin=None, sums=None)
+            ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, ycbcr_hdr_pin=None, ycbcr_hdr=None, bayer_pin=None, bayer=None, sums_pin=None, sums=None)
         return b
 
     def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
         """Write the frame table of ``frames`` into the fixed device table the kernels read, and return its name:
-        "yuv" (FearFrameYUV records) when every frame is a YUV420Frame, "ycbcr_v210" (FearFrameYCbCrV210 records) for
-        YUV frames of which any is a V210Frame, "ycbcr" (FearFrameYCbCr records) for other YUV frames of which any is
+        "yuv" (FearFrameYUV records) when every frame is a YUV420Frame, "ycbcr_hdr" (FearFrameYCbCrHDR records) for YUV
+        frames of which any has a transfer (PQ, HLG), else "ycbcr_v210" (FearFrameYCbCrV210 records) for YUV frames of
+        which any is a V210Frame, "ycbcr" (FearFrameYCbCr records) for other YUV frames of which any is
         4:2:2 or 4:4:4, "bayer" (FearFrameBayer records) for BayerFrames, "views" (FearFrameView records) otherwise.
         Numpy frames are packed into the pinned staging buffer first and sent with one host-to-device copy (the packed
         layout is recomputed only when their shapes change); CUDA tensors, YUV planes, v210 surfaces and Bayer mosaics
@@ -725,6 +763,8 @@ class FEARMultiTracker:
             name = "yuv" if all(isinstance(f, YUV420Frame) for f in frames) else "ycbcr"
             if any(isinstance(f, V210Frame) for f in frames):
                 name = "ycbcr_v210"
+            if any(f.transfer is not None for f in frames):
+                name = "ycbcr_hdr"
         elif kind == "bayer":
             name = "bayer"
         dtype = TABLE_DTYPES[name]
@@ -777,7 +817,7 @@ class FEARMultiTracker:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
         keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records, YCbCr
-        records of any subsampling, YCbCr / v210 records or Bayer records) and
+        records of any subsampling, YCbCr / v210 records, HDR records or Bayer records) and
         its buffer, and the net's generation.  ``cuda_graph=False`` in the tracking config keeps eager launches."""
         key = (n, num_frames, table, self._buf[table].data_ptr())
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):

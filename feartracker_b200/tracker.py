@@ -25,9 +25,9 @@ from .box_coder import FEARBoxCoder, TrackerDecodeResult
 from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY
 
 
-# byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrV210; a
+# byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrHDR; a
 # FearFrameBayer is 40 bytes), a FearTarget, then five float64 inputs of fear_decode_smooth
-_TARGET_OFFSET = 96
+_TARGET_OFFSET = 104
 _SMOOTH_OFFSET = _TARGET_OFFSET + 64
 _DEVICE_INPUT_BYTES = _SMOOTH_OFFSET + 5 * 8
 
@@ -285,9 +285,9 @@ class FEARTracker(Tracker):
     def _device_frame_state(self) -> dict:
         """Buffers of the device-frame step, separate from the gpu_crop path's.  ``inputs`` (pinned) and ``dev_in``
         share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView, a
-        FearFrameYCbCr, a FearFrameYCbCrV210 or a FearFrameBayer) at byte 0, the FearTarget at byte 96,
-        fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr as float64 at byte 160; then, on the
-        device only, the 16 x 16 window."""
+        FearFrameYCbCr, a FearFrameYCbCrV210, a FearFrameYCbCrHDR or a FearFrameBayer) at byte 0, the FearTarget at
+        byte 104, fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr as float64 at byte 168;
+        then, on the device only, the 16 x 16 window."""
         from . import _lib
 
         dev = self._device()
@@ -315,11 +315,13 @@ class FEARTracker(Tracker):
     def _stage_device_inputs(self, st: dict, image, kind: str, bbox, pad, prev_size=None) -> str:
         """Write the frame's record, the target (frame 0, ``bbox``, padding colour ``pad``) and, given ``prev_size``,
         the smooth scalars into the pinned inputs and send them with one host-to-device copy.  Returns the table name:
-        "views" for a tensor, "ycbcr_v210" for a V210Frame, "ycbcr" for every other YUV frame, "bayer" for a
-        BayerFrame."""
+        "views" for a tensor, "ycbcr_hdr" for a YUV frame with a transfer (PQ, HLG), "ycbcr_v210" for another
+        V210Frame, "ycbcr" for every other YUV frame, "bayer" for a BayerFrame."""
         table = "bayer" if kind == "bayer" else "views"
         if kind == "yuv":
             table = "ycbcr_v210" if isinstance(image, multi_tracker.V210Frame) else "ycbcr"
+            if image.transfer is not None:
+                table = "ycbcr_hdr"
         raw, dtype = st["inputs"].numpy(), multi_tracker.TABLE_DTYPES[table]
         multi_tracker.write_records(raw[:dtype.itemsize].view(dtype), [image], table)
         target = raw[_TARGET_OFFSET:_SMOOTH_OFFSET].view(np.int32)

@@ -39,6 +39,9 @@
  *   fear_crop_targets_ycbcr_v210_u8 / fear_advance_targets_ycbcr_v210 / fear_frame_sums_ycbcr_v210_u8   the same three
  *                         on FearFrameYCbCrV210 tables: FearFrameYCbCr entries and v210 surfaces (10-bit 4:2:2 packed
  *                         three codes to a 32-bit word, as SDI capture cards deliver it), unpacked inside the crop
+ *   fear_crop_targets_ycbcr_hdr_u8 / fear_advance_targets_ycbcr_hdr / fear_frame_sums_ycbcr_hdr_u8   the same three on
+ *                         FearFrameYCbCrHDR tables: those entries with a transfer function, PQ and HLG video
+ *                         tone-mapped to SDR BT.709 (BT.2446-1 Method A) inside the crop
  *   fear_crop_targets_bayer_u8 / fear_advance_targets_bayer / fear_frame_sums_bayer_u8   the same three on raw Bayer
  *                         mosaics located by FearFrameBayer (8 to 16 bits, MIPI RAW10 / RAW12), demosaiced inside the
  *                         crop as cv2.cvtColor(COLOR_Bayer*2RGB) demosaics them
@@ -200,6 +203,54 @@ typedef struct FearFrameYCbCrV210 {        /* 96 bytes                          
   int32_t v210;                            /* 0: a FearFrameYCbCr entry; 1: a v210 surface                      */
   int32_t reserved;                        /* not read                                                          */
 } FearFrameYCbCrV210;
+/* A FearFrameYCbCrV210 entry with its transfer characteristics, so HDR video (PQ and HLG, as phones, UHD broadcast and
+ * NVDEC's P010 / P210 surfaces deliver it) is tone-mapped to SDR inside the crop: 104 bytes, the fields of
+ * FearFrameYCbCrV210 followed by `transfer` and a reserved int32.  `transfer` holds the ITU-T H.273
+ * TransferCharacteristics code (ffmpeg's color_trc, NVDEC's transfer_characteristics):
+ *   0                     the matrix only: the entry is read exactly as the *_ycbcr_v210 entry points read its
+ *                         FearFrameYCbCrV210 fields (a planar entry or a v210 surface, SDR)
+ *   FEAR_TRC_PQ (16)      SMPTE ST 2084 / BT.2100 PQ
+ *   FEAR_TRC_HLG (18)     BT.2100 HLG
+ * A PQ or HLG entry reads its codes as the FearFrameYCbCrV210 entry does, takes the unclamped R'G'B' of FearFrameYUV's
+ * H.273 inverse (before the rounding to 8 bits), and continues in float64, each step rounded on its own (no FMA):
+ *   1. E' = clamp(R'G'B', 0, 1)
+ *   2. display light Fd in cd/m2 per component, BT.2020 primaries:
+ *        PQ:  p = E'^(1/m2);  Fd = 10000 * (max(p - c1, 0) / (c2 - c3 * p))^(1/m1)   (m1 = 2610/16384,
+ *             m2 = 2523/4096 * 128, c1 = 3424/4096, c2 = 2413/4096 * 32, c3 = 2392/4096 * 32)
+ *        HLG: E = E'^2 / 3 for E' <= 1/2, else (exp((E' - c) / a) + b) / 12  (a = 0.17883277, b = 1 - 4a,
+ *             c = 0.5 - a ln(4a));  Ys = 0.2627 E_R + 0.6780 E_G + 0.0593 E_B;  Fd = 1000 * Ys^0.2 * E  (Lw 1000,
+ *             Lb 0, system gamma 1.2)
+ *   3. L = min(Fd / 1000, 1): a fixed 1000 cd/m2 peak, PQ light above it clips
+ *   4. ITU-R BT.2446-1 Method A (L_HDR 1000, L_SDR 100): R'G'B' = L^(1/2.4); Y' = 0.2627 R' + 0.6780 G' + 0.0593 B';
+ *      Y'p = ln(1 + (rho_HDR - 1) Y') / ln(rho_HDR), rho_HDR = 1 + 32 (1000/10000)^(1/2.4);
+ *      Y'c = 1.077 Y'p (Y'p <= 0.7399), -1.1510 Y'p^2 + 2.7811 Y'p - 0.6302 (Y'p < 0.9909), 0.5 Y'p + 0.5 (otherwise);
+ *      Y'sdr = (rho_SDR^Y'c - 1) / (rho_SDR - 1), rho_SDR = 1 + 32 (100/10000)^(1/2.4);  f = Y'sdr / (1.1 Y') (0 when
+ *      Y' = 0);  Cb = f (B' - Y') / 1.8814;  Cr = f (R' - Y') / 1.4746;  Y'tmo = Y'sdr - max(0.1 Cr, 0)
+ *   5. R' = Y'tmo + 1.4746 Cr, B' = Y'tmo + 1.8814 Cb, G' = (Y'tmo - 0.2627 R' - 0.0593 B') / 0.6780; clamp to [0, 1],
+ *      ^2.4; the linear BT.2020 -> BT.709 matrix (from the primaries and D65; BT.2087's to 4 digits); clamp to [0, 1],
+ *      ^(1/2.4); out = min(max(rint(255 v), 0), 255)
+ * evaluated left to right, exp, log and pow from the CUDA double library (within 2 ulp; every step is continuous but
+ * for a 5.5e-4 step of Method A's 4-digit coefficients at 0.7399, so a difference from another libm can in practice
+ * only move an output across a rounding boundary).  The derived constants
+ * (1/m1, 1/m2, b, c, 1/2.4, rho_HDR - 1, ln rho_HDR, rho_SDR, rho_SDR - 1 and the matrix) are folded to the float64
+ * values feartracker_b200.image_ops.HDR_CONSTANTS and bt2020_to_bt709_matrix() name, which restate the chain in numpy.
+ * There is no peak or metadata parameter (HDR10 MaxCLL, HDR10+ and Dolby Vision are not read).
+ * An entry is treated like a frame index outside [0, F) when FearFrameYCbCrV210 refuses it, when transfer is not 0,
+ * 16 or 18, or when transfer is 16 or 18 and the matrix is not FEAR_YUV_BT2020 or bits is 8. */
+#define FEAR_TRC_PQ 16
+#define FEAR_TRC_HLG 18
+typedef struct FearFrameYCbCrHDR {         /* 104 bytes                                                         */
+  const void *y, *u, *v;                   /* as in FearFrameYCbCrV210                                          */
+  int64_t y_row_stride, y_pixel_stride;
+  int64_t uv_row_stride, uv_pixel_stride;
+  int32_t H, W;
+  int32_t matrix, full_range, bits, shift;
+  int32_t chroma_shift_x, chroma_shift_y;
+  int32_t v210;                            /* 0: planar; 1: a v210 surface                                      */
+  int32_t reserved;                        /* not read                                                          */
+  int32_t transfer;                        /* H.273 TransferCharacteristics: 0, FEAR_TRC_PQ or FEAR_TRC_HLG      */
+  int32_t reserved_hdr;                    /* not read                                                          */
+} FearFrameYCbCrHDR;
 /* A raw Bayer mosaic (machine-vision cameras' PFNC BayerRG8 / BayerGR12 ..., CSI-2 sensors' SRGGB10P / SRGGB12P):
  * 40 bytes.  `pattern` names the colours of the 2 x 2 block at pixel (0, 0), row by row (OpenCV 4.x's sensor-order
  * COLOR_Bayer{RGGB,GRBG,GBRG,BGGR}2RGB).  `packing` is how a row holds its samples:
@@ -395,6 +446,17 @@ int fear_crop_targets_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, Fe
 int fear_advance_targets_ycbcr_v210(const FearBox* d_boxes, const FearFrameYCbCrV210* d_views, int F,
                                     FearTarget* d_targets, int N, int instance_size, void* stream);
 int fear_frame_sums_ycbcr_v210_u8(const FearFrameYCbCrV210* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* The same three on FearFrameYCbCrHDR tables, so PQ and HLG video is tone-mapped to SDR BT.709 inside the crop, each tap
+ * converted by the chain FearFrameYCbCrHDR states, alongside SDR YUV frames and v210 surfaces.  A transfer == 0 entry
+ * gives exactly what the *_ycbcr_v210 entry points give on its FearFrameYCbCrV210 fields.  Same semantics and
+ * FEAR_EINVAL rules as the *_ycbcr_v210 entry points; an entry the kernels cannot read (see FearFrameYCbCrHDR) gets a
+ * padding-colour crop, keeps its box and sums to 0. */
+int fear_crop_targets_ycbcr_hdr_u8(const FearFrameYCbCrHDR* d_views, int F, FearTarget* d_targets, int N,
+                                   double offset, int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_ycbcr_hdr(const FearBox* d_boxes, const FearFrameYCbCrHDR* d_views, int F,
+                                   FearTarget* d_targets, int N, int instance_size, void* stream);
+int fear_frame_sums_ycbcr_hdr_u8(const FearFrameYCbCrHDR* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* The same three on FearFrameBayer tables: raw Bayer mosaics read where they are, each tap demosaiced (and above 8 bits
  * mapped to 8 bits) inside the crop, so the kernels see cv2.cvtColor(raw, COLOR_Bayer{pattern}2RGB).  Same semantics
