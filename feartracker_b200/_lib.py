@@ -100,6 +100,14 @@ _SIGNATURES = {
     "fear_frame_sums_bayer_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_decode_smooth": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fear_head_sized": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                c_void_p]),
+    "fear_track_sized": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fear_track_sized_u8": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]),
+    "fear_forward_sized": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fear_decode_sized": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "fear_decode_smooth_sized": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fear_corr_concat_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "fear_corr_concat_workspace_bytes": (c_size_t, [c_int, c_int]),
     "fear_corr_concat_ws_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),

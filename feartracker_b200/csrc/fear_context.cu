@@ -138,6 +138,8 @@ struct FearContext {
   float *zt = nullptr, *mapB = nullptr, *mapC = nullptr;
   float* zu = nullptr;  // dynamic-template (`update`) features of the cls branch, same layout as zt
 
+  int head_side = kScore;  // score-map side s of the last head run (fear_debug_head_tensor)
+
   int64_t launches = 0;
   int64_t generation = 0;  // bumped whenever workspace pointers or options change (captured CUDA graphs are stale)
   bool profiling = false;
@@ -350,21 +352,21 @@ static int launch_transpose(FearContext* c, cudaStream_t s, const float* in, int
 }
 
 // cat[b, p, 256 + k] = sum_c zt[b, k, c] * cat[b, p, c]    (MobileCorrelation matmul, blocks.py:123)
-// `groups` consecutive [B][256][320] buffers starting at cat share the templates (head: cls + reg branch).
+// `groups` consecutive [B][P][320] buffers starting at cat share the templates (head: cls + reg branch).
 static int launch_corr(FearContext* c, const Options& opt, cudaStream_t s, const float* zt, int Bz, float* cat, int B,
-                       int groups) {
+                       int groups, int P = kScorePix) {
   const int corr_impl = effective(opt.corr);
   if (corr_impl == IMPL_TC) {
     LaunchScope scope(c, ST_CORR, s);
-    int r = tc::launch_corr(s, zt, Bz, cat, B, groups);
+    int r = tc::launch_corr(s, zt, Bz, cat, B, groups, P);
     if (r) return set_err(r, "wgmma corr launch failed (%d)", r);
     return check_launch("tc::corr");
   }
   for (int g = 0; g < groups; ++g) {
-    float* cg = cat + (long long)g * B * kScorePix * kCatC;
-    FEAR_TRY(launch_gemm_ffma(c, ST_CORR, s, cg, kCatC, (long long)kScorePix * kCatC, zt, kFeatC,
+    float* cg = cat + (long long)g * B * P * kCatC;
+    FEAR_TRY(launch_gemm_ffma(c, ST_CORR, s, cg, kCatC, (long long)P * kCatC, zt, kFeatC,
                               Bz == 1 ? 0 : (long long)kCorrC * kFeatC, nullptr, nullptr, 0, cg + kFeatC, kCatC,
-                              (long long)kScorePix * kCatC, kScorePix, kCorrC, kFeatC, 0, B));
+                              (long long)P * kCatC, P, kCorrC, kFeatC, 0, B));
   }
   return 0;
 }
@@ -516,71 +518,75 @@ static int run_features(FearContext* c, cudaStream_t s, const void* img, int B, 
   return launch_pw(c, ST_NECK, s, X, kBackboneC, c->neck, nullptr, 0, out, kFeatC, B * (H / 16) * (W / 16), 0);
 }
 
-// F: NHWC search features [B][256][256]; zt: [Bz][64][256]; outputs NCHW maps.
+// F: NHWC search features [B][P][256] of s x s maps (P = s * s <= 256); zt: [Bz][64][256]; outputs NCHW maps.
 // SepConv of the head (blocks.py:45-72): depthwise 3x3 (no bias, no activation) then 1x1 (+bias, ReLU).
-// With the experimental "fuse_dwpw" bit 2 the pair runs as one wgmma kernel (the depthwise map is not written).
+// With "fuse_dwpw" bit 2 the pair runs as one wgmma kernel (the depthwise map is not written); that kernel covers
+// s = 16 only and declines other sides, which run the two kernels.
 static int launch_sepconv(FearContext* c, cudaStream_t s, const float* X, const DwW& dw, const PwW& pw, float* out,
-                          int ldc, int B) {
-  const int M = B * kScorePix;
+                          int ldc, int B, int side) {
+  const int M = B * side * side;
   if ((c->opt.fuse_dwpw & 2) && tc::available() && effective(c->opt.pw) == IMPL_TC) {
     LaunchScope scope(c, ST_HEAD_PW, s);
-    int r = tc::launch_pw_dw(s, X, B, dw.k, dw.w, dw.b, 0, pw.w_hi, pw.w_lo, pw.b, nullptr, 0, out, ldc, pw.cout, pw.cin, 1);
+    int r = tc::launch_pw_dw(s, X, B, dw.k, dw.w, dw.b, 0, pw.w_hi, pw.w_lo, pw.b, nullptr, 0, out, ldc, pw.cout, pw.cin, 1,
+                             side);
     if (r < 0) return set_err(FEAR_EINVAL, "fused SepConv launch failed (%d)", r);
     if (r == 0) return check_launch("tc::pw_tc_kernel<3>");
     scope.cancel();
   }
-  FEAR_TRY(launch_dw(c, ST_HEAD_DW, s, X, dw, c->hT, B, kScore, kScore, 1, false));
+  FEAR_TRY(launch_dw(c, ST_HEAD_DW, s, X, dw, c->hT, B, side, side, 1, false));
   return launch_pw(c, ST_HEAD_PW, s, c->hT, pw.cin, pw, nullptr, 0, out, ldc, M, 1);
 }
 
 // zu (optional): dynamic-template features [Bu][64][256] for the classification branch (BoxTower.forward's `update`
 // argument, blocks.py:174-179: cls_encode(update, search) -- the regression branch keeps the original template).
+// side: score-map side s in [1, 16] (maps of P = s * s cells; the workspace holds 256 per frame).
 static int run_head(FearContext* c, cudaStream_t s, const float* zt, int Bz, const float* F, int B, float* bbox,
-                    float* cls, const float* zu = nullptr, int Bu = 0) {
-  const int M = B * kScorePix;
+                    float* cls, const float* zu = nullptr, int Bu = 0, int side = kScore) {
+  const int P = side * side, M = B * P;
+  c->head_side = side;
   // the two concat buffers are laid out back to back for THIS batch so one correlation launch covers both
-  c->hCAT[1] = c->hCAT[0] + (long long)B * kScorePix * kCatC;
+  c->hCAT[1] = c->hCAT[0] + (long long)B * P * kCatC;
   for (int br = 0; br < 2; ++br) {
     const BranchW& w = c->branch[br];
     // MatrixMobile: x -> dw3x3 -> 1x1 (+BN) -> ReLU, written into channels [0,256) of the concat buffer
-    FEAR_TRY(launch_sepconv(c, s, F, w.enc_dw, w.enc_pw, c->hCAT[br], kCatC, B));
+    FEAR_TRY(launch_sepconv(c, s, F, w.enc_dw, w.enc_pw, c->hCAT[br], kCatC, B, side));
   }
   // pixel-wise correlation of both branches into channels [256,320) of their concat buffers
   if (zu) {
-    FEAR_TRY(launch_corr(c, c->opt, s, zu, Bu, c->hCAT[0], B, 1));  // cls branch <- update template
-    FEAR_TRY(launch_corr(c, c->opt, s, zt, Bz, c->hCAT[1], B, 1));  // reg branch <- kernel template
+    FEAR_TRY(launch_corr(c, c->opt, s, zu, Bu, c->hCAT[0], B, 1, P));  // cls branch <- update template
+    FEAR_TRY(launch_corr(c, c->opt, s, zt, Bz, c->hCAT[1], B, 1, P));  // reg branch <- kernel template
   } else {
-    FEAR_TRY(launch_corr(c, c->opt, s, zt, Bz, c->hCAT[0], B, 2));
+    FEAR_TRY(launch_corr(c, c->opt, s, zt, Bz, c->hCAT[0], B, 2, P));
   }
   for (int br = 0; br < 2; ++br) {
     const BranchW& w = c->branch[br];
     // MobileCorrelation.enc: dw3x3(320) -> 1x1 320->256 (+BN) -> ReLU
-    FEAR_TRY(launch_sepconv(c, s, c->hCAT[br], w.corr_dw, w.corr_pw, c->hD[br], kFeatC, B));
+    FEAR_TRY(launch_sepconv(c, s, c->hCAT[br], w.corr_dw, w.corr_pw, c->hD[br], kFeatC, B, side));
   }
   // towers: tower[0] = bbox_tower on reg branch (hD[1]); tower[1] = cls_tower on cls branch (hD[0])
   for (int t = 0; t < 2; ++t) {
     const float* x = c->hD[t == 0 ? 1 : 0];
     float* outs[2] = {c->hP, c->hQ[t]};
     for (int i = 0; i < 2; ++i) {
-      FEAR_TRY(launch_sepconv(c, s, x, c->tower[t].dw[i], c->tower[t].pw[i], outs[i], kFeatC, B));
+      FEAR_TRY(launch_sepconv(c, s, x, c->tower[t].dw[i], c->tower[t].pw[i], outs[i], kFeatC, B, side));
       x = outs[i];
     }
-    FEAR_TRY(launch_dw(c, ST_HEAD_DW, s, x, c->pred_dw[t], c->hT, B, kScore, kScore, 1, false));
+    FEAR_TRY(launch_dw(c, ST_HEAD_DW, s, x, c->pred_dw[t], c->hT, B, side, side, 1, false));
     LaunchScope scope(c, ST_PRED, s);
     const unsigned blocks = (unsigned)((M * 32 + 255) / 256);
     if (t == 0)
-      pred_pw_kernel<4, true><<<blocks, 256, 0, s>>>(c->hT, c->pred_w[0], c->pred_b[0], bbox, B);
+      pred_pw_kernel<4, true><<<blocks, 256, 0, s>>>(c->hT, c->pred_w[0], c->pred_b[0], bbox, B, P);
     else
-      pred_pw_kernel<1, false><<<blocks, 256, 0, s>>>(c->hT, c->pred_w[1], c->pred_b[1], cls, B);
+      pred_pw_kernel<1, false><<<blocks, 256, 0, s>>>(c->hT, c->pred_w[1], c->pred_b[1], cls, B, P);
     FEAR_TRY(check_launch("pred_pw_kernel"));
   }
   return 0;
 }
 
 static int run_decode(FearContext* c, cudaStream_t s, const float* bbox, const float* cls, int B, int apply_sigmoid,
-                      FearBox* boxes) {
+                      FearBox* boxes, int side = kScore) {
   LaunchScope scope(c, ST_DECODE, s);
-  decode_kernel<<<B, 256, 0, s>>>(bbox, cls, apply_sigmoid, boxes);
+  decode_kernel<<<B, 256, 0, s>>>(bbox, cls, apply_sigmoid, boxes, side);
   return check_launch("decode_kernel");
 }
 
@@ -928,15 +934,30 @@ static int stage_template_to(FearContext* c, cudaStream_t s, const float* d_zfea
                           (long long)kTmplPix * kFeatC, kFeatC, kTmplPix, nz);
 }
 
-extern "C" int fear_head_update(FearContext* c, const float* d_zfeat, int Bz, const float* d_zupdate, int Bu,
-                                const float* d_xfeat, int B, float* d_bbox, float* d_cls, void* stream) {
+// Search side S of the sized entry points: a multiple of 16 in [16, 256] (the sizes fear_get_features takes).
+static int check_search_size(int S) {
+  if (S % 16 || S < 16 || S > 256)
+    return set_err(FEAR_EINVAL, "search size must be a multiple of 16 in [16, 256] (got %d)", S);
+  return 0;
+}
+
+// Score-map side s = S / 16 of the sized entry points: [1, 16].
+static int check_score_side(int side) {
+  if (side < 1 || side > kScore) return set_err(FEAR_EINVAL, "score-map side must be in [1, %d] (got %d)", kScore, side);
+  return 0;
+}
+
+extern "C" int fear_head_sized(FearContext* c, const float* d_zfeat, int Bz, const float* d_zupdate, int Bu,
+                               const float* d_xfeat, int B, int side, float* d_bbox, float* d_cls, void* stream) {
   FEAR_TRY(check_ctx(c));
   DeviceGuard guard(c->device);
   if (!d_zfeat || !d_xfeat || !d_bbox || !d_cls || B < 1) return set_err(FEAR_EINVAL, "bad argument");
+  FEAR_TRY(check_score_side(side));
   if (Bz != 1 && Bz != B) return set_err(FEAR_EINVAL, "template batch must be 1 or B (got %d vs %d)", Bz, B);
   if (d_zupdate && Bu != 1 && Bu != B)
     return set_err(FEAR_EINVAL, "update-template batch must be 1 or B (got %d vs %d)", Bu, B);
   cudaStream_t s = (cudaStream_t)stream;
+  const int P = side * side;
   if (Bz == 1) FEAR_TRY(stage_template(c, s, d_zfeat, 1));
   if (d_zupdate && Bu == 1) FEAR_TRY(stage_template_to(c, s, d_zupdate, 1, c->zu));
   for (int b0 = 0; b0 < B; b0 += c->reserved) {
@@ -944,13 +965,17 @@ extern "C" int fear_head_update(FearContext* c, const float* d_zfeat, int Bz, co
     if (Bz != 1) FEAR_TRY(stage_template(c, s, d_zfeat + (long long)b0 * kFeatC * kTmplPix, nb));
     if (d_zupdate && Bu != 1)
       FEAR_TRY(stage_template_to(c, s, d_zupdate + (long long)b0 * kFeatC * kTmplPix, nb, c->zu));
-    FEAR_TRY(launch_transpose(c, s, d_xfeat + (long long)b0 * kFeatC * kScorePix, kScorePix,
-                              (long long)kFeatC * kScorePix, c->hF, kFeatC, (long long)kScorePix * kFeatC, kFeatC,
-                              kScorePix, nb));
-    FEAR_TRY(run_head(c, s, c->zt, Bz == 1 ? 1 : nb, c->hF, nb, d_bbox + (long long)b0 * 4 * kScorePix,
-                      d_cls + (long long)b0 * kScorePix, d_zupdate ? c->zu : nullptr, Bu == 1 ? 1 : nb));
+    FEAR_TRY(launch_transpose(c, s, d_xfeat + (long long)b0 * kFeatC * P, P, (long long)kFeatC * P, c->hF, kFeatC,
+                              (long long)P * kFeatC, kFeatC, P, nb));
+    FEAR_TRY(run_head(c, s, c->zt, Bz == 1 ? 1 : nb, c->hF, nb, d_bbox + (long long)b0 * 4 * P,
+                      d_cls + (long long)b0 * P, d_zupdate ? c->zu : nullptr, Bu == 1 ? 1 : nb, side));
   }
   return 0;
+}
+
+extern "C" int fear_head_update(FearContext* c, const float* d_zfeat, int Bz, const float* d_zupdate, int Bu,
+                                const float* d_xfeat, int B, float* d_bbox, float* d_cls, void* stream) {
+  return fear_head_sized(c, d_zfeat, Bz, d_zupdate, Bu, d_xfeat, B, kScore, d_bbox, d_cls, stream);
 }
 
 extern "C" int fear_head(FearContext* c, const float* d_zfeat, int Bz, const float* d_xfeat, int B, float* d_bbox,
@@ -958,9 +983,11 @@ extern "C" int fear_head(FearContext* c, const float* d_zfeat, int Bz, const flo
   return fear_head_update(c, d_zfeat, Bz, nullptr, 0, d_xfeat, B, d_bbox, d_cls, stream);
 }
 
-static int track_impl(FearContext* c, cudaStream_t s, const float* d_template, const void* d_search,
+// S: search side (a multiple of 16 in [16, 256], checked by the callers); the maps are (S / 16) x (S / 16).
+static int track_impl(FearContext* c, cudaStream_t s, const float* d_template, const void* d_search, int S,
                       const float* d_zfeat, int Bz, int B, float* d_bbox, float* d_cls, FearBox* d_boxes,
                       bool search_u8 = false) {
+  const int side = S / 16, P = side * side;
   if (d_zfeat && Bz == 1) FEAR_TRY(stage_template(c, s, d_zfeat, 1));
   for (int b0 = 0; b0 < B; b0 += c->reserved) {
     const int nb = (B - b0 < c->reserved) ? B - b0 : c->reserved;
@@ -973,35 +1000,48 @@ static int track_impl(FearContext* c, cudaStream_t s, const float* d_template, c
     } else {
       nz = 1;
     }
-    const void* sp = search_u8 ? (const void*)(static_cast<const uint8_t*>(d_search) + (long long)b0 * 3 * 256 * 256)
-                               : (const void*)(static_cast<const float*>(d_search) + (long long)b0 * 3 * 256 * 256);
-    FEAR_TRY(run_features(c, s, sp, nb, 256, 256, c->hF, search_u8));
-    float* bb = d_bbox ? d_bbox + (long long)b0 * 4 * kScorePix : c->mapB;
-    float* cc = d_cls ? d_cls + (long long)b0 * kScorePix : c->mapC;
-    FEAR_TRY(run_head(c, s, c->zt, nz, c->hF, nb, bb, cc));
-    if (d_boxes) FEAR_TRY(run_decode(c, s, bb, cc, nb, 1, d_boxes + b0));
+    const long long frame_elems = 3LL * S * S;
+    const void* sp = search_u8 ? (const void*)(static_cast<const uint8_t*>(d_search) + b0 * frame_elems)
+                               : (const void*)(static_cast<const float*>(d_search) + b0 * frame_elems);
+    FEAR_TRY(run_features(c, s, sp, nb, S, S, c->hF, search_u8));
+    float* bb = d_bbox ? d_bbox + (long long)b0 * 4 * P : c->mapB;
+    float* cc = d_cls ? d_cls + (long long)b0 * P : c->mapC;
+    FEAR_TRY(run_head(c, s, c->zt, nz, c->hF, nb, bb, cc, nullptr, 0, side));
+    if (d_boxes) FEAR_TRY(run_decode(c, s, bb, cc, nb, 1, d_boxes + b0, side));
   }
   return 0;
 }
 
-extern "C" int fear_track(FearContext* c, const float* d_search, const float* d_zfeat, int Bz, int B, float* d_bbox,
-                          float* d_cls, FearBox* d_boxes, void* stream) {
+extern "C" int fear_track_sized(FearContext* c, const float* d_search, int S, const float* d_zfeat, int Bz, int B,
+                                float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream) {
   FEAR_TRY(check_ctx(c));
   DeviceGuard guard(c->device);
   if (!d_search || !d_zfeat || B < 1) return set_err(FEAR_EINVAL, "bad argument");
   if (Bz != 1 && Bz != B) return set_err(FEAR_EINVAL, "template batch must be 1 or B (got %d vs %d)", Bz, B);
   if (!d_boxes && (!d_bbox || !d_cls)) return set_err(FEAR_EINVAL, "no output requested");
-  return track_impl(c, (cudaStream_t)stream, nullptr, d_search, d_zfeat, Bz, B, d_bbox, d_cls, d_boxes);
+  FEAR_TRY(check_search_size(S));
+  return track_impl(c, (cudaStream_t)stream, nullptr, d_search, S, d_zfeat, Bz, B, d_bbox, d_cls, d_boxes);
 }
 
-extern "C" int fear_track_u8(FearContext* c, const uint8_t* d_search_u8, const float* d_zfeat, int Bz, int B,
-                             float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream) {
+extern "C" int fear_track(FearContext* c, const float* d_search, const float* d_zfeat, int Bz, int B, float* d_bbox,
+                          float* d_cls, FearBox* d_boxes, void* stream) {
+  return fear_track_sized(c, d_search, 256, d_zfeat, Bz, B, d_bbox, d_cls, d_boxes, stream);
+}
+
+extern "C" int fear_track_sized_u8(FearContext* c, const uint8_t* d_search_u8, int S, const float* d_zfeat, int Bz,
+                                   int B, float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream) {
   FEAR_TRY(check_ctx(c));
   DeviceGuard guard(c->device);
   if (!d_search_u8 || !d_zfeat || B < 1) return set_err(FEAR_EINVAL, "bad argument");
   if (Bz != 1 && Bz != B) return set_err(FEAR_EINVAL, "template batch must be 1 or B (got %d vs %d)", Bz, B);
   if (!d_boxes && (!d_bbox || !d_cls)) return set_err(FEAR_EINVAL, "no output requested");
-  return track_impl(c, (cudaStream_t)stream, nullptr, d_search_u8, d_zfeat, Bz, B, d_bbox, d_cls, d_boxes, true);
+  FEAR_TRY(check_search_size(S));
+  return track_impl(c, (cudaStream_t)stream, nullptr, d_search_u8, S, d_zfeat, Bz, B, d_bbox, d_cls, d_boxes, true);
+}
+
+extern "C" int fear_track_u8(FearContext* c, const uint8_t* d_search_u8, const float* d_zfeat, int Bz, int B,
+                             float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream) {
+  return fear_track_sized_u8(c, d_search_u8, 256, d_zfeat, Bz, B, d_bbox, d_cls, d_boxes, stream);
 }
 
 extern "C" int fear_get_features_u8(FearContext* c, const uint8_t* d_img_u8, int B, int H, int W, float* d_feat,
@@ -1022,13 +1062,19 @@ extern "C" int fear_get_features_u8(FearContext* c, const uint8_t* d_img_u8, int
   return 0;
 }
 
-extern "C" int fear_forward(FearContext* c, const float* d_template, const float* d_search, int B, float* d_bbox,
-                            float* d_cls, FearBox* d_boxes, void* stream) {
+extern "C" int fear_forward_sized(FearContext* c, const float* d_template, const float* d_search, int S, int B,
+                                  float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream) {
   FEAR_TRY(check_ctx(c));
   DeviceGuard guard(c->device);
   if (!d_template || !d_search || B < 1) return set_err(FEAR_EINVAL, "bad argument");
   if (!d_boxes && (!d_bbox || !d_cls)) return set_err(FEAR_EINVAL, "no output requested");
-  return track_impl(c, (cudaStream_t)stream, d_template, d_search, nullptr, B, B, d_bbox, d_cls, d_boxes);
+  FEAR_TRY(check_search_size(S));
+  return track_impl(c, (cudaStream_t)stream, d_template, d_search, S, nullptr, B, B, d_bbox, d_cls, d_boxes);
+}
+
+extern "C" int fear_forward(FearContext* c, const float* d_template, const float* d_search, int B, float* d_bbox,
+                            float* d_cls, FearBox* d_boxes, void* stream) {
+  return fear_forward_sized(c, d_template, d_search, 256, B, d_bbox, d_cls, d_boxes, stream);
 }
 
 // Context crop + padding + bilinear resize on the device (get_extended_crop of the tracking loop; see
@@ -1254,17 +1300,30 @@ extern "C" int fear_frame_sums_bayer_u8(const FearFrameBayer* d_views, int F, ui
   return launch_frame_sums(d_views, BayerFrames{d_views}, F, d_sums, stream);
 }
 
+extern "C" int fear_decode_sized(const float* d_bbox, const float* d_cls, int B, int side, int apply_sigmoid,
+                                 FearBox* d_boxes, void* stream) {
+  if (!d_bbox || !d_cls || !d_boxes || B < 1) return set_err(FEAR_EINVAL, "bad argument");
+  FEAR_TRY(check_score_side(side));
+  return run_decode(nullptr, (cudaStream_t)stream, d_bbox, d_cls, B, apply_sigmoid, d_boxes, side);
+}
+
 extern "C" int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoid, FearBox* d_boxes,
                            void* stream) {
-  if (!d_bbox || !d_cls || !d_boxes || B < 1) return set_err(FEAR_EINVAL, "bad argument");
-  return run_decode(nullptr, (cudaStream_t)stream, d_bbox, d_cls, B, apply_sigmoid, d_boxes);
+  return fear_decode_sized(d_bbox, d_cls, B, kScore, apply_sigmoid, d_boxes, stream);
+}
+
+extern "C" int fear_decode_smooth_sized(const float* d_bbox, const float* d_cls, int B, int side,
+                                        const double* d_prev_size, const double* d_params, FearBox* d_boxes,
+                                        void* stream) {
+  if (!d_bbox || !d_cls || !d_prev_size || !d_params || !d_boxes || B < 1) return set_err(FEAR_EINVAL, "bad argument");
+  FEAR_TRY(check_score_side(side));
+  decode_smooth_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(d_bbox, d_cls, d_prev_size, d_params, d_boxes, side);
+  return check_launch("decode_smooth_kernel");
 }
 
 extern "C" int fear_decode_smooth(const float* d_bbox, const float* d_cls, int B, const double* d_prev_size,
                                   const double* d_params, FearBox* d_boxes, void* stream) {
-  if (!d_bbox || !d_cls || !d_prev_size || !d_params || !d_boxes || B < 1) return set_err(FEAR_EINVAL, "bad argument");
-  decode_smooth_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(d_bbox, d_cls, d_prev_size, d_params, d_boxes);
-  return check_launch("decode_smooth_kernel");
+  return fear_decode_smooth_sized(d_bbox, d_cls, B, kScore, d_prev_size, d_params, d_boxes, stream);
 }
 
 extern "C" int fear_corr_nhwc_f32(const float* d_zt, int Bz, float* d_cat, int B, void* stream) {
@@ -1340,7 +1399,7 @@ extern "C" int fear_debug_backbone_prefix(FearContext* c, const float* d_img, in
   return launch_transpose(c, s, X, ch, (long long)P * ch, d_out, P, (long long)ch * P, P, ch, B);
 }
 
-// Copy a head intermediate of the LAST run (first B frames) out as NCHW (B, C, 16, 16).
+// Copy a head intermediate of the LAST run (first B frames) out as NCHW (B, C, s, s), s the score side of that run.
 extern "C" int fear_debug_head_tensor(FearContext* c, const char* name, int B, float* d_out, void* stream) {
   FEAR_TRY(check_ctx(c));
   DeviceGuard guard(c->device);
@@ -1355,8 +1414,8 @@ extern "C" int fear_debug_head_tensor(FearContext* c, const char* name, int B, f
   else if (!strcmp(name, "cls_tower")) src = c->hQ[1];
   else if (!strcmp(name, "search_features")) src = c->hF;
   else return set_err(FEAR_EINVAL, "unknown head tensor '%s'", name);
-  return launch_transpose(c, (cudaStream_t)stream, src, ch, (long long)kScorePix * ch, d_out, kScorePix,
-                          (long long)ch * kScorePix, kScorePix, ch, B);
+  const int P = c->head_side * c->head_side;
+  return launch_transpose(c, (cudaStream_t)stream, src, ch, (long long)P * ch, d_out, P, (long long)ch * P, P, ch, B);
 }
 
 // Fill every 32-bit word of the workspace (slot padding included) with `word`.  Not a LaunchScope: the fill is no

@@ -537,14 +537,15 @@ __global__ void __launch_bounds__(256) transpose_kernel(const float* __restrict_
 // Prediction 1x1 conv (256 -> NOUT, NOUT = 4 | 1) fused with the BoxTower epilogue
 // (blocks.py:187-188,192):  bbox = exp(adjust * pred + bias), cls = 0.1 * pred.  adjust / 0.1 /
 // biases are folded into w, b on the host, so this is  out = f(w . t + b).  One warp per pixel,
-// NHWC in, NCHW out (B, NOUT, 16, 16) -- the layout FEARNet returns.
+// NHWC in, NCHW out (B, NOUT, s, s) with P = s * s cells per frame -- the layout FEARNet returns.
 // ------------------------------------------------------------------------------------------
 template <int NOUT, bool EXP>
 __global__ void __launch_bounds__(256) pred_pw_kernel(const float* __restrict__ t, const float* __restrict__ w,
-                                                      const float* __restrict__ b, float* __restrict__ out, int B) {
+                                                      const float* __restrict__ b, float* __restrict__ out, int B,
+                                                      int P) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (warp >= B * 256) return;
+  if (warp >= B * P) return;
   const float4* tp = reinterpret_cast<const float4*>(t + (long long)warp * 256);
   const float4 v0 = __ldg(tp + lane), v1 = __ldg(tp + 32 + lane);
   float acc[NOUT];
@@ -573,8 +574,8 @@ __global__ void __launch_bounds__(256) pred_pw_kernel(const float* __restrict__ 
       if (lane == o) v = acc[o];
     v += __ldg(b + lane);
     if (EXP) v = expf(v);
-    const int frame = warp >> 8, p = warp & 255;
-    out[((long long)frame * NOUT + lane) * 256 + p] = v;
+    const int frame = warp / P, p = warp - frame * P;
+    out[((long long)frame * NOUT + lane) * P + p] = v;
   }
 }
 
@@ -583,7 +584,9 @@ __global__ void __launch_bounds__(256) pred_pw_kernel(const float* __restrict__ 
 // box_coder.py:75-107): score = sigmoid(cls) in fp32, argmax = first maximum in row-major
 // order, box = [gx - l, gy - t, (gx + r) - (gx - l), (gy + b) - (gy - t)] evaluated in double
 // (the reference's grid is float64, utils/utils.py:183-199, so torch promotes).  One 256-thread
-// block per frame.
+// block per frame on an s x s score map (P = s * s <= 256 cells, thread t = cell t); the grid of a search of side
+// S = 16 s is (i - s / 2) * 16 + S / 2.  Threads t >= P read nothing and hold (-inf, t), which never wins: a cell's
+// value beats -inf or ties it with a lower index.
 // ------------------------------------------------------------------------------------------
 // Does (ov, oi) beat (v, i) in the argmax?  As torch.argmax: NaN is greater than every number, and between equal
 // values or between NaNs the lower index wins.
@@ -594,12 +597,15 @@ __device__ __forceinline__ bool decode_beats(float ov, int oi, float v, int i) {
 }
 
 __global__ void __launch_bounds__(256) decode_kernel(const float* __restrict__ bbox, const float* __restrict__ cls,
-                                                     int apply_sigmoid, FearBox* __restrict__ boxes) {
+                                                     int apply_sigmoid, FearBox* __restrict__ boxes, int s) {
   __shared__ float sv[8];
   __shared__ int si[8];
-  const int f = blockIdx.x, t = threadIdx.x;
-  float v = cls[(long long)f * 256 + t];
-  if (apply_sigmoid) v = 1.0f / (1.0f + expf(-v));
+  const int f = blockIdx.x, t = threadIdx.x, P = s * s;
+  float v = -INFINITY;
+  if (t < P) {
+    v = cls[(long long)f * P + t];
+    if (apply_sigmoid) v = 1.0f / (1.0f + expf(-v));
+  }
   int i = t;
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) {
@@ -621,11 +627,11 @@ __global__ void __launch_bounds__(256) decode_kernel(const float* __restrict__ b
         v = sv[k];
         i = si[k];
       }
-    const int r = i >> 4, c = i & 15;
-    const double gx = (double)((c - 8) * 16 + 128), gy = (double)((r - 8) * 16 + 128);
-    const float* bb = bbox + (long long)f * 4 * 256 + i;
-    const double x1 = gx - (double)bb[0], y1 = gy - (double)bb[256];
-    const double x2 = gx + (double)bb[512], y2 = gy + (double)bb[768];
+    const int r = i / s, c = i - r * s;
+    const double gx = (double)((c - s / 2) * 16 + 8 * s), gy = (double)((r - s / 2) * 16 + 8 * s);
+    const float* bb = bbox + (long long)f * 4 * P + i;
+    const double x1 = gx - (double)bb[0], y1 = gy - (double)bb[P];
+    const double x2 = gx + (double)bb[2 * P], y2 = gy + (double)bb[3 * P];
     FearBox o;
     o.x = x1;
     o.y = y1;
@@ -641,9 +647,10 @@ __global__ void __launch_bounds__(256) decode_kernel(const float* __restrict__ b
 
 // ------------------------------------------------------------------------------------------
 // Smoothed box decode (FEARTracker._smooth_postprocess, reference base_tracker.py:126-205): scale / ratio
-// penalty, window re-weighting and size smoothing.  One 256-thread block per frame, one thread per score cell.
-// Every float64 step is a rounded intrinsic (no FMA contraction) in numpy's order, so the only difference from the
-// host is CUDA's double exp (within 1 ulp).  params = penalty_k, window_influence, lr, window[256].
+// penalty, window re-weighting and size smoothing.  One 256-thread block per frame, one thread per score cell of an
+// s x s map (decode_kernel's grid; threads t >= P = s * s read nothing and hold (-inf, t)).  Every float64 step is a
+// rounded intrinsic (no FMA contraction) in numpy's order, so the only difference from the host is CUDA's double exp
+// (within 1 ulp).  params = penalty_k, window_influence, lr, window[P].
 // ------------------------------------------------------------------------------------------
 // decode_beats on the penalised float64 score (np.argmax: the first NaN wins, ties go to the lower index).
 __device__ __forceinline__ bool smooth_beats(double ov, int oi, double v, int i) {
@@ -668,24 +675,30 @@ __global__ void __launch_bounds__(256) decode_smooth_kernel(const float* __restr
                                                             const float* __restrict__ cls,
                                                             const double* __restrict__ prev_size,
                                                             const double* __restrict__ params,
-                                                            FearBox* __restrict__ boxes) {
+                                                            FearBox* __restrict__ boxes, int s) {
   __shared__ double sv[8];
   __shared__ int si[8];
   __shared__ int win;
-  const int f = blockIdx.x, t = threadIdx.x;
-  const float score = 1.0f / (1.0f + expf(-cls[(long long)f * 256 + t]));  // decode_kernel's sigmoid
-  const int r = t >> 4, c = t & 15;
-  const double gx = (double)((c - 8) * 16 + 128), gy = (double)((r - 8) * 16 + 128);
-  const float* bb = bbox + (long long)f * 4 * 256 + t;
-  const double x1 = __dsub_rn(gx, (double)bb[0]), y1 = __dsub_rn(gy, (double)bb[256]);
-  const double x2 = __dadd_rn(gx, (double)bb[512]), y2 = __dadd_rn(gy, (double)bb[768]);
-  const double w = __dsub_rn(x2, x1), h = __dsub_rn(y2, y1);
+  const int f = blockIdx.x, t = threadIdx.x, P = s * s;
+  const int r = t / s, c = t - r * s;
+  float score = 0.f;
+  double x1 = 0.0, y1 = 0.0, w = 0.0, h = 0.0, penalty = 0.0, v = -INFINITY;
   const double pw = prev_size[2LL * f], ph = prev_size[2LL * f + 1];
-  const double penalty_k = params[0], wi = params[1];
-  const double s_c = smooth_limit(__ddiv_rn(smooth_sq(w, h), smooth_sq(pw, ph)));
-  const double r_c = smooth_limit(__ddiv_rn(__ddiv_rn(pw, ph), __ddiv_rn(w, h)));
-  const double penalty = exp(__dmul_rn(-__dsub_rn(__dmul_rn(r_c, s_c), 1.0), penalty_k));
-  double v = __dadd_rn(__dmul_rn(__dmul_rn(penalty, (double)score), __dsub_rn(1.0, wi)), __dmul_rn(params[3 + t], wi));
+  if (t < P) {
+    score = 1.0f / (1.0f + expf(-cls[(long long)f * P + t]));  // decode_kernel's sigmoid
+    const double gx = (double)((c - s / 2) * 16 + 8 * s), gy = (double)((r - s / 2) * 16 + 8 * s);
+    const float* bb = bbox + (long long)f * 4 * P + t;
+    x1 = __dsub_rn(gx, (double)bb[0]);
+    y1 = __dsub_rn(gy, (double)bb[P]);
+    const double x2 = __dadd_rn(gx, (double)bb[2 * P]), y2 = __dadd_rn(gy, (double)bb[3 * P]);
+    w = __dsub_rn(x2, x1);
+    h = __dsub_rn(y2, y1);
+    const double penalty_k = params[0], wi = params[1];
+    const double s_c = smooth_limit(__ddiv_rn(smooth_sq(w, h), smooth_sq(pw, ph)));
+    const double r_c = smooth_limit(__ddiv_rn(__ddiv_rn(pw, ph), __ddiv_rn(w, h)));
+    penalty = exp(__dmul_rn(-__dsub_rn(__dmul_rn(r_c, s_c), 1.0), penalty_k));
+    v = __dadd_rn(__dmul_rn(__dmul_rn(penalty, (double)score), __dsub_rn(1.0, wi)), __dmul_rn(params[3 + t], wi));
+  }
   int i = t;
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) {

@@ -3,10 +3,11 @@
 // corr_tc_kernel -- the pixel-wise template (x) search correlation (MobileCorrelation.forward's matmul,
 // reference model_training/model/blocks.py:123) on the Hopper tensor cores:
 //
-//     s[b, p, k] = sum_c x[b, p, c] * z[b, k, c]        p in 256 search cells, k in 64 template cells, c in 256
+//     s[b, p, k] = sum_c x[b, p, c] * z[b, k, c]        p in P search cells, k in 64 template cells, c in 256
 //
+// P = s * s is the score map (s = 16 for 256 x 256 searches, any s in [1, 16] for searches of side 16 s).
 // Channels-last operands are K-major GEMM operands as they lie in HBM: x = first 256 channels of the
-// 320-channel concat buffer [B*256][320] (written there by the encode 1x1 conv), z = [Bz*64][256].
+// 320-channel concat buffer [B*P][320] (written there by the encode 1x1 conv), z = [Bz*64][256].
 // The result goes straight into channels [256,320) of the same buffer, so the "torch.cat" of the
 // reference costs nothing and the kernel moves exactly the algorithmic bytes (z + x in, s out).
 //
@@ -43,9 +44,11 @@ constexpr int kTcConsumers = 256;
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
-// corr_tc_kernel: tile = half a frame (128 search cells) x 64 template cells, K = 256 in 8 chunks.  The template
-// tile is an MMA operand in shared memory and is not pre-split: the consumers rewrite each landed tile as hi
-// (low mantissa bits cleared, in place) and write lo right behind it.
+// corr_tc_kernel: tile = 128 search cells of one frame x 64 template cells, K = 256 in 8 chunks; ceil(P / 128) tiles
+// per frame (two at P = 256), so a tile never straddles two frames.  The search operand is read through a 3-D map
+// (channel, cell, frame): TMA zero-fills the cells >= P of a frame's last tile and the epilogue does not store them.
+// The template tile is an MMA operand in shared memory and is not pre-split: the consumers rewrite each landed tile as
+// hi (low mantissa bits cleared, in place) and write lo right behind it.
 // ------------------------------------------------------------------------------------------
 constexpr int kCorrStages = 3;
 constexpr int kCorrStageBytes = kCorrABytes + 2 * kCorrBBytes;  // x raw | z hi | z lo
@@ -53,7 +56,7 @@ constexpr int kCorrSmemBytes = kCorrStages * kCorrStageBytes + 1024 /*align*/ + 
 
 __global__ void __launch_bounds__(kTcThreads, 1)
 corr_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               float* __restrict__ cat, int z_mod) {
+               float* __restrict__ cat, int z_mod, int P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kCorrStages * kCorrStageBytes);  // [stages] TMA landed
@@ -72,8 +75,8 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   __syncthreads();
   pdl_trigger();
   pdl_wait();
-  const int frame = blockIdx.x >> 1, half = blockIdx.x & 1;
-  const int arow = frame * 256 + half * 128;
+  const int tiles = (P + 127) >> 7;
+  const int frame = blockIdx.x / tiles, cell0 = (blockIdx.x - frame * tiles) * 128;
   auto st_x = [&](int s) { return smem + s * kCorrStageBytes; };
   auto st_z = [&](int s) { return smem + s * kCorrStageBytes + kCorrABytes; };
 
@@ -84,7 +87,7 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int stage = c % kCorrStages;
         mbar_wait_backoff(&empty[stage], (uint32_t)(((c / kCorrStages) & 1) ^ 1));
         mbar_arrive_expect_tx(&full[stage], kCorrABytes + kCorrBBytes);
-        tma_load_2d(st_x(stage), &tmA, &full[stage], c * kCorrChunk, arow);
+        tma_load_3d(st_x(stage), &tmA, &full[stage], c * kCorrChunk, cell0, frame);
         tma_load_2d(st_z(stage), &tmB, &full[stage], c * kCorrChunk, brow);
       }
     }
@@ -123,12 +126,18 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[stage]);
   }
-  float* out = cat + (long long)(arow + r0) * 320 + 256 + 2 * t;
+  const int cell = cell0 + r0;  // this thread's rows: cell and cell + 8
+  float* out = cat + ((long long)frame * P + cell) * 320 + 256 + 2 * t;
+  if (cell < P) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    *reinterpret_cast<float2*>(out + 8 * i) = make_float2(accm[4 * i] + accc[4 * i], accm[4 * i + 1] + accc[4 * i + 1]);
-    *reinterpret_cast<float2*>(out + 8 * 320 + 8 * i) =
-        make_float2(accm[4 * i + 2] + accc[4 * i + 2], accm[4 * i + 3] + accc[4 * i + 3]);
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<float2*>(out + 8 * i) = make_float2(accm[4 * i] + accc[4 * i], accm[4 * i + 1] + accc[4 * i + 1]);
+  }
+  if (cell + 8 < P) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<float2*>(out + 8 * 320 + 8 * i) =
+          make_float2(accm[4 * i + 2] + accc[4 * i + 2], accm[4 * i + 3] + accc[4 * i + 3]);
   }
 }
 
@@ -156,19 +165,21 @@ inline int init() {
   return 0;
 }
 
-// cat holds `groups` consecutive [B][256][320] buffers (the cls and reg branches of the head): frame f of
+// cat holds `groups` consecutive [B][P][320] buffers (the cls and reg branches of the head): frame f of
 // every group correlates with template f (or template 0 when Bz == 1).  One launch covers all groups.
-inline int launch_corr(cudaStream_t s, const float* zt, int Bz, float* cat, int B, int groups) {
+inline int launch_corr(cudaStream_t s, const float* zt, int Bz, float* cat, int B, int groups, int P) {
   if (!available()) return -20;
+  if (P < 1 || P > 256) return -21;
   CUtensorMap tmA, tmB;
   const int frames = B * groups;
   int r;
-  r = make_tmap_2d(&tmA, cat, (uint64_t)frames * 256, 320, 320, 128, kCorrChunk);
+  r = make_tmap_3d(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, cat, 320, (uint64_t)P, (uint64_t)frames, 320 * 4,
+                   (uint64_t)P * 320 * 4, kCorrChunk, 128, 1, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (r) return r;
   r = make_tmap_2d(&tmB, zt, (uint64_t)Bz * 64, 256, 256, 64, kCorrChunk);
   if (r) return r;
-  if (launch_pdl(corr_tc_kernel, dim3(frames * 2), dim3(kTcThreads), kCorrSmemBytes, s, tmA, tmB, cat, Bz == 1 ? 0 : B) !=
-      cudaSuccess)
+  if (launch_pdl(corr_tc_kernel, dim3(frames * ((P + 127) / 128)), dim3(kTcThreads), kCorrSmemBytes, s, tmA, tmB, cat,
+                 Bz == 1 ? 0 : B, P) != cudaSuccess)
     return -23;
   return 0;
 }

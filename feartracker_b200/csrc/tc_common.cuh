@@ -140,14 +140,17 @@ inline int make_tmap_nhwc(CUtensorMap* m, const float* base, uint64_t B, uint64_
                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 
-// Generic unswizzled 3-D map (dims / box innermost first, strides in bytes for dims 1 and 2); out-of-range
-// elements read as zero.  Used for the image patches of the fused stem kernel (fp32 planes or uint8 HWC rows).
+// Generic 3-D map (dims / box innermost first, strides in bytes for dims 1 and 2); out-of-range elements read as
+// zero.  Unswizzled by default: the image patches of the fused stem kernel (fp32 planes or uint8 HWC rows).  The
+// correlation reads its search cells (channel, cell, frame) with a 128-byte swizzle.
 inline int make_tmap_3d(CUtensorMap* m, CUtensorMapDataType dt, const void* base, uint64_t d0, uint64_t d1, uint64_t d2,
-                        uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t b0, uint32_t b1, uint32_t b2) {
+                        uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t b0, uint32_t b1, uint32_t b2,
+                        CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_NONE,
+                        CUtensorMapL2promotion promo = CU_TENSOR_MAP_L2_PROMOTION_L2_128B) {
   cuuint64_t dims[3] = {d0, d1, d2};
   cuuint64_t strides[2] = {stride1_bytes, stride2_bytes};
   cuuint32_t box[3] = {b0, b1, b2};
-  return encode_cached(m, dt, 3, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  return encode_cached(m, dt, 3, base, dims, strides, box, sw, promo);
 }
 
 // Plain (unswizzled) 2-D map, used for the small per-layer weight / bias tables.

@@ -155,6 +155,18 @@ class BoxTower(_Params):
         self.bias = nn.Parameter(torch.ones(1, 4, 1, 1))
 
 
+def search_side(shape, u8: bool) -> int:
+    """Side S of a square search batch: float (B,3,S,S) or uint8 (B,S,S,3), S a multiple of 16 in [16, 256] (the crop
+    sizes the library takes; the reference sets it as instance_size).  ValueError otherwise."""
+    shape = tuple(shape)
+    ok = len(shape) == 4 and (shape[3] == 3 and shape[1] == shape[2] if u8 else shape[1] == 3 and shape[2] == shape[3])
+    side = (shape[1] if u8 else shape[2]) if ok else 0
+    if not ok or side % 16 or not 16 <= side <= 256:
+        layout = "uint8 (B,S,S,3)" if u8 else "float (B,3,S,S)"
+        raise ValueError(f"search must be {layout} with S a multiple of 16 in [16, 256], got {shape}")
+    return int(side)
+
+
 def _make_grid(score_size: int, total_stride: int, instance_size: int):
     """float64 (1,S,S) pixel-centre grids: (i - S//2) * stride + instance//2 (reference
     utils/utils.py:183-199)."""
@@ -206,6 +218,7 @@ class FEARNet(nn.Module):
         self._handle: Optional[ctypes.c_void_p] = None
         self._handle_device: Optional[int] = None
         self._reserved = 0
+        self._head_side = 16  # score-map side of the last library head call (head_tensor)
 
     # ------------------------------------------------------------------ reference surface
     def grids(self, size: int) -> None:
@@ -260,13 +273,15 @@ class FEARNet(nn.Module):
         if update is not None:
             zu = self._as_input(update, xf.device)
             self._check_shapes(zu, b)
-        if tuple(xf.shape[1:]) != (256, 16, 16):
-            raise ValueError(f"search features must be (B,256,16,16), got {tuple(xf.shape)}")
-        bbox = torch.empty((b, 4, 16, 16), device=xf.device, dtype=torch.float32)
-        cls = torch.empty((b, 1, 16, 16), device=xf.device, dtype=torch.float32)
-        _lib.check(lib.fear_head_update(h, zf.data_ptr(), zf.shape[0], zu.data_ptr() if zu is not None else None,
-                                        zu.shape[0] if zu is not None else 0, xf.data_ptr(), b, bbox.data_ptr(),
-                                        cls.data_ptr(), self._stream(xf)), "fear_head_update")
+        side = xf.shape[2] if xf.dim() == 4 else 0
+        if xf.dim() != 4 or tuple(xf.shape[1:]) != (256, side, side) or not 1 <= side <= 16:
+            raise ValueError(f"search features must be (B,256,s,s) with s in [1, 16], got {tuple(xf.shape)}")
+        bbox = torch.empty((b, 4, side, side), device=xf.device, dtype=torch.float32)
+        cls = torch.empty((b, 1, side, side), device=xf.device, dtype=torch.float32)
+        _lib.check(lib.fear_head_sized(h, zf.data_ptr(), zf.shape[0], zu.data_ptr() if zu is not None else None,
+                                       zu.shape[0] if zu is not None else 0, xf.data_ptr(), b, side, bbox.data_ptr(),
+                                       cls.data_ptr(), self._stream(xf)), "fear_head_sized")
+        self._head_side = side
         return {TARGET_REGRESSION_LABEL_KEY: bbox, TARGET_CLASSIFICATION_KEY: cls}
 
     def forward(self, x: Tuple[torch.Tensor, torch.Tensor]) -> Dict[str, torch.Tensor]:
@@ -277,13 +292,16 @@ class FEARNet(nn.Module):
         t = self._as_input(template, s.device)
         b = s.shape[0]
         self.size = b
-        if tuple(t.shape) != (b, 3, 128, 128) or tuple(s.shape) != (b, 3, 256, 256):
-            raise ValueError(f"forward expects template (B,3,128,128) and search (B,3,256,256); got "
+        if tuple(t.shape) != (b, 3, 128, 128) or s.dim() != 4:
+            raise ValueError(f"forward expects template (B,3,128,128) and search (B,3,S,S); got "
                              f"{tuple(t.shape)} / {tuple(s.shape)}")
-        bbox = torch.empty((b, 4, 16, 16), device=s.device, dtype=torch.float32)
-        cls = torch.empty((b, 1, 16, 16), device=s.device, dtype=torch.float32)
-        _lib.check(lib.fear_forward(h, t.data_ptr(), s.data_ptr(), b, bbox.data_ptr(), cls.data_ptr(), None,
-                                    self._stream(s)), "fear_forward")
+        size = search_side(s.shape, u8=False)
+        side = size // 16
+        bbox = torch.empty((b, 4, side, side), device=s.device, dtype=torch.float32)
+        cls = torch.empty((b, 1, side, side), device=s.device, dtype=torch.float32)
+        _lib.check(lib.fear_forward_sized(h, t.data_ptr(), s.data_ptr(), size, b, bbox.data_ptr(), cls.data_ptr(), None,
+                                          self._stream(s)), "fear_forward_sized")
+        self._head_side = side
         return {TARGET_REGRESSION_LABEL_KEY: bbox, TARGET_CLASSIFICATION_KEY: cls}
 
     def track(self, search: torch.Tensor, template_features: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -294,21 +312,22 @@ class FEARNet(nn.Module):
 
     # ------------------------------------------------------------------ extensions
     def track_boxes(self, search: torch.Tensor, template_features: torch.Tensor, with_maps: bool = False):
-        """track() + on-device FEARBoxCoder.decode.  Returns a uint8 tensor (B,48) of FearBox records
-        (view with ``boxes_to_numpy``) and, if requested, the maps dictionary."""
+        """track() + on-device FEARBoxCoder.decode (instance_size = S for a search of side S).  Returns a uint8 tensor
+        (B,48) of FearBox records (view with ``boxes_to_numpy``) and, if requested, the maps dictionary."""
         maps, boxes = self._track(search, template_features, want_maps=with_maps, want_boxes=True)
         return (boxes, maps) if with_maps else boxes
 
     def track_boxes_from_host(self, search_host: torch.Tensor, template_features_host: torch.Tensor,
                               out_host: Optional[torch.Tensor] = None, chunks: int = 1) -> torch.Tensor:
-        """End-to-end batched call on PINNED host buffers (uint8 (B,256,256,3) raw crops or float32
-        (B,3,256,256) normalised crops, plus float32 template features).
+        """End-to-end batched call on PINNED host buffers (uint8 (B,S,S,3) raw crops or float32
+        (B,3,S,S) normalised crops, S a multiple of 16 in [16, 256], plus float32 template features).
 
         The host->device copies run on a side stream into one of TWO staging sets, so the copy of call i+1
         overlaps the kernels of call i (and, with ``chunks`` > 1, the copy of slice j+1 overlaps the kernels
         of slice j inside one call).  The 48-byte box records of the whole batch are copied back to
         ``out_host`` if given.  No host synchronisation: synchronise the current stream (or an event) before
         reading ``out_host`` / the returned device tensor, which stays valid until the call after next."""
+        search_side(search_host.shape, u8=search_host.dtype == torch.uint8)
         dev = next(self.parameters()).device
         if self.training or dev.type != "cuda":
             raise RuntimeError("track_boxes_from_host needs the model in eval mode on a CUDA device")
@@ -364,12 +383,14 @@ class FEARNet(nn.Module):
         return boxes.cpu().numpy().view(_lib.BOX_DTYPE).reshape(-1)
 
     def head_tensor(self, name: str, batch: int) -> torch.Tensor:
-        """NCHW copy of a head intermediate of the last call: "cat_cls" | "cat_reg" (B,320,16,16);
-        "search_features" | "cls_dw" | "reg_dw" | "x_reg" | "cls_tower" (B,256,16,16)."""
+        """NCHW copy of a head intermediate of the last call: "cat_cls" | "cat_reg" (B,320,s,s);
+        "search_features" | "cls_dw" | "reg_dw" | "x_reg" | "cls_tower" (B,256,s,s); s = 16 for 256 x 256 searches,
+        S / 16 for searches of side S."""
         dev = next(self.parameters()).device
         h, lib = self._ensure_handle(dev)
         ch = 320 if name.startswith("cat_") else 256
-        out = torch.empty((batch, ch, 16, 16), device=dev, dtype=torch.float32)
+        side = self._head_side
+        out = torch.empty((batch, ch, side, side), device=dev, dtype=torch.float32)
         _lib.check(lib.fear_debug_head_tensor(h, name.encode(), batch, out.data_ptr(),
                                               torch.cuda.current_stream(dev).cuda_stream), "fear_debug_head_tensor")
         return out
@@ -428,20 +449,21 @@ class FEARNet(nn.Module):
         zf = self._as_input(template_features, s.device)
         b = s.shape[0]
         self._check_shapes(zf, b)
-        if tuple(s.shape[1:]) != ((256, 256, 3) if u8 else (3, 256, 256)):
-            raise ValueError(f"search must be float (B,3,256,256) or uint8 (B,256,256,3), got {tuple(s.shape)}")
+        size = search_side(s.shape, u8)
+        side = size // 16
         bbox = cls = boxes = None
         if want_maps:
-            bbox = torch.empty((b, 4, 16, 16), device=s.device, dtype=torch.float32)
-            cls = torch.empty((b, 1, 16, 16), device=s.device, dtype=torch.float32)
+            bbox = torch.empty((b, 4, side, side), device=s.device, dtype=torch.float32)
+            cls = torch.empty((b, 1, side, side), device=s.device, dtype=torch.float32)
         if want_boxes:
             boxes = torch.empty((b, _lib.BOX_DTYPE.itemsize), device=s.device, dtype=torch.uint8)
-        entry = lib.fear_track_u8 if u8 else lib.fear_track
+        entry = lib.fear_track_sized_u8 if u8 else lib.fear_track_sized
         _lib.check(
-            entry(h, s.data_ptr(), zf.data_ptr(), zf.shape[0], b,
-                           bbox.data_ptr() if want_maps else None, cls.data_ptr() if want_maps else None,
-                           boxes.data_ptr() if want_boxes else None, self._stream(s)),
-            "fear_track")
+            entry(h, s.data_ptr(), size, zf.data_ptr(), zf.shape[0], b,
+                  bbox.data_ptr() if want_maps else None, cls.data_ptr() if want_maps else None,
+                  boxes.data_ptr() if want_boxes else None, self._stream(s)),
+            "fear_track_sized")
+        self._head_side = side
         maps = {TARGET_REGRESSION_LABEL_KEY: bbox, TARGET_CLASSIFICATION_KEY: cls} if want_maps else None
         return maps, boxes
 

@@ -531,9 +531,14 @@ class FEARMultiTracker:
             v = float(cfg[key])
             if not math.isfinite(v) or v < 0:
                 raise ValueError(f"{key} must be finite and >= 0, got {cfg[key]!r}")
-        if int(cfg["instance_size"]) != 256 or int(cfg["template_size"]) != 128:
-            raise ValueError("FEAR-XS tracks 256 x 256 search crops against 128 x 128 templates; got instance_size="
-                             f"{cfg['instance_size']}, template_size={cfg['template_size']}")
+        size = int(cfg["instance_size"])
+        if size % 16 or not 16 <= size <= 256 or int(cfg["template_size"]) != 128:
+            raise ValueError("FEAR-XS tracks S x S search crops, S a multiple of 16 in [16, 256], against 128 x 128 "
+                             f"templates; got instance_size={cfg['instance_size']}, template_size={cfg['template_size']}")
+        stride, score = cfg.get("total_stride", 16), cfg.get("score_size", size // 16)
+        if int(stride) != 16 or int(score) != size // 16:
+            raise ValueError(f"a {size} x {size} search gives a {size // 16} x {size // 16} score map at total_stride 16; "
+                             f"got score_size={score}, total_stride={stride}")
         if int(max_targets) < 1:
             raise ValueError(f"max_targets must be >= 1, got {max_targets}")
         self.net = model

@@ -126,7 +126,13 @@ class FEARTracker(Tracker):
     ``host_normalize: true`` takes numpy frames only."""
 
     def get_box_coder(self, tracking_config, cuda_id: int = 0):
+        size, stride, score = (tracking_config[k] for k in ("instance_size", "total_stride", "score_size"))
+        if isinstance(stride, int) and stride > 0 and score != size // stride:
+            raise ValueError(f"score_size must be instance_size // total_stride = {size // stride}, got {score}")
         return FEARBoxCoder(tracker_config=tracking_config)
+
+    def _score_cells(self) -> int:
+        return int(self.tracking_config["score_size"]) ** 2
 
     def initialize(self, image: np.ndarray, rect: np.ndarray, **kwargs) -> None:
         """image: RGB uint8 HxWx3 (or a device frame, see the class docstring); rect: [x, y, w, h], 0-based."""
@@ -173,9 +179,9 @@ class FEARTracker(Tracker):
         """``gpu_crop=True``: the frame is uploaded once and the context crop + constant padding + bilinear resize of
         get_extended_crop (reference utils/utils.py:215-253) runs on the device (fear_crop_resize_u8, bit-identical
         to cv2's 8-bit fixed-point INTER_LINEAR) in the same CUDA graph as the network and the decode; the host only
-        computes the integer context box and the 2 x 256 resize coefficients.  With ``smooth: true`` the network
-        writes its maps and fear_decode_smooth runs the penalty, window and size smoothing of _smooth_postprocess in
-        the same graph."""
+        computes the integer context box and the 2 x instance_size resize coefficients.  With ``smooth: true`` the
+        network writes its maps and fear_decode_smooth_sized runs the penalty, window and size smoothing of
+        _smooth_postprocess in the same graph."""
         st, cfg = self.tracking_state, self.tracking_config
         if cfg.get("host_normalize", False) or image.shape[2] != 3:
             raise NotImplementedError("gpu_crop covers the default uint8 RGB tracking path (no smooth / host_normalize)")
@@ -211,11 +217,12 @@ class FEARTracker(Tracker):
                       box_pin=torch.empty((1, 48), dtype=torch.uint8).pin_memory(),
                       graph=None, boxes=None, generation=None, zf_src=None, calls=0, graph_ok=True)
             if smooth:
-                # fear_decode_smooth's inputs in one float64 buffer: prev_size (w, h), then its 259 params (penalty_k,
-                # window_influence, lr, window).  The five scalars are copied per update, the window once here.
+                # fear_decode_smooth_sized's inputs in one float64 buffer: prev_size (w, h), then its 3 + s * s params
+                # (penalty_k, window_influence, lr, window).  The five scalars are copied per update, the window once here.
+                cells = self._score_cells()
                 st["smooth_pin"] = torch.empty(5, dtype=torch.float64).pin_memory()
-                st["smooth_in"] = torch.empty(5 + 256, dtype=torch.float64, device=dev)
-                st["smooth_in"][5:].copy_(torch.from_numpy(np.asarray(self.window, dtype=np.float64).reshape(256)))
+                st["smooth_in"] = torch.empty(5 + cells, dtype=torch.float64, device=dev)
+                st["smooth_in"][5:].copy_(torch.from_numpy(np.asarray(self.window, dtype=np.float64).reshape(cells)))
                 st["smooth_boxes"] = torch.empty((1, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8, device=dev)
             self._gpu_crop_state = st
         np.copyto(st["frame_pin"].numpy(), image)
@@ -239,9 +246,10 @@ class FEARTracker(Tracker):
                 return self.net.track_boxes(st["crop"], st["zf"])
             maps = self.net.track(st["crop"], st["zf"])  # maps only: the plain decode is skipped
             sp = st["smooth_in"].data_ptr()
-            _lib.check(lib.fear_decode_smooth(maps[TARGET_REGRESSION_LABEL_KEY].data_ptr(),
-                                              maps[TARGET_CLASSIFICATION_KEY].data_ptr(), 1, sp, sp + 16,
-                                              st["smooth_boxes"].data_ptr(), stream), "fear_decode_smooth")
+            _lib.check(lib.fear_decode_smooth_sized(maps[TARGET_REGRESSION_LABEL_KEY].data_ptr(),
+                                                    maps[TARGET_CLASSIFICATION_KEY].data_ptr(), 1, size // 16, sp,
+                                                    sp + 16, st["smooth_boxes"].data_ptr(), stream),
+                       "fear_decode_smooth_sized")
             return st["smooth_boxes"]
 
         use_graph = self.tracking_config.get("cuda_graph", True) and st["graph_ok"]
@@ -287,7 +295,7 @@ class FEARTracker(Tracker):
         share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView, a
         FearFrameYCbCr, a FearFrameYCbCrV210, a FearFrameYCbCrHDR or a FearFrameBayer) at byte 0, the FearTarget at
         byte 104, fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr as float64 at byte 168;
-        then, on the device only, the 16 x 16 window."""
+        then, on the device only, the score_size x score_size window."""
         from . import _lib
 
         dev = self._device()
@@ -298,7 +306,7 @@ class FEARTracker(Tracker):
         size, tsize = int(self.tracking_config["instance_size"]), int(self.tracking_config["template_size"])
         st = dict(device=dev, smooth=smooth,
                   inputs=torch.zeros(_DEVICE_INPUT_BYTES, dtype=torch.uint8).pin_memory(),
-                  dev_in=torch.zeros(_DEVICE_INPUT_BYTES + 256 * 8, dtype=torch.uint8, device=dev),
+                  dev_in=torch.zeros(_DEVICE_INPUT_BYTES + self._score_cells() * 8, dtype=torch.uint8, device=dev),
                   crop=torch.empty((1, size, size, 3), dtype=torch.uint8, device=dev),
                   tcrop=torch.empty((1, tsize, tsize, 3), dtype=torch.uint8, device=dev),
                   sums=torch.empty((1, 3), dtype=torch.int64, device=dev),
@@ -307,7 +315,7 @@ class FEARTracker(Tracker):
                   smooth_boxes=torch.empty((1, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8, device=dev),
                   box_pin=torch.empty((1, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
                   graph=None, boxes=None, key=None, zf_src=None, calls=0, graph_ok=True)
-        window = np.asarray(self.window, dtype=np.float64).reshape(256)
+        window = np.asarray(self.window, dtype=np.float64).reshape(self._score_cells())
         st["dev_in"][_DEVICE_INPUT_BYTES:].copy_(torch.from_numpy(window).view(torch.uint8))
         self._device_state = st
         return st
@@ -389,8 +397,8 @@ class FEARTracker(Tracker):
         return dict(bbox=pred_bbox)
 
     def _track_record_device_frame(self, image, kind: str):
-        """One update on a device frame: crop-targets (N = 1, search_context, 256) -> fear_track_u8 -> the plain decode,
-        or with smooth the maps -> fear_decode_smooth; one 48-byte record back.  The crop kernel reads the frame's record
+        """One update on a device frame: crop-targets (N = 1, search_context, instance_size) -> fear_track_sized_u8 -> the
+        plain decode, or with smooth the maps -> fear_decode_smooth_sized; one 48-byte record back.  The crop kernel reads the frame's record
         when it runs, so the graph (captured on the second update) keys on the table kind, smooth, the input buffer and
         net.generation(), not on the frame's address or shape: fresh decoder surfaces and a resolution change replay it."""
         from . import _lib
@@ -417,9 +425,10 @@ class FEARTracker(Tracker):
                     return self.net.track_boxes(st["crop"], st["zf"])
                 maps = self.net.track(st["crop"], st["zf"])
                 sp = dp + _SMOOTH_OFFSET
-                _lib.check(lib.fear_decode_smooth(maps[TARGET_REGRESSION_LABEL_KEY].data_ptr(),
-                                                  maps[TARGET_CLASSIFICATION_KEY].data_ptr(), 1, sp, sp + 16,
-                                                  st["smooth_boxes"].data_ptr(), stream), "fear_decode_smooth")
+                _lib.check(lib.fear_decode_smooth_sized(maps[TARGET_REGRESSION_LABEL_KEY].data_ptr(),
+                                                        maps[TARGET_CLASSIFICATION_KEY].data_ptr(), 1, size // 16, sp,
+                                                        sp + 16, st["smooth_boxes"].data_ptr(), stream),
+                           "fear_decode_smooth_sized")
                 return st["smooth_boxes"]
 
             key = (table, smooth, st["dev_in"].data_ptr(), self.net.generation())
@@ -467,7 +476,8 @@ class FEARTracker(Tracker):
         st = getattr(self, "_stream_state", None)
         host_norm = bool(self.tracking_config.get("host_normalize", False))
         if st is None or st["device"] != dev or st["host_norm"] != host_norm:
-            shape, dtype = ((1, 3, 256, 256), torch.float32) if host_norm else ((1, 256, 256, 3), torch.uint8)
+            size = int(self.tracking_config["instance_size"])
+            shape, dtype = ((1, 3, size, size), torch.float32) if host_norm else ((1, size, size, 3), torch.uint8)
             st = dict(device=dev, host_norm=host_norm, pin=torch.empty(shape, dtype=dtype).pin_memory(),
                       dev=torch.empty(shape, dtype=dtype, device=dev),
                       zf=torch.empty((1, 256, 8, 8), dtype=torch.float32, device=dev),
@@ -523,7 +533,7 @@ class FEARTracker(Tracker):
 
     def _smooth_postprocess(self, reg: np.ndarray, score: np.ndarray) -> Tuple[np.ndarray, float]:
         """Scale/ratio penalty + cosine window + size smoothing (reference base_tracker.py:126-205),
-        256-element float64 host math; only active when the config carries ``smooth: true``."""
+        score_size x score_size float64 host math; only active when the config carries ``smooth: true``."""
         cfg, st = self.tracking_config, self.tracking_state
         gx, gy = self.box_coder.grid_x.cpu().numpy()[0], self.box_coder.grid_y.cpu().numpy()[0]
         x1, y1, x2, y2 = gx - reg[0], gy - reg[1], gx + reg[2], gy + reg[3]
@@ -542,7 +552,7 @@ class FEARTracker(Tracker):
         pscore = penalty * score
         pscore = pscore * (1 - cfg["window_influence"]) + self.window * cfg["window_influence"]
         flat = int(np.argmax(pscore))
-        r, c = flat // 16, flat % 16
+        r, c = divmod(flat, pscore.shape[1])
         box = np.array([x1[r, c], y1[r, c], x2[r, c] - x1[r, c], y2[r, c] - y1[r, c]])
         # the reference multiplies a float64 numpy scalar into a float32 torch scalar (base_tracker.py:158): the size
         # learning rate is therefore rounded to float32 at each step -- reproduced here so boxes match to the last bit

@@ -16,6 +16,8 @@
  *   fear_decode           FEARBoxCoder.decode                 dataset/box_coder.py:75-107
  *   fear_decode_smooth    FEARTracker._postprocess with smooth: true (penalty, window, size smoothing)
  *                         tracker/base_tracker.py:126-205
+ *   fear_track_sized / fear_track_sized_u8 / fear_forward_sized / fear_head_sized / fear_decode_sized /
+ *   fear_decode_smooth_sized   the same on search crops of side S (instance_size; score_size = S / 16)
  *   fear_pack_weights     load_from_lighting + nn.Module.load_state_dict  utils/torch.py:11-24
  *
  *   fear_head_update      BoxTower.forward(search, kernel, update)   blocks.py:174-179
@@ -352,6 +354,27 @@ int fear_get_features_u8(FearContext* h, const uint8_t* d_img_u8, int B, int H, 
 int fear_forward(FearContext* h, const float* d_template, const float* d_search, int B,
                  float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream);
 
+/* ---- search crops of any size -------------------------------------------------------
+ * The reference sets its search crop in config (siam_tracker.yaml instance_size / score_size); the network is fully
+ * convolutional.  These entry points take a square search of side S, a multiple of 16 in [16, 256] (the sizes
+ * fear_get_features takes), or the score-map side s = S / 16 in [1, 16] where only maps are involved.  Maps are
+ * (B,4,s,s) and (B,1,s,s); the decode grid is (i - s / 2) * 16 + S / 2 (utils/utils.py:183-199).  The template stays
+ * (B,3,128,128) / (Bz,256,8,8): its 64 cells are the 64 correlation channels of the checkpoint.  The entry points
+ * above are these at S = 256 (s = 16), with the same results bit for bit.  Batches larger than the reserved batch are
+ * chunked as above.  FEAR_EINVAL: S or s outside its range, plus the rules of the fixed-size entry point. */
+/* fear_head_update on search features xfeat (B,256,s,s); d_zupdate may be NULL (= fear_head). */
+int fear_head_sized(FearContext* h, const float* d_zfeat, int Bz, const float* d_zupdate, int Bu, const float* d_xfeat,
+                    int B, int s, float* d_bbox, float* d_cls, void* stream);
+/* fear_track on search (B,3,S,S). */
+int fear_track_sized(FearContext* h, const float* d_search, int S, const float* d_zfeat, int Bz, int B,
+                     float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream);
+/* fear_track_u8 on raw uint8 RGB crops (B,S,S,3). */
+int fear_track_sized_u8(FearContext* h, const uint8_t* d_search_u8, int S, const float* d_zfeat, int Bz, int B,
+                        float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream);
+/* fear_forward on template (B,3,128,128) + search (B,3,S,S). */
+int fear_forward_sized(FearContext* h, const float* d_template, const float* d_search, int S, int B,
+                       float* d_bbox, float* d_cls, FearBox* d_boxes, void* stream);
+
 /* Host pre-processing of the tracking loop on the device (get_extended_crop, reference
  * model_training/utils/utils.py:215-253 = context crop, constant-colour padding, cv2.resize(INTER_LINEAR) on uint8):
  * d_frame (H,W,3) uint8 RGB stays on the device; d_crop (out_size,out_size,3) uint8 is what fear_track_u8 /
@@ -491,6 +514,15 @@ int fear_decode(const float* d_bbox, const float* d_cls, int B, int apply_sigmoi
 int fear_decode_smooth(const float* d_bbox, const float* d_cls, int B, const double* d_prev_size,
                        const double* d_params, FearBox* d_boxes, void* stream);
 
+/* fear_decode / fear_decode_smooth on s x s maps, s in [1, 16] (a search of side S = 16 s): bbox (B,4,s,s), cls
+ * (B,1,s,s); the grid is (i - s / 2) * 16 + 8 s, row = flat / s, col = flat % s; d_params (3 + s * s) float64:
+ * penalty_k, window_influence, lr, then the s x s window row-major.  Same arithmetic and argmax rules; at s = 16 they
+ * are fear_decode / fear_decode_smooth.  FEAR_EINVAL: s outside [1, 16], plus the rules of the fixed-size forms. */
+int fear_decode_sized(const float* d_bbox, const float* d_cls, int B, int s, int apply_sigmoid, FearBox* d_boxes,
+                      void* stream);
+int fear_decode_smooth_sized(const float* d_bbox, const float* d_cls, int B, int s, const double* d_prev_size,
+                             const double* d_params, FearBox* d_boxes, void* stream);
+
 /* z (Bz,256,64), x (B,256,256)  [= (B,256,16,16)]  ->  out (B,320,256):
  * out[:, :256] = x ; out[b, 256+k, p] = sum_c z[b,c,k] * x[b,c,p].   (blocks.py:121-124)
  * Workspace-free compatibility form: a direct CUDA-core kernel on the reference layouts (one D2D copy + one launch). */
@@ -539,8 +571,8 @@ int fear_stage_ms(FearContext* h, int i, float* ms, int64_t* launches);
  * (as fear_get_features). */
 int fear_debug_backbone_prefix(FearContext* h, const float* d_img, int B, int H, int W, int nblocks,
                                float* d_out, void* stream);
-/* Debug: copy a head intermediate of the last fear_head / fear_track / fear_forward call as NCHW
- * (B,C,16,16): "search_features" | "cat_cls" | "cat_reg" (320 ch: encode output + correlation) |
+/* Debug: copy a head intermediate of the last fear_head / fear_track / fear_forward call (or its _sized form) as NCHW
+ * (B,C,s,s), s the score side of that call (16 for the fixed-size entry points): "search_features" | "cat_cls" | "cat_reg" (320 ch: encode output + correlation) |
  * "cls_dw" | "reg_dw" | "x_reg" | "cls_tower" (256 ch).  (BoxTower.forward's 3rd/4th outputs.) */
 int fear_debug_head_tensor(FearContext* h, const char* name, int B, float* d_out, void* stream);
 /* Debug: write `word` into every 32-bit word of the handle's workspace (every buffer fear_reserve allocated, the
