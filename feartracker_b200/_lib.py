@@ -54,6 +54,10 @@ assert YCBCR_HDR_DTYPE.itemsize == 104
 BAYER_DTYPE = np.dtype([("data", "<u8"), ("row_stride", "<i8"), ("H", "<i4"), ("W", "<i4"), ("pattern", "<i4"),
                         ("bits", "<i4"), ("shift", "<i4"), ("packing", "<i4")])
 assert BAYER_DTYPE.itemsize == 40
+# FearFrameMono: a single-channel frame (FearFrameBayer's containers), its gain control and the code range it uses
+MONO_DTYPE = np.dtype([("data", "<u8"), ("row_stride", "<i8"), ("H", "<i4"), ("W", "<i4"), ("bits", "<i4"),
+                       ("shift", "<i4"), ("packing", "<i4"), ("agc", "<i4"), ("lo", "<i4"), ("hi", "<i4")])
+assert MONO_DTYPE.itemsize == 48
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -98,6 +102,10 @@ _SIGNATURES = {
     "fear_crop_targets_bayer_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_bayer": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_bayer_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_frame_range_mono": (c_int, [c_void_p, c_int, c_void_p]),
+    "fear_crop_targets_mono_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_mono": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_mono_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_decode_smooth": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fear_head_sized": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,

@@ -1101,6 +1101,8 @@ static_assert(sizeof(FearFrameYCbCrHDR) == 104 && offsetof(FearFrameYCbCrHDR, v2
               "FearFrameYCbCrHDR layout is part of the ABI");
 static_assert(sizeof(FearFrameBayer) == 40 && offsetof(FearFrameBayer, packing) == 36,
               "FearFrameBayer layout is part of the ABI");
+static_assert(sizeof(FearFrameMono) == 48 && offsetof(FearFrameMono, agc) == 36 && offsetof(FearFrameMono, hi) == 44,
+              "FearFrameMono layout is part of the ABI");
 
 static int check_crop_targets_args(int F, int N, double offset, int out_size) {
   if (N < 1 || N > 65535) return set_err(FEAR_EINVAL, "target count must be in [1, 65535] (got %d)", N);
@@ -1298,6 +1300,32 @@ extern "C" int fear_advance_targets_bayer(const FearBox* d_boxes, const FearFram
 
 extern "C" int fear_frame_sums_bayer_u8(const FearFrameBayer* d_views, int F, uint64_t* d_sums, void* stream) {
   return launch_frame_sums(d_views, BayerFrames{d_views}, F, d_sums, stream);
+}
+
+// Single-channel frames: the range kernel for their gain control, then the same kernels reading through MonoFrames.
+extern "C" int fear_frame_range_mono(FearFrameMono* d_views, int F, void* stream) {
+  if (!d_views) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (F < 1 || F > 65535) return set_err(FEAR_EINVAL, "frame count must be in [1, 65535] (got %d)", F);
+  frame_range_mono_kernel<<<dim3(kFrameSumCtas, F), kFrameSumThreads, 0, (cudaStream_t)stream>>>(d_views);
+  return check_launch("frame_range_mono_kernel");
+}
+
+extern "C" int fear_crop_targets_mono_u8(const FearFrameMono* d_views, int F, FearTarget* d_targets, int N,
+                                         double offset, int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_views || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(MonoFrames{d_views}, F, d_targets, N, offset, out_size, d_crops, stream);
+}
+
+extern "C" int fear_advance_targets_mono(const FearBox* d_boxes, const FearFrameMono* d_views, int F,
+                                         FearTarget* d_targets, int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_views || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return launch_advance_targets(d_boxes, MonoFrames{d_views}, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_frame_sums_mono_u8(const FearFrameMono* d_views, int F, uint64_t* d_sums, void* stream) {
+  return launch_frame_sums(d_views, MonoFrames{d_views}, F, d_sums, stream);
 }
 
 extern "C" int fear_decode_sized(const float* d_bbox, const float* d_cls, int B, int side, int apply_sigmoid,

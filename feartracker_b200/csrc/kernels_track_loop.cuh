@@ -7,16 +7,19 @@
 //   advance_targets_kernel   decoded FearBox -> next frame-space box                  (image_ops.rescale_bbox +
 //                            image_ops.clamp_bbox)
 //   frame_sums_u8_kernel     exact per-channel sums of whole frames                    (np.mean of the padding colour)
+//   frame_range_mono_kernel  code range of single-channel frames, for their gain       (the smin, smax of
+//                                                                                       cv2.normalize(NORM_MINMAX))
 //
-// The three kernels are templates over where the frames are and what they hold: a packed buffer + FearFrame table
+// The first three are templates over where the frames are and what they hold: a packed buffer + FearFrame table
 // (PackedFrames) or a FearFrameView table of strided RGB frames anywhere in device memory (FrameViews), both read
 // through TrackFrame; or a table of YUV frames, FearFrameYUV420 (YUV420Frames, 4:2:0, 8-bit BT.601 limited range),
 // FearFrameYUV (YUVFrames, 4:2:0, the format named per entry) or FearFrameYCbCr (YCbCrFrames, 4:2:0, 4:2:2 or 4:4:4 and
 // the format named per entry), all read through YUVFrame, which converts each pixel it reads to RGB; or a table of
 // FearFrameYCbCrV210 records (YCbCrV210Frames), read through V210Frame, which also unpacks v210 surfaces; or a table of
 // FearFrameYCbCrHDR records (YCbCrHDRFrames), read through HDRFrame, which also tone-maps PQ and HLG video to SDR; or a
-// table of FearFrameBayer records (BayerFrames), read through BayerFrame, which demosaics raw Bayer mosaics.  A frame
-// type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables,
+// table of FearFrameBayer records (BayerFrames), read through BayerFrame, which demosaics raw Bayer mosaics; or a
+// table of FearFrameMono records (MonoFrames), read through MonoFrame, which maps single-channel codes to grey.  A
+// frame type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables,
 // interpolation, sums and the colour conversion exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
@@ -24,6 +27,7 @@
 // rounded intrinsics.
 #pragma once
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 
 #include "../../include/fear_b200.h"
@@ -419,6 +423,26 @@ struct YCbCrHDRFrames {
   }
 };
 
+// The code of pixel (y, x) of a frame of raw samples f (BayerFrame, MonoFrame: data, rs, packing, bits, shift, the
+// fields of FearFrameBayer / FearFrameMono): a byte, a masked uint16, or a MIPI RAW10 / RAW12 group's high byte and
+// low bits.
+template <class Raw>
+__device__ __forceinline__ int raw_code(const Raw& f, int y, int x) {
+  const uint8_t* row = f.data + (long long)y * f.rs;
+  if (f.packing == FEAR_BAYER_RAW10) {
+    const uint8_t* g = row + 5LL * (x >> 2);
+    const int i = x & 3;
+    return (__ldg(g + i) << 2) | ((__ldg(g + 4) >> (2 * i)) & 3);
+  }
+  if (f.packing == FEAR_BAYER_RAW12) {
+    const uint8_t* g = row + 3LL * (x >> 1);
+    const int i = x & 1;
+    return (__ldg(g + i) << 4) | ((__ldg(g + 2) >> (4 * i)) & 15);
+  }
+  if (f.bits == 8) return __ldg(row + x);
+  return (__ldg(reinterpret_cast<const uint16_t*>(row) + x) >> f.shift) & ((1 << f.bits) - 1);
+}
+
 // A raw Bayer mosaic (FearFrameBayer): rgb(y, x) demosaics the pixel as cv2.cvtColor(COLOR_Bayer*2RGB) does, from the
 // codes of its 3 x 3 neighbourhood in int32, with (y, x) clamped into [1, H - 2] x [1, W - 2] (cv2 copies the second and
 // second-last rows and columns over the border ones).  (ry, rx) is the R site of the 2 x 2 block at (0, 0), so pixel
@@ -433,21 +457,9 @@ struct BayerFrame {
   bool bad;
   double ys;
   __device__ __forceinline__ bool empty() const { return bad || data == nullptr || H < 3 || W < 3; }
-  // the code of pixel (y, x): a byte, a masked uint16, or a MIPI RAW10 / RAW12 group's high byte and low bits
+  // the code of pixel (y, x) in the entry's container
   __device__ __forceinline__ int code(int y, int x) const {
-    const uint8_t* row = data + (long long)y * rs;
-    if (packing == FEAR_BAYER_RAW10) {
-      const uint8_t* g = row + 5LL * (x >> 2);
-      const int i = x & 3;
-      return (__ldg(g + i) << 2) | ((__ldg(g + 4) >> (2 * i)) & 3);
-    }
-    if (packing == FEAR_BAYER_RAW12) {
-      const uint8_t* g = row + 3LL * (x >> 1);
-      const int i = x & 1;
-      return (__ldg(g + i) << 4) | ((__ldg(g + 2) >> (4 * i)) & 15);
-    }
-    if (bits == 8) return __ldg(row + x);
-    return (__ldg(reinterpret_cast<const uint16_t*>(row) + x) >> shift) & ((1 << bits) - 1);
+    return raw_code(*this, y, x);
   }
   __device__ __forceinline__ int to_u8(int v) const {
     return bits == 8 ? v : yuv_unit_to_u8(__dmul_rn((double)v, ys));
@@ -498,6 +510,74 @@ struct BayerFrames {
     return BayerFrame{static_cast<const uint8_t*>(v.data), v.row_stride, v.H, v.W, v.pattern >> 1, v.pattern & 1,
                       v.packing, v.bits, v.shift, !ok,
                       ok && v.bits != 8 ? __ddiv_rn(1.0, (double)((1 << v.bits) - 1)) : 0.0};
+  }
+};
+
+// A single-channel frame (FearFrameMono): rgb(y, x) is the grey triple (g, g, g) of the pixel's code, read as
+// BayerFrame reads one (raw_code).  Without gain control g is the code at 8 bits and above it the code mapped as
+// BayerFrame maps a channel; with `agc` it is cv2.normalize(NORM_MINMAX, CV_8U)'s rint(fma(v, a, b)) with the float32
+// gain a and offset b that MonoFrames derives from the frame's range.  `bad` marks an entry the kernels cannot read.
+// A value-initialised MonoFrame{} is empty.
+struct MonoFrame {
+  const uint8_t* data;
+  long long rs;
+  int H, W;
+  int packing, bits, shift;
+  bool bad, agc;
+  double ys;
+  float a, b;
+  __device__ __forceinline__ bool empty() const { return bad || data == nullptr || H < 1 || W < 1; }
+  __device__ __forceinline__ int code(int y, int x) const {
+    return raw_code(*this, y, x);
+  }
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    const int v = code(y, x);
+    int g;
+    if (agc) g = min(max(__float2int_rn(__fmaf_rn(__int2float_rn(v), a, b)), 0), 255);
+    else g = bits == 8 ? v : yuv_unit_to_u8(__dmul_rn((double)v, ys));
+    p[0] = p[1] = p[2] = g;
+  }
+};
+
+// Frame i of a FearFrameMono table (the *_mono entry points), checked per entry against FearFrameMono's rules, with
+// the gain of its lo / hi when agc is set: scale = 255 * (1 / (hi - lo)) (0 unless hi > lo) and shift = 0 - lo * scale
+// in float64, rounded to float32, as cv2.normalize(NORM_MINMAX) derives them for convertTo.
+struct MonoFrames {
+  const FearFrameMono* views;
+  // the entry without its gain (the range kernel, which writes lo and hi, reads only these fields); the container
+  // rules are FearFrameBayer's, restated from BayerFrames (whose kernels are left to compile as they do)
+  static __device__ __forceinline__ MonoFrame unscaled(const FearFrameMono* p) {
+    const void* data = p->data;
+    const long long rs = p->row_stride;
+    const int H = p->H, W = p->W, bits = p->bits, shift = p->shift, packing = p->packing, agc = p->agc;
+    const long long w = W;
+    const bool wide = packing == FEAR_BAYER_UNPACKED && bits != 8;
+    const long long row_bytes = packing == FEAR_BAYER_RAW10   ? 5 * ((w + 3) / 4)
+                                : packing == FEAR_BAYER_RAW12 ? 3 * ((w + 1) / 2)
+                                                              : (wide ? 2 : 1) * w;
+    bool ok;
+    if (packing == FEAR_BAYER_RAW10) ok = bits == 10;
+    else if (packing == FEAR_BAYER_RAW12) ok = bits == 12;
+    else if (packing == FEAR_BAYER_UNPACKED)
+      ok = bits == 8 ? shift == 0
+                     : (bits == 10 || bits == 12 || bits == 14 || bits == 16) && shift >= 0 && shift <= 16 - bits &&
+                           !(((uintptr_t)data | (uintptr_t)rs) & 1);
+    else ok = false;
+    ok = ok && (agc == 0 || agc == FEAR_AGC_MINMAX) && rs >= row_bytes;
+    return MonoFrame{static_cast<const uint8_t*>(data), rs, H, W, packing, bits, shift, !ok, agc != 0,
+                     ok && bits != 8 ? __ddiv_rn(1.0, (double)((1 << bits) - 1)) : 0.0, 0.f, 0.f};
+  }
+  __device__ __forceinline__ MonoFrame operator()(int i) const {
+    MonoFrame f = unscaled(views + i);
+    if (f.agc && !f.bad) {
+      const double lo = (double)views[i].lo, hi = (double)views[i].hi;
+      const double d = __dsub_rn(hi, lo);
+      const double scale = __dmul_rn(255.0, d > 0x1p-52 ? __ddiv_rn(1.0, d) : 0.0);
+      const double shift = __dsub_rn(0.0, __dmul_rn(lo, scale));
+      f.a = __double2float_rn(scale);
+      f.b = __double2float_rn(shift);
+    }
+    return f;
   }
 };
 
@@ -696,6 +776,51 @@ __global__ void __launch_bounds__(kFrameSumThreads) frame_sums_u8_kernel(Frames 
 #pragma unroll
     for (int w = 0; w < kFrameSumThreads / 32; ++w) v += part[threadIdx.x][w];
     atomicAdd(sums + 3LL * blockIdx.y + threadIdx.x, v);
+  }
+}
+
+// grid (kFrameSumCtas, F), kFrameSumThreads threads: the code range of FearFrameMono entry f with agc set, over the
+// pixels CTA (g, f) visits (frame_sums_u8_kernel's grid-stride walk), reduced per warp and per CTA, then one atomicMin
+// on the entry's lo and one atomicMax on its hi.  Min and max in any order are the same, so the result is
+// deterministic.  Entries without agc and entries the kernels cannot read are not touched.
+__global__ void __launch_bounds__(kFrameSumThreads) frame_range_mono_kernel(FearFrameMono* views) {
+  __shared__ int part[2][kFrameSumThreads / 32];
+  FearFrameMono* p = views + blockIdx.y;
+  const MonoFrame fr = MonoFrames::unscaled(p);
+  if (fr.empty() || !fr.agc) return;
+  const long long W = fr.W, stride = (long long)gridDim.x * blockDim.x;
+  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long sy = stride / W, sx = stride - sy * W;
+  int lo = INT_MAX, hi = INT_MIN;
+  for (long long y = i0 / W, x = i0 - y * W; y < fr.H;) {
+    const int v = fr.code((int)y, (int)x);
+    lo = min(lo, v);
+    hi = max(hi, v);
+    x += sx;
+    y += sy;
+    if (x >= W) {
+      x -= W;
+      ++y;
+    }
+  }
+  lo = __reduce_min_sync(0xffffffffu, lo);
+  hi = __reduce_max_sync(0xffffffffu, hi);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) {
+    part[0][warp] = lo;
+    part[1][warp] = hi;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int w = 1; w < kFrameSumThreads / 32; ++w) {
+      lo = min(lo, part[0][w]);
+      hi = max(hi, part[1][w]);
+    }
+    if (lo <= hi) {  // a CTA that visited no pixel has nothing to add
+      atomicMin(&p->lo, lo);
+      atomicMax(&p->hi, hi);
+    }
   }
 }
 

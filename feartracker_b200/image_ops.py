@@ -509,18 +509,28 @@ def bayer_to_rgb(codes: np.ndarray, pattern: str = "RGGB", bits: int = 8) -> np.
     else uint16 codes in [0, 2^bits - 1], already unpacked and masked): ``bayer_demosaic`` at the codes' depth, then,
     above 8 bits, each channel value v mapped as full-range luma is, min(max(rint(255 * (v * (1 / (2^bits - 1)))), 0),
     255) in float64 (``yuv_to_rgb(v, c, c, full_range=True, bits=bits)`` at neutral chroma c = 2^(bits - 1))."""
+    return raw_to_u8(bayer_demosaic(_raw_codes(codes, bits, "Bayer"), pattern), bits)
+
+
+def _raw_codes(codes, bits: int, what: str) -> np.ndarray:
+    """``codes`` as an array, checked to be ``bits``-bit codes: uint8 at 8 bits, else uint16 below 2^bits."""
     if isinstance(bits, bool) or bits not in (8, 10, 12, 14, 16):
-        raise ValueError(f"Bayer bits must be 8, 10, 12, 14 or 16, got {bits!r}")
+        raise ValueError(f"{what} bits must be 8, 10, 12, 14 or 16, got {bits!r}")
     a = np.asarray(codes)
     if a.dtype != (np.uint8 if bits == 8 else np.uint16):
-        raise ValueError(f"{bits}-bit Bayer codes must be {'uint8' if bits == 8 else 'uint16'}, got {a.dtype}")
+        raise ValueError(f"{bits}-bit {what} codes must be {'uint8' if bits == 8 else 'uint16'}, got {a.dtype}")
     if bits < 16 and a.size and int(a.max()) >= 1 << bits:
-        raise ValueError(f"{bits}-bit Bayer codes must be below {1 << bits}, got {int(a.max())}")
-    rgb = bayer_demosaic(a, pattern)
+        raise ValueError(f"{bits}-bit {what} codes must be below {1 << bits}, got {int(a.max())}")
+    return a
+
+
+def raw_to_u8(v: np.ndarray, bits: int) -> np.ndarray:
+    """``bits``-bit values v as uint8: v itself at 8 bits, above that min(max(rint(255 * (v * (1 / (2^bits - 1)))), 0),
+    255) in float64, as full-range luma is mapped."""
     if bits == 8:
-        return rgb
+        return v
     ys = 1.0 / float((1 << bits) - 1)
-    return np.clip(np.rint(255.0 * (rgb.astype(np.float64) * ys)), 0, 255).astype(np.uint8)
+    return np.clip(np.rint(255.0 * (v.astype(np.float64) * ys)), 0, 255).astype(np.uint8)
 
 
 def mipi_row_bytes(width: int, bits: int) -> int:
@@ -578,3 +588,62 @@ def mipi_pack(codes: np.ndarray, bits: int, pitch: Optional[int] = None) -> np.n
     out = np.zeros((h, pitch), dtype=np.uint8)
     out[:, :need] = g.reshape(h, need)
     return out
+
+
+# FearFrameMono's gain control: None -> 0, "minmax" -> FEAR_AGC_MINMAX
+AGC_MODES = {None: 0, "minmax": 1}
+
+
+def check_agc(agc, what: str = "agc") -> None:
+    if not isinstance(agc, (str, type(None))) or agc not in AGC_MODES:
+        raise ValueError(f"{what} must be None or \"minmax\", got {agc!r}")
+
+
+def fma_f32(v: np.ndarray, a: np.float32, b: np.float32) -> np.ndarray:
+    """float32 fmaf(v, a, b) elementwise, rounded once (v integers below 2^24, a and b float32): v * a is exact in
+    float64; the float64 sum s and its exact error e (TwoSum) fix the one case where rounding s to float32 differs from
+    rounding v * a + b, an s that lies on a float32 midpoint while e != 0."""
+    p = np.asarray(v).astype(np.float64) * np.float64(a)
+    b64 = np.float64(b)
+    s = p + b64
+    bb = s - p
+    e = (p - (s - bb)) + (b64 - bb)
+    r = s.astype(np.float32)
+    toward = np.nextafter(r, np.where(e > 0, np.float32(np.inf), np.float32(-np.inf)).astype(np.float32))
+    tie = (e != 0) & ((r.astype(np.float64) + toward.astype(np.float64)) * 0.5 == s)
+    return np.where(tie, toward, r)
+
+
+def minmax_gain(lo: int, hi: int):
+    """The float32 (a, b) that cv2.normalize(src, None, 0, 255, NORM_MINMAX, CV_8U) passes to convertTo for codes in
+    [lo, hi]: OpenCV 4.13 computes scale = (dmax - dmin) * (smax - smin > DBL_EPSILON ? 1 / (smax - smin) : 0) and
+    shift = dmin - smin * scale in float64 (dmin = 0, dmax = 255), and convertTo to uint8 takes them as float."""
+    d = float(hi) - float(lo)
+    scale = 255.0 * (1.0 / d if d > np.finfo(np.float64).eps else 0.0)
+    shift = 0.0 - float(lo) * scale
+    return np.float32(scale), np.float32(shift)
+
+
+def minmax_normalize(codes: np.ndarray) -> np.ndarray:
+    """cv2.normalize(codes, None, 0, 255, cv2.NORM_MINMAX, dtype=cv2.CV_8U) of uint8 or uint16 codes, bit for bit:
+    with lo, hi the smallest and largest code and (a, b) = ``minmax_gain(lo, hi)``, each code v becomes
+    saturate_cast<uchar>(fmaf(v, a, b)) = min(max(rint(fmaf(v, a, b)), 0), 255).  A constant frame gives 0."""
+    a = np.asarray(codes)
+    if a.size == 0:
+        return np.zeros(a.shape, np.uint8)
+    ga, gb = minmax_gain(int(a.min()), int(a.max()))
+    return np.clip(np.rint(fma_f32(a, ga, gb)), 0, 255).astype(np.uint8)
+
+
+def mono_to_rgb(codes: np.ndarray, bits: int = 8, agc: Optional[str] = None) -> np.ndarray:
+    """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for a single-channel frame of ``bits``-bit codes (uint8 at 8
+    bits, else uint16 codes in [0, 2^bits - 1], already unpacked and shifted: ``mipi_unpack`` for packed rows):
+    ``cv2.cvtColor(g, cv2.COLOR_GRAY2RGB)`` of the 8-bit grey image g.  Without gain control g is the code at 8 bits,
+    above it the code mapped as ``bayer_to_rgb`` maps a channel; with ``agc="minmax"`` g is ``minmax_normalize`` of the
+    whole frame's codes, cv2.normalize(codes, None, 0, 255, NORM_MINMAX, CV_8U)."""
+    check_agc(agc)
+    a = _raw_codes(codes, bits, "mono")
+    if a.ndim != 2:
+        raise ValueError(f"mono codes must be a 2-D (H, W) array, got shape {a.shape}")
+    g = minmax_normalize(a) if agc == "minmax" else raw_to_u8(a, bits)
+    return np.repeat(g[..., None], 3, axis=-1)

@@ -13,7 +13,10 @@ BT.601, BT.709 or BT.2020, limited or full range, 8, 10 or 12 bits, converted to
 limited range exactly as cv2.cvtColor converts it), and V210Frame (SDI capture cards' packed 10-bit 4:2:2, unpacked
 inside the crop); or raw Bayer mosaics as machine-vision and CSI-2 cameras send them: BayerFrame (RGGB / GRBG / GBRG /
 BGGR at 8 to 16 bits, MIPI RAW10 / RAW12), demosaiced inside the crop exactly as cv2.cvtColor(COLOR_Bayer*2RGB)
-demosaics them.  Tensors, YUV planes, v210 surfaces and Bayer mosaics are read where they are, without a copy.
+demosaics them; or single-channel frames as mono cameras and thermal cores send them: MonoFrame (8 to 16 bits, MIPI
+RAW10 / RAW12), mapped to grey inside the crop, optionally with per-frame min-max gain control (cv2.normalize
+NORM_MINMAX).  Tensors, YUV planes, v210 surfaces, Bayer mosaics and mono frames are read where they are, without a
+copy.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -33,8 +36,11 @@ V210Frame puts all its frames into a fourth, of FearFrameYCbCrV210 records (a Fe
 by the *_ycbcr_v210 entry points; a call with any HDR frame (``transfer="pq"`` or ``"hlg"``) puts all its frames into
 a sixth, of FearFrameYCbCrHDR records (a FearFrameYCbCrV210 and its transfer), read by the *_ycbcr_hdr entry points,
 which tone-map HDR taps to SDR inside the crop.  BayerFrames go into a fifth, of FearFrameBayer records, read by the *_bayer entry
-points; they cannot share a call with other kinds of frames.  The host then reads back the boxes and scores.  The
-launch count of a step depends neither on N nor on the kind of frames.
+points; they cannot share a call with other kinds of frames.  MonoFrames go into a seventh, of FearFrameMono records,
+read by the *_mono entry points, and cannot share a call with other kinds either; when any of a call's MonoFrames has
+gain control, fear_frame_range_mono first writes each frame's code range into that table.  The host then reads back
+the boxes and scores.  The launch count of a step depends neither on N nor on the kind of frames, with one exception:
+a step on MonoFrames with gain control launches the range kernel too (49 launches instead of 48).
 """
 import math
 import warnings
@@ -56,9 +62,13 @@ ENTRY_POINTS = {
                    "fear_advance_targets_ycbcr_v210"),
     "ycbcr_hdr": ("fear_frame_sums_ycbcr_hdr_u8", "fear_crop_targets_ycbcr_hdr_u8", "fear_advance_targets_ycbcr_hdr"),
     "bayer": ("fear_frame_sums_bayer_u8", "fear_crop_targets_bayer_u8", "fear_advance_targets_bayer"),
+    "mono": ("fear_frame_sums_mono_u8", "fear_crop_targets_mono_u8", "fear_advance_targets_mono"),
 }
 TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE,
-                "ycbcr_v210": _lib.YCBCR_V210_DTYPE, "ycbcr_hdr": _lib.YCBCR_HDR_DTYPE, "bayer": _lib.BAYER_DTYPE}
+                "ycbcr_v210": _lib.YCBCR_V210_DTYPE, "ycbcr_hdr": _lib.YCBCR_HDR_DTYPE, "bayer": _lib.BAYER_DTYPE,
+                "mono": _lib.MONO_DTYPE}
+# the entry point that writes each frame's code range into a FearFrameMono table, for min-max gain control
+RANGE_ENTRY_POINT = "fear_frame_range_mono"
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -375,7 +385,59 @@ class V210Frame:
         return self.ycbcr_v210_record() + (image_ops.HDR_TRANSFERS.get(self.transfer, 0), 0)
 
 
-class BayerFrame:
+class _RawFrame:
+    """What BayerFrame and MonoFrame share: a CUDA (H, W) tensor of unpacked samples, or an (H, row bytes) uint8 tensor
+    of MIPI CSI-2 RAW10 / RAW12 rows, with its checks and row pitch.  ``_MIN_SIDE`` is the smallest H and W the kernels
+    read and ``_SIZE_MSG`` names the frame in the size refusal."""
+    _MIN_SIDE = 1
+    _SIZE_MSG = "a frame needs at least 1 row and 1 column"
+
+    @classmethod
+    def _check_depth(cls, bits, msb) -> torch.dtype:
+        if isinstance(bits, bool) or bits not in (8, 10, 12, 14, 16):
+            raise ValueError(f"{cls.__name__} bits must be 8, 10, 12, 14 or 16, got {bits!r}")
+        if bits == 8 and msb:
+            raise ValueError(f"{cls.__name__} msb applies to samples wider than 8 bits, not 8-bit ones")
+        return torch.uint8 if bits == 8 else torch.uint16
+
+    @classmethod
+    def _check_tensor(cls, t, dtype: torch.dtype, what: str) -> None:
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.ndim != 2 or t.device.type != "cuda":
+            got = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"{cls.__name__} takes a 2-D CUDA {dtype} {what}, got {got}")
+        m = cls._MIN_SIDE
+        if not (m <= t.shape[0] <= _MAX_SIDE and m <= t.shape[1] <= _MAX_SIDE):
+            raise ValueError(f"{cls._SIZE_MSG}, got {tuple(t.shape)}")
+
+    @classmethod
+    def _check_packed(cls, t, width, bits: int) -> int:
+        """The row bytes of RAW``bits`` rows of ``width`` pixels, after checking ``t`` and ``width``."""
+        cls._check_tensor(t, torch.uint8, f"(H, row bytes) tensor of RAW{bits} rows")
+        m = cls._MIN_SIDE
+        if isinstance(width, bool) or not isinstance(width, (int, np.integer)) or not (m <= width <= _MAX_SIDE):
+            raise ValueError(f"{cls.__name__} width must be an int in [{m}, {_MAX_SIDE}], got {width!r}")
+        need = image_ops.mipi_row_bytes(width, bits)
+        if t.shape[1] < need:
+            raise ValueError(f"a RAW{bits} row of {width} pixels needs {need} bytes, the tensor's rows have "
+                             f"{t.shape[1]}")
+        return need
+
+    def _init(self, t: torch.Tensor, bits: int, shift: int, packing: int, width: int, row_bytes: int) -> None:
+        name = type(self).__name__
+        es = t.element_size()
+        pitch = t.stride(0) * es
+        if t.stride(1) != 1 or pitch < row_bytes:
+            raise ValueError(f"{name} rows must be contiguous samples at a pitch of at least {row_bytes} bytes, "
+                             f"got strides {t.stride()}")
+        if es == 2 and (pitch % 2 or t.data_ptr() % 2):
+            raise ValueError(f"{name} uint16 rows must start on 2-byte boundaries: pitch {pitch}, address offset "
+                             f"{t.data_ptr() % 2}")
+        self.t, self.bits, self.shift, self.packing = t, bits, shift, packing
+        self.pitch = int(pitch)
+        self.shape = (t.shape[0], width, 3)
+
+
+class BayerFrame(_RawFrame):
     """A raw Bayer mosaic as machine-vision cameras (GigE Vision / USB3 Vision PFNC ``BayerRG8``, ``BayerGR12`` ...),
     CSI-2 sensors under V4L2 or libcamera (``SRGGB10P`` / ``SRGGB12P``) and raw recorders deliver it.  ``pattern`` is
     the colours of the 2 x 2 block at pixel (0, 0), row by row: "RGGB", "GRBG", "GBRG" or "BGGR" (OpenCV 4.x's
@@ -393,16 +455,15 @@ class BayerFrame:
     pattern, bits)`` of the frame's codes (``image_ops.mipi_unpack`` for packed rows), which is ``cv2.cvtColor(raw,
     cv2.COLOR_Bayer{pattern}2RGB)`` at 8 bits.  The constructors raise ValueError on a malformed tensor or format.
     ``shape`` is (H, W, 3)."""
+    _MIN_SIDE = 3
+    _SIZE_MSG = "a Bayer mosaic needs at least 3 rows and 3 columns"
 
     def __init__(self, t: torch.Tensor, pattern: str = "RGGB", bits: int = 8, msb: bool = False) -> None:
         self._check_pattern(pattern)
-        if isinstance(bits, bool) or bits not in (8, 10, 12, 14, 16):
-            raise ValueError(f"BayerFrame bits must be 8, 10, 12, 14 or 16, got {bits!r}")
-        if bits == 8 and msb:
-            raise ValueError("BayerFrame msb applies to samples wider than 8 bits, not 8-bit ones")
-        dtype = torch.uint8 if bits == 8 else torch.uint16
+        dtype = self._check_depth(bits, msb)
         self._check_tensor(t, dtype, f"(H, W) tensor at {bits} bits")
-        self._init(t, pattern, int(bits), 16 - int(bits) if msb else 0, 0, t.shape[1], t.shape[1] * t.element_size())
+        self._init(t, int(bits), 16 - int(bits) if msb else 0, 0, t.shape[1], t.shape[1] * t.element_size())
+        self.pattern = pattern
 
     @classmethod
     def raw10(cls, t: torch.Tensor, width: int, pattern: str = "RGGB") -> "BayerFrame":
@@ -415,43 +476,16 @@ class BayerFrame:
     @classmethod
     def _packed(cls, t, width, pattern, bits: int, packing: int) -> "BayerFrame":
         cls._check_pattern(pattern)
-        cls._check_tensor(t, torch.uint8, f"(H, row bytes) tensor of RAW{bits} rows")
-        if isinstance(width, bool) or not isinstance(width, (int, np.integer)) or not (3 <= width <= _MAX_SIDE):
-            raise ValueError(f"BayerFrame width must be an int in [3, {_MAX_SIDE}], got {width!r}")
-        need = image_ops.mipi_row_bytes(width, bits)
-        if t.shape[1] < need:
-            raise ValueError(f"a RAW{bits} row of {width} pixels needs {need} bytes, the tensor's rows have "
-                             f"{t.shape[1]}")
+        need = cls._check_packed(t, width, bits)
         f = cls.__new__(cls)
-        f._init(t, pattern, bits, 0, packing, int(width), need)
+        f._init(t, bits, 0, packing, int(width), need)
+        f.pattern = pattern
         return f
 
     @staticmethod
     def _check_pattern(pattern) -> None:
         if pattern not in image_ops.BAYER_PATTERNS:
             raise ValueError(f"BayerFrame pattern must be one of {sorted(image_ops.BAYER_PATTERNS)}, got {pattern!r}")
-
-    @staticmethod
-    def _check_tensor(t, dtype: torch.dtype, what: str) -> None:
-        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.ndim != 2 or t.device.type != "cuda":
-            got = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
-            raise ValueError(f"BayerFrame takes a 2-D CUDA {dtype} {what}, got {got}")
-        if not (3 <= t.shape[0] <= _MAX_SIDE and 3 <= t.shape[1] <= _MAX_SIDE):
-            raise ValueError(f"a Bayer mosaic needs at least 3 rows and 3 columns, got {tuple(t.shape)}")
-
-    def _init(self, t: torch.Tensor, pattern: str, bits: int, shift: int, packing: int, width: int,
-              row_bytes: int) -> None:
-        es = t.element_size()
-        pitch = t.stride(0) * es
-        if t.stride(1) != 1 or pitch < row_bytes:
-            raise ValueError(f"BayerFrame rows must be contiguous samples at a pitch of at least {row_bytes} bytes, "
-                             f"got strides {t.stride()}")
-        if es == 2 and (pitch % 2 or t.data_ptr() % 2):
-            raise ValueError(f"BayerFrame uint16 rows must start on 2-byte boundaries: pitch {pitch}, address offset "
-                             f"{t.data_ptr() % 2}")
-        self.t, self.pattern, self.bits, self.shift, self.packing = t, pattern, bits, shift, packing
-        self.pitch = int(pitch)
-        self.shape = (t.shape[0], width, 3)
 
     def bayer_record(self) -> tuple:
         """The FearFrameBayer record (data, row_stride, H, W, pattern, bits, shift, packing): the address of sample
@@ -460,13 +494,68 @@ class BayerFrame:
                 self.shift, self.packing)
 
 
+class MonoFrame(_RawFrame):
+    """A single-channel frame as mono machine-vision cameras (GigE Vision / USB3 Vision PFNC ``Mono8``, ``Mono10``,
+    ``Mono12``, ``Mono16``), mono CSI-2 sensors under V4L2 (``GREY``, ``Y10``, ``Y12``, ``Y16``, ``Y10P``, ``Y12P``)
+    and thermal cores (14- or 16-bit ``Y16``) deliver it.
+
+        MonoFrame(t, bits=8, msb=False, agc=None)   t a CUDA (H, W) tensor: uint8 at 8 bits, torch.uint16 at 10, 12,
+                                                    14 or 16 bits, the code in the low bits (``msb=False``) or the
+                                                    high bits (``msb=True``) of each sample; any row stride, column
+                                                    stride 1 (a view ``surface[:, :W]`` of a pitched surface is fine)
+        MonoFrame.raw10(t, width, agc=None)         t a CUDA uint8 (H, row bytes) tensor of MIPI CSI-2 RAW10 rows (Y10P)
+        MonoFrame.raw12(t, width, agc=None)         t a CUDA uint8 (H, row bytes) tensor of MIPI CSI-2 RAW12 rows (Y12P)
+
+    ``agc`` is the gain control: None maps each code to 8 bits as a BayerFrame channel is mapped; ``"minmax"`` stretches
+    the frame's own code range to [0, 255] as ``cv2.normalize(codes, None, 0, 255, cv2.NORM_MINMAX, cv2.CV_8U)`` does,
+    which a thermal core's narrow band of codes needs.  FEARMultiTracker and FEARTracker read the samples where they are
+    (with ``agc`` they first find the frame's range with one pass over it) and map every pixel they read to grey, so no
+    RGB copy is made: the RGB frame the tracker sees is ``image_ops.mono_to_rgb(codes, bits, agc)`` of the frame's codes
+    (``image_ops.mipi_unpack`` for packed rows).  The constructors raise ValueError on a malformed tensor or format.
+    ``shape`` is (H, W, 3)."""
+    _SIZE_MSG = "a mono frame needs at least 1 row and 1 column"
+
+    def __init__(self, t: torch.Tensor, bits: int = 8, msb: bool = False, agc: Optional[str] = None) -> None:
+        image_ops.check_agc(agc, "MonoFrame agc")
+        dtype = self._check_depth(bits, msb)
+        self._check_tensor(t, dtype, f"(H, W) tensor at {bits} bits")
+        self._init(t, int(bits), 16 - int(bits) if msb else 0, 0, t.shape[1], t.shape[1] * t.element_size())
+        self.agc = agc
+
+    @classmethod
+    def raw10(cls, t: torch.Tensor, width: int, agc: Optional[str] = None) -> "MonoFrame":
+        return cls._packed(t, width, agc, 10, 1)
+
+    @classmethod
+    def raw12(cls, t: torch.Tensor, width: int, agc: Optional[str] = None) -> "MonoFrame":
+        return cls._packed(t, width, agc, 12, 2)
+
+    @classmethod
+    def _packed(cls, t, width, agc, bits: int, packing: int) -> "MonoFrame":
+        image_ops.check_agc(agc, "MonoFrame agc")
+        need = cls._check_packed(t, width, bits)
+        f = cls.__new__(cls)
+        f._init(t, bits, 0, packing, int(width), need)
+        f.agc = agc
+        return f
+
+    def mono_record(self) -> tuple:
+        """The FearFrameMono record (data, row_stride, H, W, bits, shift, packing, agc, lo, hi): the address of sample
+        (0, 0) (packed: of row 0's first byte), the row pitch in bytes, the size, the format and the gain control, then
+        the empty range lo = INT32_MAX, hi = INT32_MIN that fear_frame_range_mono narrows to the frame's."""
+        return (self.t.data_ptr(), self.pitch, *self.shape[:2], self.bits, self.shift, self.packing,
+                image_ops.AGC_MODES[self.agc], 2 ** 31 - 1, -2 ** 31)
+
+
 def frame_kind(frame) -> str:
-    """"yuv" for a YUV420Frame, YUV422Frame, YUV444Frame or V210Frame, "bayer" for a BayerFrame, "cuda" for a torch
-    tensor (checked by ``check_device_frame``), "numpy" for anything else."""
+    """"yuv" for a YUV420Frame, YUV422Frame, YUV444Frame or V210Frame, "bayer" for a BayerFrame, "mono" for a
+    MonoFrame, "cuda" for a torch tensor (checked by ``check_device_frame``), "numpy" for anything else."""
     if isinstance(frame, (_YUVFrame, V210Frame)):
         return "yuv"
     if isinstance(frame, BayerFrame):
         return "bayer"
+    if isinstance(frame, MonoFrame):
+        return "mono"
     return "cuda" if isinstance(frame, torch.Tensor) else "numpy"
 
 
@@ -492,9 +581,16 @@ def check_tensor_frame(i: int, f: torch.Tensor, device) -> None:
     check_device(i, device, f)
 
 
+def uses_agc(frames, kind: str) -> bool:
+    """Whether any of a call's frames of kind ``kind`` is a MonoFrame with gain control: its table needs
+    fear_frame_range_mono before the sums or the crop read it."""
+    return kind == "mono" and any(f.agc is not None for f in frames)
+
+
 def check_device_frame(i: int, f, kind: str, device) -> None:
-    """The checks of a frame of kind "cuda", "yuv" or "bayer" (``frame_kind``): ValueError before any device call."""
-    if kind == "bayer":
+    """The checks of a frame of kind "cuda", "yuv", "bayer" or "mono" (``frame_kind``): ValueError before any device
+    call."""
+    if kind in ("bayer", "mono"):
         check_device(i, device, f.t)
     elif kind == "yuv":
         check_device(i, device, *((f.t,) if isinstance(f, V210Frame) else (f.y, f.u, f.v)))
@@ -505,7 +601,8 @@ def check_device_frame(i: int, f, kind: str, device) -> None:
 def write_records(table: np.ndarray, frames, name: str) -> None:
     """Write the records of device frames into rows of ``table`` (a numpy view of ``TABLE_DTYPES[name]``):
     FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr",
-    FearFrameYCbCrV210 for "ycbcr_v210", FearFrameYCbCrHDR for "ycbcr_hdr", FearFrameBayer for "bayer"."""
+    FearFrameYCbCrV210 for "ycbcr_v210", FearFrameYCbCrHDR for "ycbcr_hdr", FearFrameBayer for "bayer", FearFrameMono
+    for "mono"."""
     for i, f in enumerate(frames):
         if name == "yuv":
             table[i] = f.yuv_record()
@@ -517,6 +614,8 @@ def write_records(table: np.ndarray, frames, name: str) -> None:
             table[i] = f.hdr_record()
         elif name == "bayer":
             table[i] = f.bayer_record()
+        elif name == "mono":
+            table[i] = f.mono_record()
         else:
             table[i] = frame_view(f)
 
@@ -578,9 +677,9 @@ class FEARMultiTracker:
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
         ``frames`` are all numpy arrays, all CUDA tensors, all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame,
-        V210Frame) or all BayerFrames (see ``update``).  A target's padding colour is the mean colour of its frame (of
-        the converted RGB frame for a YUV frame, of the demosaiced 8-bit frame for a Bayer frame), from exact
-        per-channel sums computed on the device."""
+        V210Frame), all BayerFrames or all MonoFrames (see ``update``).  A target's padding colour is the mean colour of
+        its frame (of the converted RGB frame for a YUV frame, of the demosaiced 8-bit frame for a Bayer frame, of the
+        grey frame after gain control for a mono frame), from exact per-channel sums computed on the device."""
         frames, kind = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
         if rects.ndim == 1 and rects.size == 4:
@@ -611,6 +710,9 @@ class FEARMultiTracker:
             sums_fn, crop_fn, _ = ENTRY_POINTS[table]
             lib = _lib.load()
             stream = torch.cuda.current_stream(dev)
+            if uses_agc(frames, kind):
+                _lib.check(getattr(lib, RANGE_ENTRY_POINT)(b[table].data_ptr(), num_frames, stream.cuda_stream),
+                           RANGE_ENTRY_POINT)
             _lib.check(getattr(lib, sums_fn)(b[table].data_ptr(), num_frames, b["sums"].data_ptr(), stream.cuda_stream),
                        sums_fn)
             b["sums_pin"][:num_frames].copy_(b["sums"][:num_frames], non_blocking=True)
@@ -664,7 +766,9 @@ class FEARMultiTracker:
         words are read in place as well and give what its ``image_ops.v210_unpack`` planes give at 10 bits, 4:2:2.
         Frames of one call may have different colour formats and subsamplings.  ``frames`` may also be all
         ``BayerFrame``s (any patterns, depths and packings), never mixed with other kinds; their samples are read in
-        place and give exactly what ``image_ops.bayer_to_rgb`` of their codes gives as numpy arrays.  Device frames must
+        place and give exactly what ``image_ops.bayer_to_rgb`` of their codes gives as numpy arrays.  ``frames`` may
+        also be all ``MonoFrame``s (any depths, packings and gain controls), never mixed with other kinds; they give
+        exactly what ``image_ops.mono_to_rgb`` of their codes gives as numpy arrays.  Device frames must
         be ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
@@ -679,7 +783,7 @@ class FEARMultiTracker:
         with torch.cuda.device(dev):
             b = self._buffers(dev)
             table = self._upload_frames(frames, kind, dev)
-            boxes = self._run_step(n, len(frames), table, dev)
+            boxes = self._run_step(n, len(frames), table, dev, uses_agc(frames, kind))
             b["state_pin"][:n].copy_(b["state"][:n], non_blocking=True)
             b["box_pin"][:n].copy_(boxes, non_blocking=True)
             torch.cuda.current_stream(dev).synchronize()
@@ -699,9 +803,9 @@ class FEARMultiTracker:
         return torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
 
     def _check_frames(self, frames):
-        """-> (list of frames, their kind: "numpy", "cuda", "yuv" or "bayer").  Raises ValueError before any device
-        call."""
-        if isinstance(frames, (_YUVFrame, V210Frame, BayerFrame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
+        """-> (list of frames, their kind: "numpy", "cuda", "yuv", "bayer" or "mono").  Raises ValueError before any
+        device call."""
+        if isinstance(frames, (_YUVFrame, V210Frame, _RawFrame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
                                                           and frames.ndim == 3):
             frames = [frames]
         frames = list(frames)
@@ -712,6 +816,9 @@ class FEARMultiTracker:
             if any(frame_kind(f) == "bayer" for f in frames):
                 raise ValueError("BayerFrames cannot share a call with other kinds of frames (numpy arrays, CUDA "
                                  "tensors, YUV frames): pass all of a call's frames as BayerFrames")
+            if any(frame_kind(f) == "mono" for f in frames):
+                raise ValueError("MonoFrames cannot share a call with other kinds of frames (numpy arrays, CUDA "
+                                 "tensors, YUV frames): pass all of a call's frames as MonoFrames")
             raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV frames "
                              "(YUV420Frame, YUV422Frame, YUV444Frame, V210Frame), not a mix")
         for i, f in enumerate(frames):
@@ -750,7 +857,8 @@ class FEARMultiTracker:
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
             frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, ycbcr_pin=None,
-            ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, ycbcr_hdr_pin=None, ycbcr_hdr=None, bayer_pin=None, bayer=None, sums_pin=None, sums=None)
+            ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, ycbcr_hdr_pin=None, ycbcr_hdr=None, bayer_pin=None,
+            bayer=None, mono_pin=None, mono=None, sums_pin=None, sums=None)
         return b
 
     def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
@@ -758,10 +866,10 @@ class FEARMultiTracker:
         "yuv" (FearFrameYUV records) when every frame is a YUV420Frame, "ycbcr_hdr" (FearFrameYCbCrHDR records) for YUV
         frames of which any has a transfer (PQ, HLG), else "ycbcr_v210" (FearFrameYCbCrV210 records) for YUV frames of
         which any is a V210Frame, "ycbcr" (FearFrameYCbCr records) for other YUV frames of which any is
-        4:2:2 or 4:4:4, "bayer" (FearFrameBayer records) for BayerFrames, "views" (FearFrameView records) otherwise.
-        Numpy frames are packed into the pinned staging buffer first and sent with one host-to-device copy (the packed
-        layout is recomputed only when their shapes change); CUDA tensors, YUV planes, v210 surfaces and Bayer mosaics
-        are used where they are."""
+        4:2:2 or 4:4:4, "bayer" (FearFrameBayer records) for BayerFrames, "mono" (FearFrameMono records) for
+        MonoFrames, "views" (FearFrameView records) otherwise.  Numpy frames are packed into the pinned staging buffer
+        first and sent with one host-to-device copy (the packed layout is recomputed only when their shapes change);
+        CUDA tensors, YUV planes, v210 surfaces, Bayer mosaics and mono frames are used where they are."""
         b, num_frames = self._buf, len(frames)
         name = "views"
         if kind == "yuv":
@@ -770,8 +878,8 @@ class FEARMultiTracker:
                 name = "ycbcr_v210"
             if any(f.transfer is not None for f in frames):
                 name = "ycbcr_hdr"
-        elif kind == "bayer":
-            name = "bayer"
+        elif kind in ("bayer", "mono"):
+            name = kind
         dtype = TABLE_DTYPES[name]
         nbytes = num_frames * dtype.itemsize
         if b[name] is None or b[name].numel() < nbytes:  # grows only: the step graph keys on it
@@ -806,11 +914,14 @@ class FEARMultiTracker:
         b[name][:nbytes].copy_(b[name + "_pin"][:nbytes], non_blocking=True)
         return name
 
-    def _step(self, n: int, num_frames: int, dev: torch.device, table: str = "views") -> torch.Tensor:
+    def _step(self, n: int, num_frames: int, dev: torch.device, table: str = "views",
+              agc: bool = False) -> torch.Tensor:
         b, cfg, lib = self._buf, self.tracking_config, _lib.load()
         _, crop_fn, advance_fn = ENTRY_POINTS[table]
         size = int(cfg["instance_size"])
         s = torch.cuda.current_stream(dev).cuda_stream
+        if agc:  # the frames' code ranges, written into the table the crop reads
+            _lib.check(getattr(lib, RANGE_ENTRY_POINT)(b[table].data_ptr(), num_frames, s), RANGE_ENTRY_POINT)
         _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b["state"].data_ptr(), n,
                                          float(cfg["search_context"]), size, b["crops"].data_ptr(), s), crop_fn)
         boxes = self.net.track_boxes(b["crops"][:n], b["zf"][:n])
@@ -818,13 +929,14 @@ class FEARMultiTracker:
                                             n, size, s), advance_fn)
         return boxes
 
-    def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device) -> torch.Tensor:
+    def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device, agc: bool = False) -> torch.Tensor:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
         keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records, YCbCr
-        records of any subsampling, YCbCr / v210 records, HDR records or Bayer records) and
-        its buffer, and the net's generation.  ``cuda_graph=False`` in the tracking config keeps eager launches."""
-        key = (n, num_frames, table, self._buf[table].data_ptr())
+        records of any subsampling, YCbCr / v210 records, HDR records, Bayer records or mono records) and
+        its buffer, whether the step starts with the mono range kernel (``agc``), and the net's generation.
+        ``cuda_graph=False`` in the tracking config keeps eager launches."""
+        key = (n, num_frames, table, self._buf[table].data_ptr(), agc)
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):
             # new target or frame count, another table or a new table buffer, or the net's workspace / weights /
             # options changed: the pointers and sizes baked into the captured graph are stale -> warm up eagerly and
@@ -835,7 +947,7 @@ class FEARMultiTracker:
             try:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    self._graph_boxes = self._step(n, num_frames, dev, table)
+                    self._graph_boxes = self._step(n, num_frames, dev, table, agc)
                 self._graph, self._graph_gen = g, self.net.generation()
             except RuntimeError as exc:
                 warnings.warn(f"FEARMultiTracker: CUDA-graph capture of the step failed ({exc}); using eager launches")
@@ -845,4 +957,4 @@ class FEARMultiTracker:
         if use_graph and self._graph is not None:
             self._graph.replay()
             return self._graph_boxes
-        return self._step(n, num_frames, dev, table)
+        return self._step(n, num_frames, dev, table, agc)

@@ -8,10 +8,11 @@ of the reference's observable behaviour); network + decode run in libfear_b200 a
 48-byte box record comes back per frame.  With ``gpu_crop: true`` the numpy frame is uploaded and cropped on the device.
 
 Frames already in GPU memory -- uint8 (H, W, 3) CUDA tensors with any non-negative strides, YUV420Frame /
-YUV422Frame / YUV444Frame decoder surfaces, V210Frame capture buffers and BayerFrame raw mosaics -- are read in place:
+YUV422Frame / YUV444Frame decoder surfaces, V210Frame capture buffers, BayerFrame raw mosaics and MonoFrame
+single-channel frames -- are read in place:
 the crop, the conversion to RGB (or the demosaic), the network and the decode (plain or smoothed) run on the device, and
 the tracker returns exactly what it returns for the same pixels as a numpy array (``image_ops.yuv_to_rgb`` of a YUV
-frame's planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes).
+frame's planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes, ``image_ops.mono_to_rgb`` of a mono frame's).
 """
 from collections import deque
 from typing import Any, Dict, Optional, Tuple, Union
@@ -26,7 +27,7 @@ from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY
 
 
 # byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrHDR; a
-# FearFrameBayer is 40 bytes), a FearTarget, then five float64 inputs of fear_decode_smooth
+# FearFrameBayer is 40 bytes, a FearFrameMono 48), a FearTarget, then five float64 inputs of fear_decode_smooth
 _TARGET_OFFSET = 104
 _SMOOTH_OFFSET = _TARGET_OFFSET + 64
 _DEVICE_INPUT_BYTES = _SMOOTH_OFFSET + 5 * 8
@@ -110,19 +111,21 @@ class FEARTracker(Tracker):
     """The reference's single-object tracker.  ``initialize``, ``update`` and ``get_template_features`` take a frame as
     a uint8 (H, W, 3) RGB numpy array, as a uint8 (H, W, 3) CUDA tensor on the tracker's device (any non-negative
     strides: ``rgba[..., :3]``, ``chw.permute(1, 2, 0)``, a region of interest), or as a YUV420Frame, YUV422Frame,
-    YUV444Frame, V210Frame or BayerFrame whose planes, words or samples are on the tracker's device; the kind may
-    change from one call to the next.
+    YUV444Frame, V210Frame, BayerFrame or MonoFrame whose planes, words or samples are on the tracker's device; the
+    kind may change from one call to the next.
 
     Numpy frames take the host crop, or with ``gpu_crop: true`` an upload and the device crop.  Device frames always
     take the device step, whatever ``gpu_crop`` says, since the host crop could only read them after copying them back:
-    fear_crop_targets_view_u8 (tensors), fear_crop_targets_ycbcr_u8 (YUV frames, converted to RGB inside the crop) or
-    fear_crop_targets_ycbcr_v210_u8 (v210 frames, unpacked and converted inside the crop) or fear_crop_targets_bayer_u8
-    (Bayer frames, demosaiced inside the crop) makes the search crop, then the network and the decode, plain or with
-    ``smooth: true`` the smoothed one, run as one CUDA graph and one 48-byte record comes back.  The results,
-    ``tracking_state`` included, are those of the same tracker fed the same pixels as numpy arrays
+    fear_crop_targets_view_u8 (tensors), fear_crop_targets_ycbcr_u8 (YUV frames, converted to RGB inside the crop),
+    fear_crop_targets_ycbcr_v210_u8 (v210 frames, unpacked and converted inside the crop), fear_crop_targets_bayer_u8
+    (Bayer frames, demosaiced inside the crop) or fear_crop_targets_mono_u8 (mono frames, mapped to grey inside the
+    crop, after fear_frame_range_mono when the frame has gain control) makes the search crop, then the network and the
+    decode, plain or with ``smooth: true`` the smoothed one, run as one CUDA graph and one 48-byte record comes back.
+    The results, ``tracking_state`` included, are those of the same tracker fed the same pixels as numpy arrays
     (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its ``CHROMA_SHIFT``, of a v210 frame's
-    ``image_ops.v210_unpack`` planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes).  Device frames must be ready
-    on the current CUDA stream; every call synchronises it before it returns, so they only need to live for the call.
+    ``image_ops.v210_unpack`` planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes, ``image_ops.mono_to_rgb``
+    of a mono frame's codes with its ``agc``).  Device frames must be ready on the current CUDA stream; every call
+    synchronises it before it returns, so they only need to live for the call.
     ``host_normalize: true`` takes numpy frames only."""
 
     def get_box_coder(self, tracking_config, cuda_id: int = 0):
@@ -279,8 +282,8 @@ class FEARTracker(Tracker):
 
     # -- device frames: CUDA tensors and YUV frames, read in place by the crop-targets entry points (one target) --
     def _frame_kind(self, image) -> str:
-        """"numpy", "cuda", "yuv" or "bayer" (multi_tracker.frame_kind).  A device frame is checked here, before any
-        device call or state change: NotImplementedError with ``host_normalize``, ValueError when malformed."""
+        """"numpy", "cuda", "yuv", "bayer" or "mono" (multi_tracker.frame_kind).  A device frame is checked here, before
+        any device call or state change: NotImplementedError with ``host_normalize``, ValueError when malformed."""
         kind = multi_tracker.frame_kind(image)
         if kind == "numpy":
             return kind
@@ -293,9 +296,9 @@ class FEARTracker(Tracker):
     def _device_frame_state(self) -> dict:
         """Buffers of the device-frame step, separate from the gpu_crop path's.  ``inputs`` (pinned) and ``dev_in``
         share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView, a
-        FearFrameYCbCr, a FearFrameYCbCrV210, a FearFrameYCbCrHDR or a FearFrameBayer) at byte 0, the FearTarget at
-        byte 104, fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr as float64 at byte 168;
-        then, on the device only, the score_size x score_size window."""
+        FearFrameYCbCr, a FearFrameYCbCrV210, a FearFrameYCbCrHDR, a FearFrameBayer or a FearFrameMono) at byte 0, the
+        FearTarget at byte 104, fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr as float64 at
+        byte 168; then, on the device only, the score_size x score_size window."""
         from . import _lib
 
         dev = self._device()
@@ -324,8 +327,8 @@ class FEARTracker(Tracker):
         """Write the frame's record, the target (frame 0, ``bbox``, padding colour ``pad``) and, given ``prev_size``,
         the smooth scalars into the pinned inputs and send them with one host-to-device copy.  Returns the table name:
         "views" for a tensor, "ycbcr_hdr" for a YUV frame with a transfer (PQ, HLG), "ycbcr_v210" for another
-        V210Frame, "ycbcr" for every other YUV frame, "bayer" for a BayerFrame."""
-        table = "bayer" if kind == "bayer" else "views"
+        V210Frame, "ycbcr" for every other YUV frame, "bayer" for a BayerFrame, "mono" for a MonoFrame."""
+        table = kind if kind in ("bayer", "mono") else "views"
         if kind == "yuv":
             table = "ycbcr_v210" if isinstance(image, multi_tracker.V210Frame) else "ycbcr"
             if image.transfer is not None:
@@ -343,6 +346,16 @@ class FEARTracker(Tracker):
         st["dev_in"][:_DEVICE_INPUT_BYTES].copy_(st["inputs"], non_blocking=True)
         return table
 
+    @staticmethod
+    def _device_frame_range(st: dict, image, kind: str, stream) -> None:
+        """For a MonoFrame with gain control, fear_frame_range_mono on the staged FearFrameMono record: the frame's code
+        range, which the mono sums and crop read, written into the record on the device."""
+        from . import _lib
+
+        if multi_tracker.uses_agc([image], kind):
+            fn = multi_tracker.RANGE_ENTRY_POINT
+            _lib.check(getattr(_lib.load(), fn)(st["dev_in"].data_ptr(), 1, stream), fn)
+
     def _device_mean_color(self, image, kind: str) -> np.ndarray:
         """np.mean(frame, axis=(0, 1)) of the RGB frame, bit for bit: exact per-channel sums on the device over H * W."""
         from . import _lib
@@ -353,6 +366,7 @@ class FEARTracker(Tracker):
             table = self._stage_device_inputs(st, image, kind, (0, 0, 0, 0), (0, 0, 0))
             sums_fn = multi_tracker.ENTRY_POINTS[table][0]
             stream = torch.cuda.current_stream(dev)
+            self._device_frame_range(st, image, kind, stream.cuda_stream)
             _lib.check(getattr(_lib.load(), sums_fn)(st["dev_in"].data_ptr(), 1, st["sums"].data_ptr(),
                                                      stream.cuda_stream), sums_fn)
             st["sums_pin"].copy_(st["sums"], non_blocking=True)
@@ -377,6 +391,7 @@ class FEARTracker(Tracker):
             table = self._stage_device_inputs(st, image, kind, box.astype(np.int32), image_ops.padding_color(mean_color))
             crop_fn = multi_tracker.ENTRY_POINTS[table][1]
             stream = torch.cuda.current_stream(dev)
+            self._device_frame_range(st, image, kind, stream.cuda_stream)
             dp = st["dev_in"].data_ptr()
             _lib.check(getattr(_lib.load(), crop_fn)(dp, 1, dp + _TARGET_OFFSET, 1, offset, size,
                                                      st["tcrop"].data_ptr(), stream.cuda_stream), crop_fn)
@@ -399,7 +414,8 @@ class FEARTracker(Tracker):
     def _track_record_device_frame(self, image, kind: str):
         """One update on a device frame: crop-targets (N = 1, search_context, instance_size) -> fear_track_sized_u8 -> the
         plain decode, or with smooth the maps -> fear_decode_smooth_sized; one 48-byte record back.  The crop kernel reads the frame's record
-        when it runs, so the graph (captured on the second update) keys on the table kind, smooth, the input buffer and
+        when it runs, so the graph (captured on the second update) keys on the table kind, smooth, the input buffer,
+        whether it starts with the mono range kernel and
         net.generation(), not on the frame's address or shape: fresh decoder surfaces and a resolution change replay it."""
         from . import _lib
 
@@ -415,9 +431,11 @@ class FEARTracker(Tracker):
                 st["zf_src"] = self._template_features
             lib = _lib.load()
             crop_fn = multi_tracker.ENTRY_POINTS[table][1]
+            agc = multi_tracker.uses_agc([image], kind)
 
             def step():
                 stream = torch.cuda.current_stream(dev).cuda_stream
+                self._device_frame_range(st, image, kind, stream)
                 dp = st["dev_in"].data_ptr()
                 _lib.check(getattr(lib, crop_fn)(dp, 1, dp + _TARGET_OFFSET, 1, float(cfg["search_context"]), size,
                                                  st["crop"].data_ptr(), stream), crop_fn)
@@ -431,7 +449,7 @@ class FEARTracker(Tracker):
                            "fear_decode_smooth_sized")
                 return st["smooth_boxes"]
 
-            key = (table, smooth, st["dev_in"].data_ptr(), self.net.generation())
+            key = (table, smooth, st["dev_in"].data_ptr(), self.net.generation(), agc)
             if key != st["key"]:  # another entry point, or stale workspace / weight pointers: warm up and capture again
                 st["graph"], st["key"], st["calls"] = None, key, 0
             use_graph = cfg.get("cuda_graph", True) and st["graph_ok"]

@@ -47,6 +47,10 @@
  *   fear_crop_targets_bayer_u8 / fear_advance_targets_bayer / fear_frame_sums_bayer_u8   the same three on raw Bayer
  *                         mosaics located by FearFrameBayer (8 to 16 bits, MIPI RAW10 / RAW12), demosaiced inside the
  *                         crop as cv2.cvtColor(COLOR_Bayer*2RGB) demosaics them
+ *   fear_frame_range_mono  per-frame code range (min, max) of single-channel frames located by FearFrameMono, written
+ *                         into the table for their min-max gain control (thermal cores, mono cameras)
+ *   fear_crop_targets_mono_u8 / fear_advance_targets_mono / fear_frame_sums_mono_u8   the same three on FearFrameMono
+ *                         tables (8 to 16 bits, MIPI RAW10 / RAW12), each tap mapped to grey (g, g, g) inside the crop
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -287,6 +291,36 @@ typedef struct FearFrameBayer {               /* 40 bytes                       
   int32_t H, W;                               /* size in pixels, both >= 3                                      */
   int32_t pattern, bits, shift, packing;      /* FEAR_BAYER_*, code depth, uint16 alignment, FEAR_BAYER_* packing */
 } FearFrameBayer;
+/* A single-channel frame (machine-vision cameras' PFNC Mono8 / Mono10 / Mono12 / Mono16, CSI-2 mono sensors' GREY /
+ * Y10 / Y12 / Y16 / Y10P / Y12P, thermal cores' 14- or 16-bit Y16): 48 bytes.  data, row_stride, bits, shift and
+ * packing are FearFrameBayer's, read the same way (FEAR_BAYER_UNPACKED, FEAR_BAYER_RAW10, FEAR_BAYER_RAW12).  Pixel
+ * (y, x) is the grey triple (g, g, g) of its code v:
+ *   agc 0                without gain control: g = v at 8 bits; above 8 bits v is mapped as FearFrameBayer maps a
+ *                        channel, min(max(rint(255 * (v * (1 / (2^bits - 1)))), 0), 255) in float64
+ *   agc FEAR_AGC_MINMAX  min-max gain control over the whole frame, cv2.normalize(codes, None, 0, 255, NORM_MINMAX,
+ *                        CV_8U) of the frame's codes: with lo, hi its smallest and largest code,
+ *                        scale = 255 * (hi - lo > DBL_EPSILON ? 1 / (hi - lo) : 0) and shift = 0 - lo * scale in
+ *                        float64, each operation rounded; then a = (float)scale, b = (float)shift and
+ *                        g = min(max(rint(fmaf((float)v, a, b)), 0), 255), the multiply-add rounded once.  A constant
+ *                        frame (hi == lo) is 0 everywhere, as in cv2.  lo and hi are read from the record, where
+ *                        fear_frame_range_mono writes them: the record's writer sets lo = INT32_MAX and
+ *                        hi = INT32_MIN (an empty range, which maps every code to 0) and the range kernel lowers and
+ *                        raises them atomically to the frame's range, so a captured graph that rewrites the table
+ *                        before the range kernel sees each frame's own range.
+ * An entry is treated like a frame index outside [0, F) when data is null, H or W is below 1, the bits, shift or
+ * packing break FearFrameBayer's rules (bits in {8, 10, 12, 14, 16} unpacked with 0 <= shift <= 16 - bits and shift 0
+ * at 8 bits; 10 for RAW10, 12 for RAW12; packing 0..2), agc is neither 0 nor FEAR_AGC_MINMAX, an unpacked uint16 entry
+ * has an odd address or row_stride, or row_stride is below the bytes of a row (W, 2 W, 5 * ceil(W / 4) or
+ * 3 * ceil(W / 2)).  Unlike FearFrameBayer there is no neighbourhood, so 1 x 1 frames are read. */
+#define FEAR_AGC_MINMAX 1
+typedef struct FearFrameMono {                /* 48 bytes                                                       */
+  const void* data;                           /* device address of sample (0, 0) / of row 0's first byte        */
+  int64_t row_stride;                         /* bytes                                                          */
+  int32_t H, W;                               /* size in pixels, both >= 1                                      */
+  int32_t bits, shift, packing;               /* code depth, uint16 alignment, FEAR_BAYER_* packing             */
+  int32_t agc;                                /* 0: none; FEAR_AGC_MINMAX: min-max gain control                 */
+  int32_t lo, hi;                             /* the frame's code range, written by fear_frame_range_mono       */
+} FearFrameMono;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -490,6 +524,22 @@ int fear_crop_targets_bayer_u8(const FearFrameBayer* d_views, int F, FearTarget*
 int fear_advance_targets_bayer(const FearBox* d_boxes, const FearFrameBayer* d_views, int F, FearTarget* d_targets,
                                int N, int instance_size, void* stream);
 int fear_frame_sums_bayer_u8(const FearFrameBayer* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* The code range of every readable FearFrameMono entry with agc != 0: lo = min(lo, smallest code) and
+ * hi = max(hi, largest code), atomically, in the device table itself (codes after unpacking and the shift).  Entries
+ * with agc 0 and entries the kernels cannot read (see FearFrameMono) are left untouched.  Run it after the table is
+ * written and before the crop or the sums; a table written with lo = INT32_MAX, hi = INT32_MIN gets each frame's
+ * exact range.  FEAR_EINVAL for a null table or F outside [1, 65535]. */
+int fear_frame_range_mono(FearFrameMono* d_views, int F, void* stream);
+/* The same three on FearFrameMono tables: single-channel frames read where they are, each tap mapped to grey (with or
+ * without min-max gain control, see FearFrameMono) inside the crop, so the kernels see cv2.cvtColor(g, COLOR_GRAY2RGB).
+ * Same semantics and FEAR_EINVAL rules as the *_bayer entry points; an entry the kernels cannot read gets a
+ * padding-colour crop, keeps its box and sums to 0. */
+int fear_crop_targets_mono_u8(const FearFrameMono* d_views, int F, FearTarget* d_targets, int N, double offset,
+                              int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_mono(const FearBox* d_boxes, const FearFrameMono* d_views, int F, FearTarget* d_targets,
+                              int N, int instance_size, void* stream);
+int fear_frame_sums_mono_u8(const FearFrameMono* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
