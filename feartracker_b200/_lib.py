@@ -58,6 +58,12 @@ assert BAYER_DTYPE.itemsize == 40
 MONO_DTYPE = np.dtype([("data", "<u8"), ("row_stride", "<i8"), ("H", "<i4"), ("W", "<i4"), ("bits", "<i4"),
                        ("shift", "<i4"), ("packing", "<i4"), ("agc", "<i4"), ("lo", "<i4"), ("hi", "<i4")])
 assert MONO_DTYPE.itemsize == 48
+# FearFrameRGB: three channel addresses in one kind of little-endian container, shared strides, the code's depth and
+# each channel's shift
+RGB_DTYPE = np.dtype([("r", "<u8"), ("g", "<u8"), ("b", "<u8"), ("row_stride", "<i8"), ("pixel_stride", "<i8"),
+                      ("H", "<i4"), ("W", "<i4"), ("container", "<i4"), ("bits", "<i4"), ("shift_r", "<i4"),
+                      ("shift_g", "<i4"), ("shift_b", "<i4"), ("reserved", "<i4")])
+assert RGB_DTYPE.itemsize == 72
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -106,6 +112,9 @@ _SIGNATURES = {
     "fear_crop_targets_mono_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_mono": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_mono_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_rgb_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "fear_advance_targets_rgb": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "fear_frame_sums_rgb_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "fear_decode_smooth": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fear_head_sized": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,

@@ -1103,6 +1103,9 @@ static_assert(sizeof(FearFrameBayer) == 40 && offsetof(FearFrameBayer, packing) 
               "FearFrameBayer layout is part of the ABI");
 static_assert(sizeof(FearFrameMono) == 48 && offsetof(FearFrameMono, agc) == 36 && offsetof(FearFrameMono, hi) == 44,
               "FearFrameMono layout is part of the ABI");
+static_assert(sizeof(FearFrameRGB) == 72 && offsetof(FearFrameRGB, row_stride) == 24 &&
+                  offsetof(FearFrameRGB, container) == 48 && offsetof(FearFrameRGB, reserved) == 68,
+              "FearFrameRGB layout is part of the ABI");
 
 static int check_crop_targets_args(int F, int N, double offset, int out_size) {
   if (N < 1 || N > 65535) return set_err(FEAR_EINVAL, "target count must be in [1, 65535] (got %d)", N);
@@ -1326,6 +1329,25 @@ extern "C" int fear_advance_targets_mono(const FearBox* d_boxes, const FearFrame
 
 extern "C" int fear_frame_sums_mono_u8(const FearFrameMono* d_views, int F, uint64_t* d_sums, void* stream) {
   return launch_frame_sums(d_views, MonoFrames{d_views}, F, d_sums, stream);
+}
+
+// RGB frames in any channel order and container: the same kernels, reading through RGBFrames.
+extern "C" int fear_crop_targets_rgb_u8(const FearFrameRGB* d_views, int F, FearTarget* d_targets, int N, double offset,
+                                        int out_size, uint8_t* d_crops, void* stream) {
+  if (!d_views || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return launch_crop_targets(RGBFrames{d_views}, F, d_targets, N, offset, out_size, d_crops, stream);
+}
+
+extern "C" int fear_advance_targets_rgb(const FearBox* d_boxes, const FearFrameRGB* d_views, int F,
+                                        FearTarget* d_targets, int N, int instance_size, void* stream) {
+  if (!d_boxes || !d_views || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return launch_advance_targets(d_boxes, RGBFrames{d_views}, F, d_targets, N, instance_size, stream);
+}
+
+extern "C" int fear_frame_sums_rgb_u8(const FearFrameRGB* d_views, int F, uint64_t* d_sums, void* stream) {
+  return launch_frame_sums(d_views, RGBFrames{d_views}, F, d_sums, stream);
 }
 
 extern "C" int fear_decode_sized(const float* d_bbox, const float* d_cls, int B, int side, int apply_sigmoid,

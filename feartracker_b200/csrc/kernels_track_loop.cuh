@@ -18,8 +18,9 @@
 // FearFrameYCbCrV210 records (YCbCrV210Frames), read through V210Frame, which also unpacks v210 surfaces; or a table of
 // FearFrameYCbCrHDR records (YCbCrHDRFrames), read through HDRFrame, which also tone-maps PQ and HLG video to SDR; or a
 // table of FearFrameBayer records (BayerFrames), read through BayerFrame, which demosaics raw Bayer mosaics; or a
-// table of FearFrameMono records (MonoFrames), read through MonoFrame, which maps single-channel codes to grey.  A
-// frame type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables,
+// table of FearFrameMono records (MonoFrames), read through MonoFrame, which maps single-channel codes to grey; or a
+// table of FearFrameRGB records (RGBFrames), read through RGBFrame, which fetches each channel from its own address in
+// an 8-, 16- or 32-bit container (any channel order, packed or planar) and maps it to 8 bits.  A frame type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables,
 // interpolation, sums and the colour conversion exist once.
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
@@ -578,6 +579,73 @@ struct MonoFrames {
       f.b = __double2float_rn(shift);
     }
     return f;
+  }
+};
+
+// An RGB frame (FearFrameRGB): channel c of pixel (y, x) is the container at c_ptr + y * rs + x * ps, its code
+// (value >> shift_c) & (2^bits - 1), mapped to 8 bits as BayerFrame maps a channel (the code itself at 8 bits).  A byte
+// container is read with three byte loads and no float64 work; a 32-bit container (x2rgb10: r == g == b) with one word
+// load.  `bad` marks an entry the kernels cannot read.  A value-initialised RGBFrame{} is empty.
+struct RGBFrame {
+  const uint8_t *r, *g, *b;
+  long long rs, ps;
+  int H, W;
+  int container, bits;
+  int sr, sg, sb;
+  bool bad;
+  double ys;
+  __device__ __forceinline__ bool empty() const { return bad || r == nullptr || H < 1 || W < 1; }
+  __device__ __forceinline__ int to_u8(int v) const { return yuv_unit_to_u8(__dmul_rn((double)v, ys)); }
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    const long long o = (long long)y * rs + (long long)x * ps;
+    if (container == 1) {
+      p[0] = __ldg(r + o);
+      p[1] = __ldg(g + o);
+      p[2] = __ldg(b + o);
+      return;
+    }
+    const int m = (1 << bits) - 1;
+    int v[3];
+    if (container == 4) {
+      const unsigned w = __ldg(reinterpret_cast<const unsigned*>(r + o));
+      v[0] = (int)(w >> sr) & m;
+      v[1] = (int)(w >> sg) & m;
+      v[2] = (int)(w >> sb) & m;
+    } else {
+      v[0] = (__ldg(reinterpret_cast<const uint16_t*>(r + o)) >> sr) & m;
+      v[1] = (__ldg(reinterpret_cast<const uint16_t*>(g + o)) >> sg) & m;
+      v[2] = (__ldg(reinterpret_cast<const uint16_t*>(b + o)) >> sb) & m;
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) p[c] = to_u8(v[c]);
+  }
+};
+
+// Frame i of a FearFrameRGB table (the *_rgb entry points), checked per entry against FearFrameRGB's rules.
+struct RGBFrames {
+  const FearFrameRGB* views;
+  __device__ __forceinline__ RGBFrame operator()(int i) const {
+    const FearFrameRGB v = views[i];
+    const int bits = v.bits, sr = v.shift_r, sg = v.shift_g, sb = v.shift_b;
+    const uintptr_t addr = (uintptr_t)v.r | (uintptr_t)v.g | (uintptr_t)v.b | (uintptr_t)v.row_stride |
+                           (uintptr_t)v.pixel_stride;
+    bool ok;
+    if (v.container == 1) {
+      ok = bits == 8 && (sr | sg | sb) == 0;
+    } else if (v.container == 2) {
+      const int top = 16 - bits;
+      ok = (bits == 10 || bits == 12 || bits == 16) && sr >= 0 && sr <= top && sg >= 0 && sg <= top && sb >= 0 &&
+           sb <= top && !(addr & 1);
+    } else if (v.container == 4) {
+      // with every shift in [0, 20], the three bits are set at 0, 10 and 20 only for a permutation of {0, 10, 20}
+      ok = bits == 10 && v.r == v.g && v.r == v.b && sr >= 0 && sr <= 20 && sg >= 0 && sg <= 20 && sb >= 0 &&
+           sb <= 20 && ((1 << sr) | (1 << sg) | (1 << sb)) == ((1 << 0) | (1 << 10) | (1 << 20)) && !(addr & 3);
+    } else {
+      ok = false;
+    }
+    ok = ok && v.g != nullptr && v.b != nullptr && v.row_stride >= 0 && v.pixel_stride >= 0;
+    return RGBFrame{v.r, v.g, v.b, v.row_stride, v.pixel_stride, v.H, v.W, v.container, bits, sr, sg, sb, !ok,
+                    ok && bits != 8 ? __ddiv_rn(1.0, (double)((1 << bits) - 1)) : 0.0};
   }
 };
 

@@ -647,3 +647,74 @@ def mono_to_rgb(codes: np.ndarray, bits: int = 8, agc: Optional[str] = None) -> 
         raise ValueError(f"mono codes must be a 2-D (H, W) array, got shape {a.shape}")
     g = minmax_normalize(a) if agc == "minmax" else raw_to_u8(a, bits)
     return np.repeat(g[..., None], 3, axis=-1)
+
+
+# Packed RGB layouts by ffmpeg pix_fmt name: sample type, samples per pixel, and the sample indices of R, G and B
+RGB_PACKED_LAYOUTS = {
+    "rgb24": (np.uint8, 3, (0, 1, 2)), "bgr24": (np.uint8, 3, (2, 1, 0)),
+    "rgba": (np.uint8, 4, (0, 1, 2)), "bgra": (np.uint8, 4, (2, 1, 0)), "argb": (np.uint8, 4, (1, 2, 3)),
+    "abgr": (np.uint8, 4, (3, 2, 1)), "rgb0": (np.uint8, 4, (0, 1, 2)), "bgr0": (np.uint8, 4, (2, 1, 0)),
+    "0rgb": (np.uint8, 4, (1, 2, 3)), "0bgr": (np.uint8, 4, (3, 2, 1)),
+    "rgb48le": (np.uint16, 3, (0, 1, 2)), "bgr48le": (np.uint16, 3, (2, 1, 0)),
+    "rgba64le": (np.uint16, 4, (0, 1, 2)), "bgra64le": (np.uint16, 4, (2, 1, 0)),
+}
+# 10-bit RGB in one little-endian 32-bit word (the top 2 bits spare): the bit offsets of R, G and B
+X2RGB10_LAYOUTS = {"x2rgb10le": (20, 10, 0), "x2bgr10le": (0, 10, 20)}
+# the depths of planar RGB (ffmpeg's gbrp, gbrp10le, gbrp12le, gbrp16le): uint8 at 8 bits, else LSB-aligned uint16
+RGB_PLANAR_BITS = (8, 10, 12, 16)
+
+
+def x2rgb10_pack(codes: np.ndarray, layout: str = "x2rgb10le", spare: Optional[np.ndarray] = None) -> np.ndarray:
+    """The (H, W) uint32 words of (H, W, 3) RGB codes in [0, 1023] in ``layout`` ("x2rgb10le": B in bits 0-9, G in
+    10-19, R in 20-29; "x2bgr10le": R, G, B from bit 0), with ``spare`` (values in [0, 3], default 0) in bits 30-31."""
+    shifts = X2RGB10_LAYOUTS[layout]
+    c = np.asarray(codes)
+    if c.ndim != 3 or c.shape[2] != 3 or (c.size and (c.min() < 0 or c.max() > 1023)):
+        raise ValueError(f"x2rgb10 codes must be an (H, W, 3) array in [0, 1023], got {c.dtype} {c.shape}")
+    w = np.zeros(c.shape[:2], dtype=np.uint32)
+    for ch, s in enumerate(shifts):
+        w |= c[..., ch].astype(np.uint32) << np.uint32(s)
+    if spare is not None:
+        w |= (np.asarray(spare).astype(np.uint32) & np.uint32(3)) << np.uint32(30)
+    return w
+
+
+def x2rgb10_unpack(words: np.ndarray, layout: str = "x2rgb10le") -> np.ndarray:
+    """The (H, W, 3) uint16 RGB codes of (H, W) 32-bit words in ``layout``; the 2 spare bits are not read."""
+    shifts = X2RGB10_LAYOUTS[layout]
+    w = np.asarray(words).view(np.uint32)
+    return np.stack([(w >> np.uint32(s)) & np.uint32(1023) for s in shifts], -1).astype(np.uint16)
+
+
+def rgb_frame_to_rgb(data, layout: str, bits: Optional[int] = None) -> np.ndarray:
+    """The (H, W, 3) uint8 RGB frame FEARMultiTracker sees for an RGBFrame of ``layout`` holding ``data``:
+        a packed layout (RGB_PACKED_LAYOUTS)   data (H, W, C) samples of the layout's type; R, G, B picked out, and at
+                                               16 bits each mapped by ``raw_to_u8``
+        "x2rgb10le" / "x2bgr10le"              data (H, W) 32-bit words: ``x2rgb10_unpack``, then ``raw_to_u8`` at 10
+        "planar"                               data the R, G and B planes ((3, H, W) or three (H, W)), ``bits`` 8, 10,
+                                               12 or 16: uint8 at 8 bits, else uint16 whose low ``bits`` bits are the
+                                               code (the high bits are not read), mapped by ``raw_to_u8``
+    At 8 bits this is cv2.cvtColor(data, COLOR_BGR2RGB / COLOR_BGRA2RGB / COLOR_RGBA2RGB) for the layouts cv2 names."""
+    if layout in RGB_PACKED_LAYOUTS:
+        dtype, n, idx = RGB_PACKED_LAYOUTS[layout]
+        a = np.asarray(data)
+        if a.dtype != dtype or a.ndim != 3 or a.shape[2] != n:
+            raise ValueError(f"{layout} data must be (H, W, {n}) {np.dtype(dtype).name}, got {a.dtype} {a.shape}")
+        return raw_to_u8(a[..., list(idx)], 8 if dtype == np.uint8 else 16)
+    if layout in X2RGB10_LAYOUTS:
+        a = np.asarray(data)
+        if a.dtype not in (np.uint32, np.int32) or a.ndim != 2:
+            raise ValueError(f"{layout} data must be (H, W) 32-bit words, got {a.dtype} {a.shape}")
+        return raw_to_u8(x2rgb10_unpack(a, layout), 10)
+    if layout == "planar":
+        if isinstance(bits, bool) or bits not in RGB_PLANAR_BITS:
+            raise ValueError(f"planar RGB bits must be 8, 10, 12 or 16, got {bits!r}")
+        a = np.stack([np.asarray(p) for p in data])
+        if a.dtype != (np.uint8 if bits == 8 else np.uint16) or a.ndim != 3 or a.shape[0] != 3:
+            raise ValueError(f"planar RGB at {bits} bits takes three (H, W) {'uint8' if bits == 8 else 'uint16'} "
+                             f"planes, got {a.dtype} {a.shape}")
+        codes = np.moveaxis(a, 0, -1)
+        if bits not in (8, 16):
+            codes = codes & np.uint16((1 << bits) - 1)
+        return raw_to_u8(codes, bits)
+    raise ValueError(f"unknown RGB layout {layout!r}")

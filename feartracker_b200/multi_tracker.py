@@ -15,8 +15,10 @@ inside the crop); or raw Bayer mosaics as machine-vision and CSI-2 cameras send 
 BGGR at 8 to 16 bits, MIPI RAW10 / RAW12), demosaiced inside the crop exactly as cv2.cvtColor(COLOR_Bayer*2RGB)
 demosaics them; or single-channel frames as mono cameras and thermal cores send them: MonoFrame (8 to 16 bits, MIPI
 RAW10 / RAW12), mapped to grey inside the crop, optionally with per-frame min-max gain control (cv2.normalize
-NORM_MINMAX).  Tensors, YUV planes, v210 surfaces, Bayer mosaics and mono frames are read where they are, without a
-copy.
+NORM_MINMAX); or RGB frames in any channel order and container: RGBFrame (OpenCV's BGR and BGRA, RGBA / ARGB / ABGR
+and their X variants, 10-bit x2rgb10 / x2bgr10 words, 16-bit rgb48 / rgba64, planar gbrp at 8 to 16 bits), each tap's
+channels fetched and mapped to 8 bits inside the crop.  Tensors, YUV planes, v210 surfaces, Bayer mosaics, mono frames
+and RGB frames are read where they are, without a copy.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -38,7 +40,9 @@ a sixth, of FearFrameYCbCrHDR records (a FearFrameYCbCrV210 and its transfer), r
 which tone-map HDR taps to SDR inside the crop.  BayerFrames go into a fifth, of FearFrameBayer records, read by the *_bayer entry
 points; they cannot share a call with other kinds of frames.  MonoFrames go into a seventh, of FearFrameMono records,
 read by the *_mono entry points, and cannot share a call with other kinds either; when any of a call's MonoFrames has
-gain control, fear_frame_range_mono first writes each frame's code range into that table.  The host then reads back
+gain control, fear_frame_range_mono first writes each frame's code range into that table.  A call with any RGBFrame
+puts all its frames, RGBFrames and CUDA tensors alike, into an eighth, of FearFrameRGB records, read by the *_rgb entry
+points; RGBFrames cannot share a call with numpy arrays or YUV, Bayer or mono frames.  The host then reads back
 the boxes and scores.  The launch count of a step depends neither on N nor on the kind of frames, with one exception:
 a step on MonoFrames with gain control launches the range kernel too (49 launches instead of 48).
 """
@@ -63,10 +67,11 @@ ENTRY_POINTS = {
     "ycbcr_hdr": ("fear_frame_sums_ycbcr_hdr_u8", "fear_crop_targets_ycbcr_hdr_u8", "fear_advance_targets_ycbcr_hdr"),
     "bayer": ("fear_frame_sums_bayer_u8", "fear_crop_targets_bayer_u8", "fear_advance_targets_bayer"),
     "mono": ("fear_frame_sums_mono_u8", "fear_crop_targets_mono_u8", "fear_advance_targets_mono"),
+    "rgb": ("fear_frame_sums_rgb_u8", "fear_crop_targets_rgb_u8", "fear_advance_targets_rgb"),
 }
 TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.YCBCR_DTYPE,
                 "ycbcr_v210": _lib.YCBCR_V210_DTYPE, "ycbcr_hdr": _lib.YCBCR_HDR_DTYPE, "bayer": _lib.BAYER_DTYPE,
-                "mono": _lib.MONO_DTYPE}
+                "mono": _lib.MONO_DTYPE, "rgb": _lib.RGB_DTYPE}
 # the entry point that writes each frame's code range into a FearFrameMono table, for min-max gain control
 RANGE_ENTRY_POINT = "fear_frame_range_mono"
 
@@ -547,9 +552,133 @@ class MonoFrame(_RawFrame):
                 image_ops.AGC_MODES[self.agc], 2 ** 31 - 1, -2 ** 31)
 
 
+def _unstepped(t: torch.Tensor, *fixed) -> tuple:
+    """``t``'s element strides, with the stride of each dimension of size 1 (never stepped, so torch may report any
+    value) replaced by ``fixed[d]`` when given."""
+    return tuple(f if n == 1 and f is not None else s for n, s, f in zip(t.shape, t.stride(), fixed))
+
+
+class RGBFrame:
+    """An RGB frame in device memory in any channel order and container, read where it is, as OpenCV and capture
+    APIs hand it over.  Layout names are ffmpeg ``pix_fmt`` names:
+
+        RGBFrame(t, layout)                 t a CUDA tensor whose rows may be pitched (any row stride >= W * C, a view
+                                            ``surface[:, :W]`` is fine), channel stride 1, pixel stride C:
+            uint8 (H, W, 3)                 "rgb24", "bgr24" (OpenCV's BGR)
+            uint8 (H, W, 4)                 "rgba", "bgra", "argb", "abgr", "rgb0", "bgr0", "0rgb", "0bgr"
+                                            (cv2.cudacodec's BGRA, DeckLink bmdFormat8BitBGRA, desktop duplication)
+            torch.uint16 (H, W, 3 | 4)      "rgb48le", "bgr48le", "rgba64le", "bgra64le" (ProRes 4444, 16-bit PNG / TIFF)
+            torch.int32 / torch.uint32      "x2rgb10le" (B in bits 0-9, G 10-19, R 20-29; DRM XRGB2101010), "x2bgr10le"
+            (H, W), column stride 1         (R 0-9, G 10-19, B 20-29; DXGI R10G10B10A2_UNORM)
+        RGBFrame.planar(r, g, b, bits=8)    three CUDA (H, W) planes of one shape, dtype and strides: uint8 at 8 bits,
+                                            torch.uint16 with the code in the low bits at 10, 12 or 16; ffmpeg's gbrp*
+                                            is ``planar(data[2], data[0], data[1], bits)`` and a (3, H, W) uint16
+                                            tensor from torchvision's decode_png is ``planar(*t, bits=16)``
+
+    Alpha and X samples and the spare bits of a word are never read.  Codes above 8 bits are mapped to 8 bits as a
+    BayerFrame channel is, full range.  FEARMultiTracker and FEARTracker read each tap's channels where they are, so no
+    RGB copy is made: the frame the tracker sees is ``image_ops.rgb_frame_to_rgb(data, layout)`` of the same samples
+    (``"planar"`` with ``bits`` for planes), which at 8 bits is ``cv2.cvtColor(data, COLOR_BGR2RGB / COLOR_BGRA2RGB /
+    COLOR_RGBA2RGB)`` for the layouts cv2 names.  The constructors raise ValueError on a malformed tensor or layout;
+    they make no device call.  ``shape`` is (H, W, 3)."""
+
+    def __init__(self, t: torch.Tensor, layout: str) -> None:
+        if layout in image_ops.RGB_PACKED_LAYOUTS:
+            np_dtype, n, idx = image_ops.RGB_PACKED_LAYOUTS[layout]
+            dtype = torch.uint8 if np_dtype == np.uint8 else torch.uint16
+            self._check_tensor(t, (dtype,), 3, f"(H, W, {n}) tensor for {layout!r}")
+            if t.shape[2] != n:
+                raise ValueError(f"RGBFrame {layout!r} takes (H, W, {n}) samples, got {tuple(t.shape)}")
+            h, w = t.shape[:2]
+            rs, ps, cs = _unstepped(t, w * n, n, None)
+            if cs != 1 or ps != n or rs < w * n:
+                raise ValueError(f"RGBFrame {layout!r} needs channel stride 1, pixel stride {n} and a row stride of at "
+                                 f"least {w * n}, got strides {t.stride()}")
+            es, base = t.element_size(), t.data_ptr()
+            self._check_aligned(base, rs * es, es)
+            self._record = (base + idx[0] * es, base + idx[1] * es, base + idx[2] * es, rs * es, n * es, h, w, es,
+                            8 * es, 0, 0, 0, 0)
+        elif layout in image_ops.X2RGB10_LAYOUTS:
+            self._check_tensor(t, (torch.int32, torch.uint32), 2, f"(H, W) tensor of 32-bit words for {layout!r}")
+            h, w = t.shape
+            rs, ps = _unstepped(t, w, 1)
+            if ps != 1 or rs < w:
+                raise ValueError(f"RGBFrame {layout!r} needs column stride 1 and a row stride of at least {w}, got "
+                                 f"strides {t.stride()}")
+            base = t.data_ptr()
+            self._check_aligned(base, rs * 4, 4)
+            self._record = (base, base, base, rs * 4, 4, h, w, 4, 10, *image_ops.X2RGB10_LAYOUTS[layout], 0)
+        else:
+            raise ValueError(f"unknown RGBFrame layout {layout!r}: one of "
+                             f"{sorted(image_ops.RGB_PACKED_LAYOUTS) + sorted(image_ops.X2RGB10_LAYOUTS)}")
+        self.tensors = (t,)
+        self.layout, self.bits = layout, self._record[8]
+        self.shape = (h, w, 3)
+
+    @classmethod
+    def planar(cls, r: torch.Tensor, g: torch.Tensor, b: torch.Tensor, bits: int = 8) -> "RGBFrame":
+        if isinstance(bits, bool) or bits not in image_ops.RGB_PLANAR_BITS:
+            raise ValueError(f"RGBFrame.planar bits must be 8, 10, 12 or 16, got {bits!r}")
+        dtype = torch.uint8 if bits == 8 else torch.uint16
+        for p in (r, g, b):
+            cls._check_tensor(p, (dtype,), 2, f"(H, W) plane at {bits} bits")
+        if not (r.shape == g.shape == b.shape):
+            raise ValueError(f"RGBFrame.planar planes must share one shape, got {tuple(r.shape)}, {tuple(g.shape)} "
+                             f"and {tuple(b.shape)}")
+        strides = [_unstepped(p, 0, 0) for p in (r, g, b)]
+        if not (strides[0] == strides[1] == strides[2]):
+            raise ValueError(f"RGBFrame.planar planes must share their strides, got {r.stride()}, {g.stride()} and "
+                             f"{b.stride()}")
+        es = r.element_size()
+        rs, ps = strides[0]
+        for p in (r, g, b):
+            cls._check_aligned(p.data_ptr(), rs * es, es)
+        f = cls.__new__(cls)
+        h, w = r.shape
+        f._record = (r.data_ptr(), g.data_ptr(), b.data_ptr(), rs * es, ps * es, h, w, es, int(bits), 0, 0, 0, 0)
+        f.tensors = (r, g, b)
+        f.layout, f.bits = "planar", int(bits)
+        f.shape = (h, w, 3)
+        return f
+
+    @staticmethod
+    def _check_tensor(t, dtypes: tuple, ndim: int, what: str) -> None:
+        if not isinstance(t, torch.Tensor) or t.dtype not in dtypes or t.ndim != ndim or t.device.type != "cuda":
+            got = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+            want = " or ".join(str(d) for d in dtypes)
+            raise ValueError(f"RGBFrame takes a {ndim}-D CUDA {want} {what}, got {got}")
+        if min(t.stride(), default=0) < 0:
+            raise ValueError(f"RGBFrame tensors need non-negative strides, got {t.stride()}")
+        if not (1 <= t.shape[0] <= _MAX_SIDE and 1 <= t.shape[1] <= _MAX_SIDE):
+            raise ValueError(f"an RGB frame needs 1 to {_MAX_SIDE} rows and columns, got {tuple(t.shape)}")
+
+    @staticmethod
+    def _check_aligned(address: int, row_bytes: int, es: int) -> None:
+        if es > 1 and (address % es or row_bytes % es):
+            raise ValueError(f"RGBFrame {8 * es}-bit samples must start on {es}-byte boundaries: address offset "
+                             f"{address % es}, row pitch {row_bytes}")
+
+    def rgb_record(self) -> tuple:
+        """The FearFrameRGB record (r, g, b, row_stride, pixel_stride, H, W, container, bits, shift_r, shift_g,
+        shift_b, reserved): the addresses of the containers holding R, G and B of pixel (0, 0), the byte strides, the
+        size, the container's bytes, the code depth and each channel's shift."""
+        return self._record
+
+
+def tensor_rgb_record(t: torch.Tensor) -> tuple:
+    """The FearFrameRGB record of a uint8 (H, W, 3) RGB tensor (``frame_view`` as an 8-bit RGBFrame): channel c at
+    data + c * channel_stride."""
+    p, rs, ps, cs, h, w = frame_view(t)
+    return (p, p + cs, p + 2 * cs, rs, ps, h, w, 1, 8, 0, 0, 0, 0)
+
+
 def frame_kind(frame) -> str:
     """"yuv" for a YUV420Frame, YUV422Frame, YUV444Frame or V210Frame, "bayer" for a BayerFrame, "mono" for a
-    MonoFrame, "cuda" for a torch tensor (checked by ``check_device_frame``), "numpy" for anything else."""
+    MonoFrame, "rgb" for an RGBFrame (any channel order and container: BGR, BGRA / ABGR, x2rgb10, rgb48 / rgba64, planar
+    RGB; the kernels read its channels where they are), "cuda" for a torch tensor (checked by ``check_device_frame``),
+    "numpy" for anything else.  Host frames are always H x W x 3 RGB."""
+    if isinstance(frame, RGBFrame):
+        return "rgb"
     if isinstance(frame, (_YUVFrame, V210Frame)):
         return "yuv"
     if isinstance(frame, BayerFrame):
@@ -588,9 +717,11 @@ def uses_agc(frames, kind: str) -> bool:
 
 
 def check_device_frame(i: int, f, kind: str, device) -> None:
-    """The checks of a frame of kind "cuda", "yuv", "bayer" or "mono" (``frame_kind``): ValueError before any device
-    call."""
-    if kind in ("bayer", "mono"):
+    """The checks of a frame of kind "cuda", "yuv", "bayer", "mono" or "rgb" (``frame_kind``): ValueError before any
+    device call."""
+    if kind == "rgb":
+        check_device(i, device, *f.tensors)
+    elif kind in ("bayer", "mono"):
         check_device(i, device, f.t)
     elif kind == "yuv":
         check_device(i, device, *((f.t,) if isinstance(f, V210Frame) else (f.y, f.u, f.v)))
@@ -602,9 +733,11 @@ def write_records(table: np.ndarray, frames, name: str) -> None:
     """Write the records of device frames into rows of ``table`` (a numpy view of ``TABLE_DTYPES[name]``):
     FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr",
     FearFrameYCbCrV210 for "ycbcr_v210", FearFrameYCbCrHDR for "ycbcr_hdr", FearFrameBayer for "bayer", FearFrameMono
-    for "mono"."""
+    for "mono", FearFrameRGB for "rgb" (of RGBFrames and of CUDA tensors, ``tensor_rgb_record``)."""
     for i, f in enumerate(frames):
-        if name == "yuv":
+        if name == "rgb":
+            table[i] = f.rgb_record() if isinstance(f, RGBFrame) else tensor_rgb_record(f)
+        elif name == "yuv":
             table[i] = f.yuv_record()
         elif name == "ycbcr":
             table[i] = f.ycbcr_record()
@@ -677,9 +810,10 @@ class FEARMultiTracker:
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
         ``frames`` are all numpy arrays, all CUDA tensors, all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame,
-        V210Frame), all BayerFrames or all MonoFrames (see ``update``).  A target's padding colour is the mean colour of
-        its frame (of the converted RGB frame for a YUV frame, of the demosaiced 8-bit frame for a Bayer frame, of the
-        grey frame after gain control for a mono frame), from exact per-channel sums computed on the device."""
+        V210Frame), all BayerFrames, all MonoFrames, or RGBFrames and CUDA tensors (see ``update``).  A target's padding
+        colour is the mean colour of its frame (of the converted RGB frame for a YUV frame, of the demosaiced 8-bit frame
+        for a Bayer frame, of the grey frame after gain control for a mono frame, of the 8-bit RGB frame for an
+        RGBFrame), from exact per-channel sums computed on the device."""
         frames, kind = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
         if rects.ndim == 1 and rects.size == 4:
@@ -768,7 +902,9 @@ class FEARMultiTracker:
         ``BayerFrame``s (any patterns, depths and packings), never mixed with other kinds; their samples are read in
         place and give exactly what ``image_ops.bayer_to_rgb`` of their codes gives as numpy arrays.  ``frames`` may
         also be all ``MonoFrame``s (any depths, packings and gain controls), never mixed with other kinds; they give
-        exactly what ``image_ops.mono_to_rgb`` of their codes gives as numpy arrays.  Device frames must
+        exactly what ``image_ops.mono_to_rgb`` of their codes gives as numpy arrays.  ``frames`` may also be
+        ``RGBFrame``s (any layouts and depths) mixed freely with CUDA tensors, never with other kinds; they give exactly
+        what ``image_ops.rgb_frame_to_rgb`` of their samples gives as numpy arrays.  Device frames must
         be ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
@@ -803,27 +939,33 @@ class FEARMultiTracker:
         return torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
 
     def _check_frames(self, frames):
-        """-> (list of frames, their kind: "numpy", "cuda", "yuv", "bayer" or "mono").  Raises ValueError before any
-        device call."""
-        if isinstance(frames, (_YUVFrame, V210Frame, _RawFrame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
+        """-> (list of frames, their kind: "numpy", "cuda", "yuv", "bayer", "mono" or "rgb", the last for RGBFrames
+        with or without CUDA tensors).  Raises ValueError before any device call."""
+        if isinstance(frames, (_YUVFrame, V210Frame, _RawFrame, RGBFrame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
                                                           and frames.ndim == 3):
             frames = [frames]
         frames = list(frames)
         if not frames:
             raise ValueError("no frames given")
-        kind = frame_kind(frames[0])
-        if any(frame_kind(f) != kind for f in frames):
+        kinds = [frame_kind(f) for f in frames]
+        kind = kinds[0]
+        if set(kinds) == {"rgb", "cuda"}:  # RGBFrames and RGB tensors share the rgb table
+            kind = "rgb"
+        elif any(k != kind for k in kinds):
             if any(frame_kind(f) == "bayer" for f in frames):
                 raise ValueError("BayerFrames cannot share a call with other kinds of frames (numpy arrays, CUDA "
                                  "tensors, YUV frames): pass all of a call's frames as BayerFrames")
             if any(frame_kind(f) == "mono" for f in frames):
                 raise ValueError("MonoFrames cannot share a call with other kinds of frames (numpy arrays, CUDA "
                                  "tensors, YUV frames): pass all of a call's frames as MonoFrames")
+            if "rgb" in kinds:
+                raise ValueError("RGBFrames can share a call only with CUDA uint8 RGB tensors, not with numpy arrays or "
+                                 "YUV frames: pass the call's frames as RGBFrames or CUDA tensors")
             raise ValueError("frames of one call must be all numpy arrays, all CUDA tensors or all YUV frames "
                              "(YUV420Frame, YUV422Frame, YUV444Frame, V210Frame), not a mix")
         for i, f in enumerate(frames):
             if kind != "numpy":
-                check_device_frame(i, f, kind, self._device)
+                check_device_frame(i, f, kinds[i], self._device)
             elif not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
                     or f.shape[0] < 1 or f.shape[1] < 1:
                 what = f"{f.dtype} {f.shape}" if isinstance(f, np.ndarray) else type(f).__name__
@@ -858,7 +1000,7 @@ class FEARMultiTracker:
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
             frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, ycbcr_pin=None,
             ycbcr=None, ycbcr_v210_pin=None, ycbcr_v210=None, ycbcr_hdr_pin=None, ycbcr_hdr=None, bayer_pin=None,
-            bayer=None, mono_pin=None, mono=None, sums_pin=None, sums=None)
+            bayer=None, mono_pin=None, mono=None, rgb_pin=None, rgb=None, sums_pin=None, sums=None)
         return b
 
     def _upload_frames(self, frames, kind: str, dev: torch.device) -> str:
@@ -867,9 +1009,10 @@ class FEARMultiTracker:
         frames of which any has a transfer (PQ, HLG), else "ycbcr_v210" (FearFrameYCbCrV210 records) for YUV frames of
         which any is a V210Frame, "ycbcr" (FearFrameYCbCr records) for other YUV frames of which any is
         4:2:2 or 4:4:4, "bayer" (FearFrameBayer records) for BayerFrames, "mono" (FearFrameMono records) for
-        MonoFrames, "views" (FearFrameView records) otherwise.  Numpy frames are packed into the pinned staging buffer
+        MonoFrames, "rgb" (FearFrameRGB records) for a call with any RGBFrame, "views" (FearFrameView records)
+        otherwise.  Numpy frames are packed into the pinned staging buffer
         first and sent with one host-to-device copy (the packed layout is recomputed only when their shapes change);
-        CUDA tensors, YUV planes, v210 surfaces, Bayer mosaics and mono frames are used where they are."""
+        CUDA tensors, YUV planes, v210 surfaces, Bayer mosaics, mono frames and RGB frames are used where they are."""
         b, num_frames = self._buf, len(frames)
         name = "views"
         if kind == "yuv":
@@ -878,7 +1021,7 @@ class FEARMultiTracker:
                 name = "ycbcr_v210"
             if any(f.transfer is not None for f in frames):
                 name = "ycbcr_hdr"
-        elif kind in ("bayer", "mono"):
+        elif kind in ("bayer", "mono", "rgb"):
             name = kind
         dtype = TABLE_DTYPES[name]
         nbytes = num_frames * dtype.itemsize
@@ -933,7 +1076,7 @@ class FEARMultiTracker:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
         keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records, YCbCr
-        records of any subsampling, YCbCr / v210 records, HDR records, Bayer records or mono records) and
+        records of any subsampling, YCbCr / v210 records, HDR records, Bayer records, mono records or RGB records) and
         its buffer, whether the step starts with the mono range kernel (``agc``), and the net's generation.
         ``cuda_graph=False`` in the tracking config keeps eager launches."""
         key = (n, num_frames, table, self._buf[table].data_ptr(), agc)

@@ -8,11 +8,12 @@ of the reference's observable behaviour); network + decode run in libfear_b200 a
 48-byte box record comes back per frame.  With ``gpu_crop: true`` the numpy frame is uploaded and cropped on the device.
 
 Frames already in GPU memory -- uint8 (H, W, 3) CUDA tensors with any non-negative strides, YUV420Frame /
-YUV422Frame / YUV444Frame decoder surfaces, V210Frame capture buffers, BayerFrame raw mosaics and MonoFrame
-single-channel frames -- are read in place:
+YUV422Frame / YUV444Frame decoder surfaces, V210Frame capture buffers, BayerFrame raw mosaics, MonoFrame
+single-channel frames and RGBFrame BGR / BGRA / ABGR, 10-bit, 16-bit and planar RGB frames -- are read in place:
 the crop, the conversion to RGB (or the demosaic), the network and the decode (plain or smoothed) run on the device, and
 the tracker returns exactly what it returns for the same pixels as a numpy array (``image_ops.yuv_to_rgb`` of a YUV
-frame's planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes, ``image_ops.mono_to_rgb`` of a mono frame's).
+frame's planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes, ``image_ops.mono_to_rgb`` of a mono frame's,
+``image_ops.rgb_frame_to_rgb`` of an RGB frame's samples).
 """
 from collections import deque
 from typing import Any, Dict, Optional, Tuple, Union
@@ -27,7 +28,7 @@ from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY
 
 
 # byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrHDR; a
-# FearFrameBayer is 40 bytes, a FearFrameMono 48), a FearTarget, then five float64 inputs of fear_decode_smooth
+# FearFrameBayer is 40 bytes, a FearFrameMono 48, a FearFrameRGB 72), a FearTarget, then five float64 inputs of fear_decode_smooth
 _TARGET_OFFSET = 104
 _SMOOTH_OFFSET = _TARGET_OFFSET + 64
 _DEVICE_INPUT_BYTES = _SMOOTH_OFFSET + 5 * 8
@@ -111,20 +112,22 @@ class FEARTracker(Tracker):
     """The reference's single-object tracker.  ``initialize``, ``update`` and ``get_template_features`` take a frame as
     a uint8 (H, W, 3) RGB numpy array, as a uint8 (H, W, 3) CUDA tensor on the tracker's device (any non-negative
     strides: ``rgba[..., :3]``, ``chw.permute(1, 2, 0)``, a region of interest), or as a YUV420Frame, YUV422Frame,
-    YUV444Frame, V210Frame, BayerFrame or MonoFrame whose planes, words or samples are on the tracker's device; the
-    kind may change from one call to the next.
+    YUV444Frame, V210Frame, BayerFrame, MonoFrame or RGBFrame whose planes, words or samples are on the tracker's
+    device; the kind may change from one call to the next.
 
     Numpy frames take the host crop, or with ``gpu_crop: true`` an upload and the device crop.  Device frames always
     take the device step, whatever ``gpu_crop`` says, since the host crop could only read them after copying them back:
     fear_crop_targets_view_u8 (tensors), fear_crop_targets_ycbcr_u8 (YUV frames, converted to RGB inside the crop),
     fear_crop_targets_ycbcr_v210_u8 (v210 frames, unpacked and converted inside the crop), fear_crop_targets_bayer_u8
-    (Bayer frames, demosaiced inside the crop) or fear_crop_targets_mono_u8 (mono frames, mapped to grey inside the
-    crop, after fear_frame_range_mono when the frame has gain control) makes the search crop, then the network and the
+    (Bayer frames, demosaiced inside the crop), fear_crop_targets_mono_u8 (mono frames, mapped to grey inside the
+    crop, after fear_frame_range_mono when the frame has gain control) or fear_crop_targets_rgb_u8 (RGB frames in any
+    channel order and container, mapped to 8 bits inside the crop) makes the search crop, then the network and the
     decode, plain or with ``smooth: true`` the smoothed one, run as one CUDA graph and one 48-byte record comes back.
     The results, ``tracking_state`` included, are those of the same tracker fed the same pixels as numpy arrays
     (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its ``CHROMA_SHIFT``, of a v210 frame's
     ``image_ops.v210_unpack`` planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes, ``image_ops.mono_to_rgb``
-    of a mono frame's codes with its ``agc``).  Device frames must be ready on the current CUDA stream; every call
+    of a mono frame's codes with its ``agc``, ``image_ops.rgb_frame_to_rgb`` of an RGB frame's samples).  Device
+    frames must be ready on the current CUDA stream; every call
     synchronises it before it returns, so they only need to live for the call.
     ``host_normalize: true`` takes numpy frames only."""
 
@@ -282,7 +285,7 @@ class FEARTracker(Tracker):
 
     # -- device frames: CUDA tensors and YUV frames, read in place by the crop-targets entry points (one target) --
     def _frame_kind(self, image) -> str:
-        """"numpy", "cuda", "yuv", "bayer" or "mono" (multi_tracker.frame_kind).  A device frame is checked here, before
+        """"numpy", "cuda", "yuv", "bayer", "mono" or "rgb" (multi_tracker.frame_kind).  A device frame is checked here, before
         any device call or state change: NotImplementedError with ``host_normalize``, ValueError when malformed."""
         kind = multi_tracker.frame_kind(image)
         if kind == "numpy":
@@ -296,9 +299,9 @@ class FEARTracker(Tracker):
     def _device_frame_state(self) -> dict:
         """Buffers of the device-frame step, separate from the gpu_crop path's.  ``inputs`` (pinned) and ``dev_in``
         share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView, a
-        FearFrameYCbCr, a FearFrameYCbCrV210, a FearFrameYCbCrHDR, a FearFrameBayer or a FearFrameMono) at byte 0, the
-        FearTarget at byte 104, fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr as float64 at
-        byte 168; then, on the device only, the score_size x score_size window."""
+        FearFrameYCbCr, a FearFrameYCbCrV210, a FearFrameYCbCrHDR, a FearFrameBayer, a FearFrameMono or a FearFrameRGB)
+        at byte 0, the FearTarget at byte 104, fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr
+        as float64 at byte 168; then, on the device only, the score_size x score_size window."""
         from . import _lib
 
         dev = self._device()
@@ -327,8 +330,9 @@ class FEARTracker(Tracker):
         """Write the frame's record, the target (frame 0, ``bbox``, padding colour ``pad``) and, given ``prev_size``,
         the smooth scalars into the pinned inputs and send them with one host-to-device copy.  Returns the table name:
         "views" for a tensor, "ycbcr_hdr" for a YUV frame with a transfer (PQ, HLG), "ycbcr_v210" for another
-        V210Frame, "ycbcr" for every other YUV frame, "bayer" for a BayerFrame, "mono" for a MonoFrame."""
-        table = kind if kind in ("bayer", "mono") else "views"
+        V210Frame, "ycbcr" for every other YUV frame, "bayer" for a BayerFrame, "mono" for a MonoFrame, "rgb" for an
+        RGBFrame."""
+        table = kind if kind in ("bayer", "mono", "rgb") else "views"
         if kind == "yuv":
             table = "ycbcr_v210" if isinstance(image, multi_tracker.V210Frame) else "ycbcr"
             if image.transfer is not None:

@@ -51,6 +51,9 @@
  *                         into the table for their min-max gain control (thermal cores, mono cameras)
  *   fear_crop_targets_mono_u8 / fear_advance_targets_mono / fear_frame_sums_mono_u8   the same three on FearFrameMono
  *                         tables (8 to 16 bits, MIPI RAW10 / RAW12), each tap mapped to grey (g, g, g) inside the crop
+ *   fear_crop_targets_rgb_u8 / fear_advance_targets_rgb / fear_frame_sums_rgb_u8   the same three on RGB frames in any
+ *                         channel order located by FearFrameRGB (BGR / BGRA / ABGR, x2rgb10, rgb48 / rgba64, planar
+ *                         gbrp at 8 to 16 bits), each tap's channels read and mapped to 8 bits inside the crop
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -321,6 +324,28 @@ typedef struct FearFrameMono {                /* 48 bytes                       
   int32_t agc;                                /* 0: none; FEAR_AGC_MINMAX: min-max gain control                 */
   int32_t lo, hi;                             /* the frame's code range, written by fear_frame_range_mono       */
 } FearFrameMono;
+/* An RGB frame whose three channels are samples of one fixed-size little-endian container at a common row and pixel
+ * stride (72 bytes): packed rgb24 / bgr24, RGBA / BGRA / ARGB / ABGR (and their X variants), rgb48le / rgba64le,
+ * x2rgb10le / x2bgr10le (DRM XRGB2101010, DXGI R10G10B10A2) and planar gbrp at 8 to 16 bits.  Channel c of pixel
+ * (y, x) is the container at c_ptr + y * row_stride + x * pixel_stride (c_ptr = r, g or b); its code is
+ * (container value >> shift_c) & (2^bits - 1), mapped to 8 bits as the code itself at 8 bits and above 8 bits as
+ * FearFrameBayer maps a channel, min(max(rint(255 * (v * (1 / (2^bits - 1)))), 0), 255) in float64.  Full range only;
+ * alpha and X bytes and the spare bits of a container are never read into the result.  Readable combinations:
+ *   container 1   bits 8, every shift 0, any addresses and strides (byte loads, no float64 work)
+ *   container 2   bits 10, 12 or 16, each shift in [0, 16 - bits]; every channel address and both strides even
+ *   container 4   bits 10, the shifts a permutation of {0, 10, 20}, r == g == b, the address and both strides
+ *                 multiples of 4 (one word load per tap)
+ * An entry is treated like a frame index outside [0, F) when any other combination is given, a channel address is
+ * null, a stride is negative, or H or W is below 1. */
+typedef struct FearFrameRGB {                 /* 72 bytes                                                       */
+  const uint8_t *r, *g, *b;                   /* device address of the container holding R / G / B of (0, 0)    */
+  int64_t row_stride, pixel_stride;           /* bytes, >= 0, shared by the three channels                      */
+  int32_t H, W;                               /* size in pixels, both >= 1                                      */
+  int32_t container;                          /* bytes per container: 1, 2 (LE uint16) or 4 (LE uint32)         */
+  int32_t bits;                               /* code depth                                                     */
+  int32_t shift_r, shift_g, shift_b;          /* code of channel c = (container value >> shift_c) & (2^bits - 1) */
+  int32_t reserved;
+} FearFrameRGB;
 typedef struct FearTarget {      /* 64 bytes                                                         */
   int32_t frame;                 /* index into the frame table                                       */
   int32_t x, y, w, h;            /* current box in frame pixels (TrackingState.bbox)                 */
@@ -540,6 +565,15 @@ int fear_crop_targets_mono_u8(const FearFrameMono* d_views, int F, FearTarget* d
 int fear_advance_targets_mono(const FearBox* d_boxes, const FearFrameMono* d_views, int F, FearTarget* d_targets,
                               int N, int instance_size, void* stream);
 int fear_frame_sums_mono_u8(const FearFrameMono* d_views, int F, uint64_t* d_sums, void* stream);
+/* The same three on FearFrameRGB tables: RGB frames in any channel order, 8-, 10-, 12- or 16-bit containers, packed
+ * or planar, read where they are, each tap's channels fetched and mapped to 8 bits inside the crop (see FearFrameRGB).
+ * Same semantics and FEAR_EINVAL rules as the *_mono entry points; an entry the kernels cannot read gets a
+ * padding-colour crop, keeps its box and sums to 0. */
+int fear_crop_targets_rgb_u8(const FearFrameRGB* d_views, int F, FearTarget* d_targets, int N, double offset,
+                             int out_size, uint8_t* d_crops, void* stream);
+int fear_advance_targets_rgb(const FearBox* d_boxes, const FearFrameRGB* d_views, int F, FearTarget* d_targets, int N,
+                             int instance_size, void* stream);
+int fear_frame_sums_rgb_u8(const FearFrameRGB* d_views, int F, uint64_t* d_sums, void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
