@@ -1350,6 +1350,36 @@ extern "C" int fear_frame_sums_rgb_u8(const FearFrameRGB* d_views, int F, uint64
   return launch_frame_sums(d_views, RGBFrames{d_views}, F, d_sums, stream);
 }
 
+// A step over some targets only: their rows and templates gathered into compact step buffers, stepped there by the
+// entry points above, and their boxes scattered back.
+static int check_select_args(int N, int M) {
+  if (N < 1) return set_err(FEAR_EINVAL, "target row count must be >= 1 (got %d)", N);
+  if (M < 1 || M > 65535) return set_err(FEAR_EINVAL, "step row count must be in [1, 65535] (got %d)", M);
+  return 0;
+}
+
+extern "C" int fear_gather_targets(const FearTarget* d_targets, int N, const float* d_templates,
+                                   const int32_t* d_select, int M, FearTarget* d_step_targets,
+                                   float* d_step_templates, void* stream) {
+  if (!d_targets || !d_templates || !d_select || !d_step_targets || !d_step_templates)
+    return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_select_args(N, M)) return r;
+  if (reinterpret_cast<uintptr_t>(d_templates) % 16 || reinterpret_cast<uintptr_t>(d_step_templates) % 16)
+    return set_err(FEAR_EINVAL, "template buffers must be 16-byte aligned");
+  gather_targets_kernel<<<dim3(kGatherCtasPerRow, M), kGatherThreads, 0, (cudaStream_t)stream>>>(
+      d_targets, N, reinterpret_cast<const float4*>(d_templates), d_select, d_step_targets,
+      reinterpret_cast<float4*>(d_step_templates));
+  return check_launch("gather_targets_kernel");
+}
+
+extern "C" int fear_scatter_targets(const FearTarget* d_step_targets, const int32_t* d_select, int M,
+                                    FearTarget* d_targets, int N, void* stream) {
+  if (!d_step_targets || !d_select || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_select_args(N, M)) return r;
+  scatter_targets_kernel<<<(M + 127) / 128, 128, 0, (cudaStream_t)stream>>>(d_step_targets, d_select, M, d_targets, N);
+  return check_launch("scatter_targets_kernel");
+}
+
 extern "C" int fear_decode_sized(const float* d_bbox, const float* d_cls, int B, int side, int apply_sigmoid,
                                  FearBox* d_boxes, void* stream) {
   if (!d_bbox || !d_cls || !d_boxes || B < 1) return set_err(FEAR_EINVAL, "bad argument");

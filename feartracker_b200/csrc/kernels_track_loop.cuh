@@ -9,6 +9,8 @@
 //   frame_sums_u8_kernel     exact per-channel sums of whole frames                    (np.mean of the padding colour)
 //   frame_range_mono_kernel  code range of single-channel frames, for their gain       (the smin, smax of
 //                                                                                       cv2.normalize(NORM_MINMAX))
+//   gather_targets_kernel    selected FearTarget rows and templates -> compact step buffers (a step over the targets
+//   scatter_targets_kernel   the stepped boxes and context boxes -> their FearTarget rows    of some streams only)
 //
 // The first three are templates over where the frames are and what they hold: a packed buffer + FearFrame table
 // (PackedFrames) or a FearFrameView table of strided RGB frames anywhere in device memory (FrameViews), both read
@@ -890,6 +892,65 @@ __global__ void __launch_bounds__(kFrameSumThreads) frame_range_mono_kernel(Fear
       atomicMax(&p->hi, hi);
     }
   }
+}
+
+constexpr int kTemplateVec4 = 256 * 8 * 8 / 4;  // float4s of one (256, 8, 8) fp32 template: 64 KB
+constexpr int kGatherCtasPerRow = 4;            // CTAs copying one template
+constexpr int kGatherThreads = 256;
+constexpr int kGatherVec4PerThread = kTemplateVec4 / (kGatherCtasPerRow * kGatherThreads);
+static_assert(kGatherVec4PerThread * kGatherCtasPerRow * kGatherThreads == kTemplateVec4, "gather tiling");
+
+// grid (kGatherCtasPerRow, M), kGatherThreads threads.  Step row i takes target row select[2 i]: CTA (c, i) copies
+// quarter c of its template with 16-byte loads and stores (all loads issued before the stores), and thread 0 of CTA
+// (0, i) writes the FearTarget with frame = select[2 i + 1].  A row outside [0, N) gives an inert step row: a zero
+// FearTarget with frame = -1 and a zero template.
+__global__ void __launch_bounds__(kGatherThreads) gather_targets_kernel(const FearTarget* __restrict__ targets, int N,
+                                                                        const float4* __restrict__ templates,
+                                                                        const int32_t* __restrict__ select,
+                                                                        FearTarget* __restrict__ step_targets,
+                                                                        float4* __restrict__ step_templates) {
+  const int i = blockIdx.y;
+  const int row = __ldg(select + 2 * i);
+  const bool valid = row >= 0 && row < N;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    FearTarget t = {};
+    t.frame = -1;
+    if (valid) {
+      t = targets[row];
+      t.frame = __ldg(select + 2 * i + 1);
+    }
+    step_targets[i] = t;
+  }
+  const int k0 = blockIdx.x * (kGatherThreads * kGatherVec4PerThread) + threadIdx.x;
+  float4* dst = step_templates + (long long)i * kTemplateVec4 + k0;
+  float4 v[kGatherVec4PerThread];
+#pragma unroll
+  for (int j = 0; j < kGatherVec4PerThread; ++j)
+    v[j] = valid ? __ldg(templates + (long long)row * kTemplateVec4 + k0 + j * kGatherThreads)
+                 : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int j = 0; j < kGatherVec4PerThread; ++j) dst[j * kGatherThreads] = v[j];
+}
+
+// One thread per step row: x, y, w, h, cx, cy, cw, ch of step row i go back to target row select[2 i]; frame, the
+// padding colour and the reserved words of the target row are not written.  Rows outside [0, N) are skipped.
+__global__ void __launch_bounds__(128) scatter_targets_kernel(const FearTarget* __restrict__ step_targets,
+                                                              const int32_t* __restrict__ select, int M,
+                                                              FearTarget* __restrict__ targets, int N) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M) return;
+  const int row = select[2 * i];
+  if (row < 0 || row >= N) return;
+  const FearTarget s = step_targets[i];
+  FearTarget* t = targets + row;
+  t->x = s.x;
+  t->y = s.y;
+  t->w = s.w;
+  t->h = s.h;
+  t->cx = s.cx;
+  t->cy = s.cy;
+  t->cw = s.cw;
+  t->ch = s.ch;
 }
 
 }  // namespace fear

@@ -3,7 +3,12 @@
     trk = FEARMultiTracker(net, cuda_id=0, max_targets=64, **FEAR_XS_TRACKER_KWARGS)
     ids = trk.add(frames, rects, streams=None)   # frames: one HxWx3 uint8 array or a list of F; streams -> frame index
     out = trk.update(frames)                      # {"bbox": (N,4) int64, "score": (N,) float32, "ids": (N,) int64}
+    out = trk.update({3: f3, 17: f17})            # only the streams that have a new frame: their M targets' results
     trk.remove(ids); trk.reset()
+
+A list holds one frame of every stream.  Streams that do not tick together (cameras at different rates, a stalled or
+reconnecting camera, frames batched as they arrive) pass a mapping {stream id: frame} of the streams at hand to update
+and add: only the targets of those streams are stepped, and every other target's state and template stay as they were.
 
 Frames are numpy arrays in host memory, uint8 (H, W, 3) CUDA tensors already on the tracker's device, strided views
 included (t[..., :3] of an RGBA surface, t.permute(1, 2, 0) of a CHW tensor, t[y0:y1, x0:x1]), or YUV frames on the
@@ -45,9 +50,21 @@ puts all its frames, RGBFrames and CUDA tensors alike, into an eighth, of FearFr
 points; RGBFrames cannot share a call with numpy arrays or YUV, Bayer or mono frames.  The host then reads back
 the boxes and scores.  The launch count of a step depends neither on N nor on the kind of frames, with one exception:
 a step on MonoFrames with gain control launches the range kernel too (49 launches instead of 48).
+
+A step over the M targets of a mapping's streams runs on compact buffers of max_targets rows:
+
+    fear_gather_targets -> [fear_frame_range_mono] -> crop (M) -> fear_track_u8 (B = M, Bz = M) -> advance (M)
+                        -> fear_scatter_targets
+
+The host writes the (target row, frame index) pair of each selected target into a fixed selection buffer, sent with the
+frame table; gather copies those rows (frame replaced by the index) and their templates into the step buffers, and
+scatter writes the new boxes and context boxes back.  The step is two launches longer than a list step whatever M is,
+and is replayed from a small cache of captured graphs keyed by its shape, kept apart from the list step's graph.
 """
 import math
 import warnings
+from collections import OrderedDict
+from collections.abc import Mapping
 from typing import Any, Dict, Optional, Sequence, Union
 
 import numpy as np
@@ -57,6 +74,11 @@ from . import _lib, image_ops
 
 _FRAME_ALIGN = 16  # byte alignment of each frame inside the packed buffer
 _MAX_SIDE = 2 ** 31 - 1  # H and W are int32 in FearFrameView, FearFrameYUV and FearFrameYCbCr
+_MAX_STREAM = 2 ** 31 - 1  # stream ids are int32 in FearTarget.frame
+# Captured subset-step graphs kept per tracker.  A graph is keyed by the step's shape (step rows, frame count, table),
+# not by which streams are in it, so a steady pattern of subsets uses one or two keys; 8 covers patterns whose subset
+# sizes keep changing, and each graph holds little device memory (its box output; the network's workspace is shared).
+SUBSET_GRAPHS = 8
 # the entry points that read each frame table: frame sums, target crops, box advance
 ENTRY_POINTS = {
     "views": ("fear_frame_sums_u8", "fear_crop_targets_view_u8", "fear_advance_targets_view"),
@@ -688,6 +710,12 @@ def frame_kind(frame) -> str:
     return "cuda" if isinstance(frame, torch.Tensor) else "numpy"
 
 
+def _positions(keys: np.ndarray, streams: np.ndarray) -> np.ndarray:
+    """The index in ``keys`` (distinct stream ids) of each of ``streams``, every one of which is in ``keys``."""
+    order = np.argsort(keys)
+    return order[np.searchsorted(keys[order], streams)]
+
+
 def check_device(i: int, device, *tensors: torch.Tensor) -> None:
     """ValueError unless every tensor is on the tracker's CUDA device; ``device()`` gives that device and is called
     only once a tensor is known to be on some CUDA device."""
@@ -785,6 +813,8 @@ class FEARMultiTracker:
         self._graph_gen = None
         self._graph_ok = True
         self._calls = 0
+        self._subset_graphs = OrderedDict()  # subset step graphs: key -> {"calls", "graph", "boxes"}, LRU order
+        self._subset_gen = None  # the net's generation the cached subset graphs were captured at
         self.reset()
 
     # ------------------------------------------------------------------ public API
@@ -810,25 +840,35 @@ class FEARMultiTracker:
         current frame is ``frames[streams[i]]``.  Returns the new targets' ids.
 
         ``frames`` are all numpy arrays, all CUDA tensors, all YUV frames (YUV420Frame, YUV422Frame, YUV444Frame,
-        V210Frame), all BayerFrames, all MonoFrames, or RGBFrames and CUDA tensors (see ``update``).  A target's padding
-        colour is the mean colour of its frame (of the converted RGB frame for a YUV frame, of the demosaiced 8-bit frame
-        for a Bayer frame, of the grey frame after gain control for a mono frame, of the 8-bit RGB frame for an
-        RGBFrame), from exact per-channel sums computed on the device."""
-        frames, kind = self._check_frames(frames)
+        V210Frame), all BayerFrames, all MonoFrames, or RGBFrames and CUDA tensors (see ``update``).  ``frames`` may
+        also be a mapping {stream id: frame} of the streams at hand (ids ints in [0, 2^31 - 1], possibly sparse, such as
+        cameras 3 and 17); ``streams[i]`` is then a key of it (the default stream 0 must be one), and only its frames
+        are read.  A target's padding colour is the mean colour of its frame (of the converted RGB frame for a YUV
+        frame, of the demosaiced 8-bit frame for a Bayer frame, of the grey frame after gain control for a mono frame,
+        of the 8-bit RGB frame for an RGBFrame), from exact per-channel sums computed on the device."""
+        keys = None
+        if isinstance(frames, Mapping):
+            keys, frames, kind = self._check_mapping(frames)
+        else:
+            frames, kind = self._check_frames(frames)
         rects = np.asarray(rects, dtype=np.float64)
         if rects.ndim == 1 and rects.size == 4:
             rects = rects[None]
         if rects.ndim != 2 or rects.shape[1] != 4:
             raise ValueError(f"rects must be (n, 4) [x, y, w, h], got shape {rects.shape}")
         n = rects.shape[0]
-        streams = self._check_streams(np.zeros(n, dtype=np.int64) if streams is None else streams, n, len(frames))
+        streams = np.zeros(n, dtype=np.int64) if streams is None else streams
+        if keys is None:
+            streams = pos = self._check_streams(streams, n, len(frames))
+        else:
+            streams, pos = self._check_mapping_streams(streams, n, keys)
         if len(self._ids) + n > self.max_targets:
             raise ValueError(f"{len(self._ids)} + {n} targets exceed max_targets = {self.max_targets}")
         if n == 0:
             return np.zeros(0, dtype=np.int64)
         cfg = self.tracking_config
         recs = np.zeros((n, _lib.TARGET_INTS), dtype=np.int32)
-        for i, (rect, s) in enumerate(zip(rects, streams)):
+        for i, (rect, s) in enumerate(zip(rects, pos)):  # the template crop reads frame index s of this call's table
             box = image_ops.clamp_bbox(rect, tuple(frames[s].shape))
             ctx = image_ops.context_box(box, cfg["template_bbox_offset"])
             inner = image_ops.trim_box([box[0] - ctx[0], box[1] - ctx[1], box[2], box[3]], (ctx[3], ctx[2]))
@@ -856,7 +896,7 @@ class FEARMultiTracker:
             sums = b["sums_pin"].numpy()[:num_frames].view(np.uint64)
             pixels = np.array([f.shape[0] * f.shape[1] for f in frames], dtype=np.float64)
             pads = np.clip(np.rint(sums / pixels[:, None]), 0, 255).astype(np.int32)
-            recs[:, 9:12] = pads[streams]
+            recs[:, 9:12] = pads[pos]
             n0 = len(self._ids)
             b["state"][n0:n0 + n].copy_(torch.from_numpy(recs).pin_memory(), non_blocking=True)
             size = int(cfg["template_size"])
@@ -865,6 +905,9 @@ class FEARMultiTracker:
                                              float(cfg["template_bbox_offset"]), size, crops.data_ptr(),
                                              stream.cuda_stream), crop_fn)
             b["zf"][n0:n0 + n].copy_(self.net.get_features(crops))
+            if keys is not None:  # the rows keep their stream ids, not this call's frame indices
+                b["state"][n0:n0 + n, 0].copy_(torch.from_numpy(streams.astype(np.int32)).pin_memory(),
+                                               non_blocking=True)
             stream.synchronize()  # the pinned staging buffers are reused by the next call
         new_ids = np.arange(self._next_id, self._next_id + n, dtype=np.int64)
         self._next_id += n
@@ -887,9 +930,19 @@ class FEARMultiTracker:
         self._ids, self._streams = self._ids[keep], self._streams[keep]
 
     def update(self, frames) -> Dict[str, np.ndarray]:
-        """One frame of every stream -> the new box and score of every target, in the order of ``ids``.
+        """One frame of every stream -> the new box and score of every target, in the order of ``ids``; or the frames
+        of some streams -> the new boxes and scores of their targets only.
 
-        ``frames`` (one frame or a list of F, stream i's frame at index i) are all ``np.ndarray``, all
+        ``frames`` is one frame, a list of F (stream i's frame at index i), or a mapping {stream id: frame} of the
+        streams that have a new frame, for streams that do not tick together (cameras at different rates, a stalled
+        stream, frames batched as they arrive).  With a mapping only the targets of its streams are stepped, and the
+        result holds their "bbox", "score" and "ids" alone, in the order of ``ids``; every other target's state and
+        template stay exactly as they were, so each target's trajectory is that of its own tracker fed the frames its
+        stream delivered.  Keys are ints in [0, 2^31 - 1]; a key with no targets is allowed (its frame is checked, not
+        read); a mapping that selects no target returns empty arrays without a device call.  The values follow the
+        rules of a list below.
+
+        The frames are all ``np.ndarray``, all
         ``torch.Tensor`` or all YUV frames (``YUV420Frame``, ``YUV422Frame``, ``YUV444Frame``, mixed freely); the kind
         may change from one call to the next.  A tensor frame is uint8 of shape (H, W, 3) on the tracker's CUDA device,
         with any non-negative strides: views are read as they are, nothing is copied.  A YUV frame's planes must be on
@@ -908,6 +961,8 @@ class FEARMultiTracker:
         be ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
+        if isinstance(frames, Mapping):
+            return self._update_streams(*self._check_mapping(frames))
         frames, kind = self._check_frames(frames)
         n = len(self._ids)
         if n and int(self._streams.max()) >= len(frames):
@@ -928,6 +983,54 @@ class FEARMultiTracker:
         return dict(bbox=state[:, 1:5].astype(np.int64), score=rec["score"].astype(np.float32), ids=self._ids.copy())
 
     # ------------------------------------------------------------------ internals
+    def _update_streams(self, keys: np.ndarray, frames: list, kind: str) -> Dict[str, np.ndarray]:
+        """``update`` of a mapping: step the targets whose stream is in ``keys`` (the mapping's stream ids, in the order
+        of ``frames``) on compact step rows, through the selection (target row, frame index) pairs."""
+        rows = np.flatnonzero(np.isin(self._streams, keys))  # ascending: the order of ids
+        m = rows.size
+        if m == 0:
+            return dict(bbox=np.zeros((0, 4), dtype=np.int64), score=np.zeros(0, dtype=np.float32),
+                        ids=np.zeros(0, dtype=np.int64))
+        dev = self._device()
+        with torch.cuda.device(dev):
+            b = self._buffers(dev)
+            table = self._upload_frames(frames, kind, dev)
+            sel = b["select_pin"].numpy()
+            sel[:m, 0] = rows
+            sel[:m, 1] = _positions(keys, self._streams[rows])
+            b["select"][:m].copy_(b["select_pin"][:m], non_blocking=True)
+            boxes = self._run_subset_step(m, len(frames), table, dev, uses_agc(frames, kind))
+            b["state_pin"][:m].copy_(b["step_state"][:m], non_blocking=True)
+            b["box_pin"][:m].copy_(boxes, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+        state = b["state_pin"].numpy()[:m]
+        rec = b["box_pin"].numpy()[:m].view(_lib.BOX_DTYPE).reshape(-1)
+        return dict(bbox=state[:, 1:5].astype(np.int64), score=rec["score"].astype(np.float32), ids=self._ids[rows])
+
+    def _check_mapping(self, frames: Mapping):
+        """-> (stream ids (F,) int64, list of frames, their kind) of a {stream id: frame} mapping, in its order.  Raises
+        ValueError before any device call."""
+        keys = list(frames)
+        for k in keys:
+            if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 0 <= k <= _MAX_STREAM:
+                raise ValueError(f"stream ids must be ints in [0, {_MAX_STREAM}], got {k!r}")
+        if not keys:
+            raise ValueError("no frames given")
+        frames, kind = self._check_frames([frames[k] for k in keys])
+        return np.array(keys, dtype=np.int64), frames, kind
+
+    @staticmethod
+    def _check_mapping_streams(streams, n: int, keys: np.ndarray):
+        """-> (stream ids (n,) int64, their frame indices in the mapping) of ``add``'s ``streams`` for a mapping."""
+        s = np.asarray(streams)
+        if s.shape != (n,) or (s.size and not np.issubdtype(s.dtype, np.integer)):
+            raise ValueError(f"streams must be ({n},) integer stream ids, got {s.dtype} {s.shape}")
+        s = s.astype(np.int64)
+        missing = np.setdiff1d(s, keys)
+        if missing.size:
+            raise ValueError(f"streams {missing.tolist()} are not keys of the frames mapping {keys.tolist()}")
+        return s, _positions(keys, s)
+
     def _device(self) -> torch.device:
         if not torch.cuda.is_available():
             raise RuntimeError("FEARMultiTracker (H100) needs a CUDA device: there is no CPU path")
@@ -996,6 +1099,11 @@ class FEARMultiTracker:
             zf=torch.zeros((m, 256, 8, 8), dtype=torch.float32, device=dev),
             crops=torch.empty((m, size, size, 3), dtype=torch.uint8, device=dev),
             tcrops=torch.empty((m, tsize, tsize, 3), dtype=torch.uint8, device=dev),
+            # the compact rows and templates of a subset step, and its selection: (target row, frame index) pairs
+            step_state=torch.zeros((m, _lib.TARGET_INTS), dtype=torch.int32, device=dev),
+            step_zf=torch.zeros((m, 256, 8, 8), dtype=torch.float32, device=dev),
+            select=torch.zeros((m, 2), dtype=torch.int32, device=dev),
+            select_pin=torch.zeros((m, 2), dtype=torch.int32).pin_memory(),
             state_pin=torch.empty((m, _lib.TARGET_INTS), dtype=torch.int32).pin_memory(),
             box_pin=torch.empty((m, _lib.BOX_DTYPE.itemsize), dtype=torch.uint8).pin_memory(),
             frames_pin=None, frames=None, views_pin=None, views=None, yuv_pin=None, yuv=None, ycbcr_pin=None,
@@ -1058,19 +1166,68 @@ class FEARMultiTracker:
         return name
 
     def _step(self, n: int, num_frames: int, dev: torch.device, table: str = "views",
-              agc: bool = False) -> torch.Tensor:
+              agc: bool = False, state: str = "state", zf: str = "zf") -> torch.Tensor:
+        """crop -> network -> advance on the first ``n`` rows of the FearTarget buffer ``state`` and the templates
+        ``zf`` (the targets' own rows, or the compact step rows of a subset step)."""
         b, cfg, lib = self._buf, self.tracking_config, _lib.load()
         _, crop_fn, advance_fn = ENTRY_POINTS[table]
         size = int(cfg["instance_size"])
         s = torch.cuda.current_stream(dev).cuda_stream
         if agc:  # the frames' code ranges, written into the table the crop reads
             _lib.check(getattr(lib, RANGE_ENTRY_POINT)(b[table].data_ptr(), num_frames, s), RANGE_ENTRY_POINT)
-        _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b["state"].data_ptr(), n,
+        _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b[state].data_ptr(), n,
                                          float(cfg["search_context"]), size, b["crops"].data_ptr(), s), crop_fn)
-        boxes = self.net.track_boxes(b["crops"][:n], b["zf"][:n])
-        _lib.check(getattr(lib, advance_fn)(boxes.data_ptr(), b[table].data_ptr(), num_frames, b["state"].data_ptr(),
+        boxes = self.net.track_boxes(b["crops"][:n], b[zf][:n])
+        _lib.check(getattr(lib, advance_fn)(boxes.data_ptr(), b[table].data_ptr(), num_frames, b[state].data_ptr(),
                                             n, size, s), advance_fn)
         return boxes
+
+    def _subset_step(self, m: int, num_frames: int, dev: torch.device, table: str, agc: bool) -> torch.Tensor:
+        """One step of the ``m`` targets named by the selection buffer: gather their rows and templates into the
+        compact step buffers, step those, and scatter the new boxes back.  Rows are bounded by ``max_targets`` (the
+        buffer's size), not by the target count, so adding or removing targets does not change the captured graph."""
+        b, lib, rows = self._buf, _lib.load(), self.max_targets
+        s = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(lib.fear_gather_targets(b["state"].data_ptr(), rows, b["zf"].data_ptr(), b["select"].data_ptr(), m,
+                                           b["step_state"].data_ptr(), b["step_zf"].data_ptr(), s),
+                   "fear_gather_targets")
+        boxes = self._step(m, num_frames, dev, table, agc, state="step_state", zf="step_zf")
+        _lib.check(lib.fear_scatter_targets(b["step_state"].data_ptr(), b["select"].data_ptr(), m,
+                                            b["state"].data_ptr(), rows, s), "fear_scatter_targets")
+        return boxes
+
+    def _run_subset_step(self, m: int, num_frames: int, table: str, dev: torch.device, agc: bool) -> torch.Tensor:
+        """One subset step, replayed from a cache of captured graphs kept apart from the list path's ``_graph``, so
+        neither path recaptures the other's graph.  The selection is read from its buffer when the kernels run, so a
+        graph is keyed by the step's shape only: the step row count, the frame count, the table and its buffer,
+        ``agc`` and the selection buffer.  A key is captured on its second call, as in ``_run_step``.  The cache holds
+        at most ``SUBSET_GRAPHS`` keys (captured or counting calls) and evicts the least recently used one; a change of
+        the net's generation drops every graph."""
+        gen = self.net.generation()
+        if gen != self._subset_gen:
+            self._subset_graphs.clear()
+            self._subset_gen = gen
+        key = (m, num_frames, table, self._buf[table].data_ptr(), agc, self._buf["select"].data_ptr())
+        entry = self._subset_graphs.pop(key, None) or {"calls": 0, "graph": None, "boxes": None}
+        self._subset_graphs[key] = entry  # most recently used last
+        while len(self._subset_graphs) > SUBSET_GRAPHS:
+            self._subset_graphs.popitem(last=False)
+        use_graph = self.tracking_config.get("cuda_graph", True) and self._graph_ok
+        if use_graph and entry["graph"] is None and entry["calls"] >= 1:
+            try:
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    entry["boxes"] = self._subset_step(m, num_frames, dev, table, agc)
+                entry["graph"] = g
+            except RuntimeError as exc:
+                warnings.warn(f"FEARMultiTracker: CUDA-graph capture of the step failed ({exc}); using eager launches")
+                self._graph_ok = False
+                torch.cuda.synchronize(dev)
+        entry["calls"] += 1
+        if use_graph and entry["graph"] is not None:
+            entry["graph"].replay()
+            return entry["boxes"]
+        return self._subset_step(m, num_frames, dev, table, agc)
 
     def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device, agc: bool = False) -> torch.Tensor:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The

@@ -54,6 +54,8 @@
  *   fear_crop_targets_rgb_u8 / fear_advance_targets_rgb / fear_frame_sums_rgb_u8   the same three on RGB frames in any
  *                         channel order located by FearFrameRGB (BGR / BGRA / ABGR, x2rgb10, rgb48 / rgba64, planar
  *                         gbrp at 8 to 16 bits), each tap's channels read and mapped to 8 bits inside the crop
+ *   fear_gather_targets / fear_scatter_targets   the selected targets' rows and templates into compact step buffers,
+ *                         and their new boxes back, for a step over the targets of some streams only
  *
  * Conventions: every pointer named d_* is a DEVICE pointer owned by the caller (torch keeps
  * ownership); tensors are dense fp32 in the reference's NCHW layout unless stated; `stream`
@@ -574,6 +576,26 @@ int fear_crop_targets_rgb_u8(const FearFrameRGB* d_views, int F, FearTarget* d_t
 int fear_advance_targets_rgb(const FearBox* d_boxes, const FearFrameRGB* d_views, int F, FearTarget* d_targets, int N,
                              int instance_size, void* stream);
 int fear_frame_sums_rgb_u8(const FearFrameRGB* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* A step over some of the targets (FEARMultiTracker fed the frames of some streams only):
+ *   fear_gather_targets -> crop (M) -> fear_track_u8 (B = M, Bz = M) -> advance (M) -> fear_scatter_targets
+ * d_select (M pairs of int32 in device memory, read when the kernels run, so a captured graph sees each step's
+ * selection): step row i is target row select[2 i], and select[2 i + 1] is the index of its frame in the step's frame
+ * table.  d_targets (N FearTarget) and d_templates (N, 256, 8, 8) fp32 are the targets' rows and templates; the step
+ * runs on the compact d_step_targets (M) and d_step_templates (M, 256, 8, 8) with the crop / advance entry points of
+ * any frame table above.  Both calls are handle-free, never allocate and never synchronise.
+ *
+ * fear_gather_targets: one launch for all M.  Step row i = target row select[2 i] with frame = select[2 i + 1]; its
+ * 64 KB template is copied with 16-byte loads and stores.  A row index outside [0, N) gives an inert step row: a zero
+ * FearTarget with frame = -1 (so the crop gives a padding-colour crop and the advance keeps the box) and a zero
+ * template.  FEAR_EINVAL: a null pointer, N < 1, M outside [1, 65535], a template buffer not 16-byte aligned. */
+int fear_gather_targets(const FearTarget* d_targets, int N, const float* d_templates, const int32_t* d_select, int M,
+                        FearTarget* d_step_targets, float* d_step_templates, void* stream);
+/* fear_scatter_targets: one launch.  x, y, w, h, cx, cy, cw, ch of step row i are written to target row select[2 i];
+ * frame, the padding colour and the reserved words are never written.  Rows outside [0, N) are skipped; the caller
+ * guarantees the rows in [0, N) are distinct.  FEAR_EINVAL: a null pointer, N < 1, M outside [1, 65535]. */
+int fear_scatter_targets(const FearTarget* d_step_targets, const int32_t* d_select, int M, FearTarget* d_targets, int N,
+                         void* stream);
 
 /* Decode maps produced elsewhere: bbox (B,4,16,16), cls logits (B,1,16,16) -> boxes[B].
  * apply_sigmoid = 0 treats cls as already-activated scores (decode(use_sigmoid=False)).
