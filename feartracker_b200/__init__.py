@@ -4,8 +4,8 @@ from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY  #
 from .fear_net import FEARNet  # noqa: F401
 from .box_coder import FEARBoxCoder, TrackerDecodeResult  # noqa: F401
 from .tracker import FEARTracker, Tracker, TrackingState  # noqa: F401
-from .multi_tracker import (BayerFrame, FEARMultiTracker, MonoFrame, RGBFrame, V210Frame, YUV420Frame,  # noqa: F401
-                            YUV422Frame, YUV444Frame)
+from .multi_tracker import (BayerFrame, FEARMultiTracker, MonoFrame, Oriented, RGBFrame, V210Frame,  # noqa: F401
+                            YUV420Frame, YUV422Frame, YUV444Frame)
 
 FEAR_XS_MODEL_KWARGS = dict(  # reference model_training/config/model/fear.yaml
     backbone="custom_fbnet", img_size=256, pretrained=True, stride=2, conv_block="sep_conv", towernum=2, mobile=True,

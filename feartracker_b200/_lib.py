@@ -64,6 +64,9 @@ RGB_DTYPE = np.dtype([("r", "<u8"), ("g", "<u8"), ("b", "<u8"), ("row_stride", "
                       ("H", "<i4"), ("W", "<i4"), ("container", "<i4"), ("bits", "<i4"), ("shift_r", "<i4"),
                       ("shift_g", "<i4"), ("shift_b", "<i4"), ("reserved", "<i4")])
 assert RGB_DTYPE.itemsize == 72
+# the `table` argument of fear_crop_targets_oriented_u8 / fear_advance_targets_oriented: FEAR_TABLE_* of the header,
+# keyed by the name FEARMultiTracker gives each table
+ORIENT_TABLES = {"views": 0, "yuv": 1, "ycbcr": 2, "ycbcr_v210": 3, "ycbcr_hdr": 4, "bayer": 5, "mono": 6, "rgb": 7}
 
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -115,6 +118,10 @@ _SIGNATURES = {
     "fear_crop_targets_rgb_u8": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_int, c_void_p, c_void_p]),
     "fear_advance_targets_rgb": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "fear_frame_sums_rgb_u8": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fear_crop_targets_oriented_u8": (c_int, [c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_double, c_int,
+                                              c_void_p, c_void_p]),
+    "fear_advance_targets_oriented": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int,
+                                              c_void_p]),
     "fear_gather_targets": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "fear_scatter_targets": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "fear_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

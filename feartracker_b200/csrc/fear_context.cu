@@ -1350,6 +1350,60 @@ extern "C" int fear_frame_sums_rgb_u8(const FearFrameRGB* d_views, int F, uint64
   return launch_frame_sums(d_views, RGBFrames{d_views}, F, d_sums, stream);
 }
 
+// Rotated and mirrored frames: the crop and advance kernels of any of the eight frame tables, reading through
+// Oriented (each display pixel mapped to its stored pixel before the table's conversion).  fn gets the table's frame
+// source wrapped in Oriented.
+template <class Fn>
+static int with_oriented_table(int table, const void* d_table, const int32_t* d_orient, Fn fn) {
+  switch (table) {
+    case FEAR_TABLE_VIEW:
+      return fn(Oriented<FrameViews>{{static_cast<const FearFrameView*>(d_table)}, d_orient});
+    case FEAR_TABLE_YUV:
+      return fn(Oriented<YUVFrames>{{static_cast<const FearFrameYUV*>(d_table)}, d_orient});
+    case FEAR_TABLE_YCBCR:
+      return fn(Oriented<YCbCrFrames>{{static_cast<const FearFrameYCbCr*>(d_table)}, d_orient});
+    case FEAR_TABLE_YCBCR_V210:
+      return fn(Oriented<YCbCrV210Frames>{{static_cast<const FearFrameYCbCrV210*>(d_table)}, d_orient});
+    case FEAR_TABLE_YCBCR_HDR:
+      return fn(Oriented<YCbCrHDRFrames>{{static_cast<const FearFrameYCbCrHDR*>(d_table)}, d_orient});
+    case FEAR_TABLE_BAYER:
+      return fn(Oriented<BayerFrames>{{static_cast<const FearFrameBayer*>(d_table)}, d_orient});
+    case FEAR_TABLE_MONO:
+      return fn(Oriented<MonoFrames>{{static_cast<const FearFrameMono*>(d_table)}, d_orient});
+    case FEAR_TABLE_RGB:
+      return fn(Oriented<RGBFrames>{{static_cast<const FearFrameRGB*>(d_table)}, d_orient});
+  }
+  return set_err(FEAR_EINVAL, "unknown frame table %d (FEAR_TABLE_VIEW .. FEAR_TABLE_RGB)", table);
+}
+
+static int check_table(int table) {
+  if (table < FEAR_TABLE_VIEW || table > FEAR_TABLE_RGB)
+    return set_err(FEAR_EINVAL, "unknown frame table %d (FEAR_TABLE_VIEW .. FEAR_TABLE_RGB)", table);
+  return 0;
+}
+
+extern "C" int fear_crop_targets_oriented_u8(int table, const void* d_table, const int32_t* d_orient, int F,
+                                             FearTarget* d_targets, int N, double offset, int out_size,
+                                             uint8_t* d_crops, void* stream) {
+  if (int r = check_table(table)) return r;
+  if (!d_table || !d_targets || !d_crops) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_crop_targets_args(F, N, offset, out_size)) return r;
+  return with_oriented_table(table, d_table, d_orient, [&](auto frames) {
+    return launch_crop_targets(frames, F, d_targets, N, offset, out_size, d_crops, stream);
+  });
+}
+
+extern "C" int fear_advance_targets_oriented(const FearBox* d_boxes, int table, const void* d_table,
+                                             const int32_t* d_orient, int F, FearTarget* d_targets, int N,
+                                             int instance_size, void* stream) {
+  if (int r = check_table(table)) return r;
+  if (!d_boxes || !d_table || !d_targets) return set_err(FEAR_EINVAL, "null pointer argument");
+  if (int r = check_advance_targets_args(F, N, instance_size)) return r;
+  return with_oriented_table(table, d_table, d_orient, [&](auto frames) {
+    return launch_advance_targets(d_boxes, frames, F, d_targets, N, instance_size, stream);
+  });
+}
+
 // A step over some targets only: their rows and templates gathered into compact step buffers, stepped there by the
 // entry points above, and their boxes scattered back.
 static int check_select_args(int N, int M) {

@@ -23,7 +23,9 @@
 // table of FearFrameMono records (MonoFrames), read through MonoFrame, which maps single-channel codes to grey; or a
 // table of FearFrameRGB records (RGBFrames), read through RGBFrame, which fetches each channel from its own address in
 // an 8-, 16- or 32-bit container (any channel order, packed or planar) and maps it to 8 bits.  A frame type gives H, W, empty() and the RGB triple of one pixel, rgb(y, x, p); the context box, resize tables,
-// interpolation, sums and the colour conversion exist once.
+// interpolation, sums and the colour conversion exist once.  Oriented wraps any of those sources for the crop and
+// advance kernels: its OrientedFrame is the stored frame turned by a per-frame code (90-degree turns after an optional
+// left-right flip), each display pixel mapped to its stored pixel before the stored frame's rgb().
 //
 // The crop and advance kernels reproduce the host's float64 / float32 arithmetic bit for bit.  nvcc contracts a*b+c
 // into an FMA by default, which rounds once instead of twice, so every multiply-add here is spelled with the explicitly
@@ -648,6 +650,42 @@ struct RGBFrames {
     ok = ok && v.g != nullptr && v.b != nullptr && v.row_stride >= 0 && v.pixel_stride >= 0;
     return RGBFrame{v.r, v.g, v.b, v.row_stride, v.pixel_stride, v.H, v.W, v.container, bits, sr, sg, sb, !ok,
                     ok && bits != 8 ? __ddiv_rn(1.0, (double)((1 << bits) - 1)) : 0.0};
+  }
+};
+
+// A frame as it is shown: the stored frame f turned by orientation code `code` (include/fear_b200.h,
+// fear_crop_targets_oriented_u8): 90 * (code & 3) degrees clockwise, after a left-right flip when code & 4.  H, W are
+// the display sizes (f's swapped for odd codes) and rgb(y, x) is f.rgb at the stored pixel of display pixel (y, x):
+//   code & 3:   0 (y, x)   1 (Hs - 1 - x, y)   2 (Hs - 1 - y, Ws - 1 - x)   3 (x, Ws - 1 - y)
+// then xs = Ws - 1 - xs when mirrored.  Every conversion behind f.rgb is a function of the stored pixel and its stored
+// neighbours, so orienting the coordinates equals orienting the converted frame, bit for bit.  A code outside [0, 7]
+// is empty, as is an empty f; a value-initialised OrientedFrame{} is empty.
+template <class Frame>
+struct OrientedFrame {
+  Frame f;
+  int code;
+  int H, W;
+  __device__ __forceinline__ bool empty() const { return code < 0 || code > 7 || f.empty(); }
+  __device__ __forceinline__ void rgb(int y, int x, int p[3]) const {
+    const int r = code & 3;
+    int ys = r == 0 ? y : r == 1 ? f.H - 1 - x : r == 2 ? f.H - 1 - y : x;
+    int xs = r == 0 ? x : r == 1 ? y : r == 2 ? f.W - 1 - x : f.W - 1 - y;
+    if (code & 4) xs = f.W - 1 - xs;
+    f.rgb(ys, xs, p);
+  }
+};
+
+// Frame i of any frame source above, turned by code codes[i] (int32 in device memory, read when the kernel runs; a
+// null codes gives code 0 everywhere).
+template <class Frames>
+struct Oriented {
+  Frames frames;
+  const int32_t* codes;
+  __device__ __forceinline__ OrientedFrame<decltype(Frames{}(0))> operator()(int i) const {
+    const auto f = frames(i);
+    const int code = codes != nullptr ? __ldg(codes + i) : 0;
+    const bool turned = code & 1;
+    return {f, code, turned ? f.W : f.H, turned ? f.H : f.W};
   }
 };
 

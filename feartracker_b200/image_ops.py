@@ -718,3 +718,25 @@ def rgb_frame_to_rgb(data, layout: str, bits: Optional[int] = None) -> np.ndarra
             codes = codes & np.uint16((1 << bits) - 1)
         return raw_to_u8(codes, bits)
     raise ValueError(f"unknown RGB layout {layout!r}")
+
+
+ORIENT_ROTATIONS = (0, 90, 180, 270)  # the clockwise turns of an orientation code, code & 3 = rotate / 90
+
+
+def orient_code(rotate: int = 0, mirror: bool = False) -> int:
+    """The orientation code of a clockwise turn by ``rotate`` degrees (0, 90, 180 or 270) after a left-right flip when
+    ``mirror``: rotate / 90, plus 4 when mirrored.  ffmpeg's autorotate turns a display-matrix rotation of r degrees
+    (ffprobe's ``rotation=-90``) by rotate = (-r) mod 360 (here 90)."""
+    if isinstance(rotate, (bool, np.bool_)) or not isinstance(rotate, (int, np.integer)) \
+            or int(rotate) not in ORIENT_ROTATIONS:
+        raise ValueError(f"rotate must be 0, 90, 180 or 270 (degrees clockwise), got {rotate!r}")
+    return int(rotate) // 90 + (4 if mirror else 0)
+
+
+def orient(rgb: np.ndarray, code: int) -> np.ndarray:
+    """The frame a tracker sees for orientation ``code`` in [0, 7]: ``rgb`` (H, W, ...) turned 90 * (code & 3) degrees
+    clockwise, after a left-right flip when code & 4.  Display pixel (y, x) is stored pixel (ys, xs):
+        code & 3 = 0: (y, x);  1: (H - 1 - x, y);  2: (H - 1 - y, W - 1 - x);  3: (x, W - 1 - y)
+    then xs = W - 1 - xs when mirrored; the display is W x H for odd codes.  A view, no copy: for host frames this is
+    the whole of orientation (pass ``np.ascontiguousarray`` of it, or the view, to a tracker)."""
+    return np.rot90(rgb[:, ::-1] if code & 4 else rgb, -(code & 3))

@@ -23,7 +23,10 @@ RAW10 / RAW12), mapped to grey inside the crop, optionally with per-frame min-ma
 NORM_MINMAX); or RGB frames in any channel order and container: RGBFrame (OpenCV's BGR and BGRA, RGBA / ARGB / ABGR
 and their X variants, 10-bit x2rgb10 / x2bgr10 words, 16-bit rgb48 / rgba64, planar gbrp at 8 to 16 bits), each tap's
 channels fetched and mapped to 8 bits inside the crop.  Tensors, YUV planes, v210 surfaces, Bayer mosaics, mono frames
-and RGB frames are read where they are, without a copy.
+and RGB frames are read where they are, without a copy.  Any of them may be wrapped in Oriented(frame, rotate, mirror)
+to track on the picture as it is shown (phone video's display rotation, cameras mounted upside down or mirrored):
+rects and boxes are then in the turned picture's coordinates, and each display pixel is mapped to its stored pixel
+inside the crop.
 
 Every target behaves exactly like its own ``FEARTracker(gpu_crop=True)`` started on the same frame with the same
 rect: the rect is clamped, the padding colour is the mean colour of the init frame, the template is the network
@@ -49,7 +52,10 @@ gain control, fear_frame_range_mono first writes each frame's code range into th
 puts all its frames, RGBFrames and CUDA tensors alike, into an eighth, of FearFrameRGB records, read by the *_rgb entry
 points; RGBFrames cannot share a call with numpy arrays or YUV, Bayer or mono frames.  The host then reads back
 the boxes and scores.  The launch count of a step depends neither on N nor on the kind of frames, with one exception:
-a step on MonoFrames with gain control launches the range kernel too (49 launches instead of 48).
+a step on MonoFrames with gain control launches the range kernel too (49 launches instead of 48).  When any frame of a
+call is Oriented, the call's F int32 orientation codes follow the records in the same table buffer and copy, and the
+step runs fear_crop_targets_oriented_u8 / fear_advance_targets_oriented on the same table in place of its crop and
+advance (the sums and the range kernel are unchanged: neither depends on orientation); the launch count is the same.
 
 A step over the M targets of a mapping's streams runs on compact buffers of max_targets rows:
 
@@ -96,6 +102,9 @@ TABLE_DTYPES = {"views": _lib.VIEW_DTYPE, "yuv": _lib.YUV_DTYPE, "ycbcr": _lib.Y
                 "mono": _lib.MONO_DTYPE, "rgb": _lib.RGB_DTYPE}
 # the entry point that writes each frame's code range into a FearFrameMono table, for min-max gain control
 RANGE_ENTRY_POINT = "fear_frame_range_mono"
+# the crop and advance of any table on rotated and mirrored frames (Oriented), with the table named by
+# _lib.ORIENT_TABLES and the call's orientation codes; the sums and the range do not depend on orientation
+ORIENTED_ENTRY_POINTS = ("fear_crop_targets_oriented_u8", "fear_advance_targets_oriented")
 
 
 def frame_view(frame: torch.Tensor) -> tuple:
@@ -694,11 +703,67 @@ def tensor_rgb_record(t: torch.Tensor) -> tuple:
     return (p, p + cs, p + 2 * cs, rs, ps, h, w, 1, 8, 0, 0, 0, 0)
 
 
+_DEVICE_FRAMES = (_YUVFrame, V210Frame, _RawFrame, RGBFrame)
+
+
+class Oriented:
+    """A device frame as it is shown rather than as it is stored: ``frame`` turned ``rotate`` degrees clockwise (0, 90,
+    180 or 270), after a left-right flip when ``mirror``.  For phone video (a portrait recording is coded in landscape
+    and carries a display-matrix rotation) and for cameras mounted upside down or mirrored (ceiling CCTV, a rear
+    camera, a mirrored selfie camera).  ffmpeg's autorotate convention: rotate = (-display-matrix rotation) mod 360,
+    so ffprobe's ``rotation=-90`` is ``rotate=90``; nothing is read from containers.
+
+        Oriented(frame, rotate=0, mirror=False)   frame: a CUDA uint8 (H, W, 3) tensor, YUV420Frame, YUV422Frame,
+                                                  YUV444Frame, V210Frame, BayerFrame, MonoFrame or RGBFrame
+
+    FEARMultiTracker and FEARTracker read the stored frame where it is and map each display pixel to its stored pixel
+    inside the crop, so no turned copy is made: the frame the tracker sees is ``image_ops.orient(rgb, code)`` of the
+    frame it sees for ``frame`` (``image_ops.yuv_to_rgb``, ``bayer_to_rgb``, ``mono_to_rgb``, ``rgb_frame_to_rgb`` or
+    the tensor), and rects and boxes are in that frame's coordinates.  ``code`` is rotate / 90 + 4 * mirror
+    (``image_ops.orient_code``); ``shape`` is the display shape, (W, H, 3) for 90 and 270 degrees.  The frame's kind
+    (``frame_kind``) is the wrapped frame's, so the rules on mixing kinds in one call are unchanged, and oriented and
+    plain frames, with different codes, may share a call.  The constructor raises ValueError on a bad rotation, a numpy
+    array (turn host frames with ``image_ops.orient``: ``np.rot90`` is a free view there), a nested Oriented or
+    anything that is not a device frame; the frame itself is checked by the tracker, as a plain one is."""
+
+    def __init__(self, frame, rotate: int = 0, mirror: bool = False) -> None:
+        code = image_ops.orient_code(rotate, mirror)
+        if isinstance(frame, np.ndarray):
+            raise ValueError("Oriented wraps device frames; turn a numpy frame with image_ops.orient(frame, code) "
+                             "(np.rot90 and a flip are free views of a host frame) and pass the result")
+        if isinstance(frame, Oriented):
+            raise ValueError("Oriented frames cannot be nested: combine the turns into one rotate and mirror")
+        if not isinstance(frame, _DEVICE_FRAMES + (torch.Tensor,)):
+            raise ValueError(f"Oriented wraps a CUDA uint8 tensor, YUV420Frame, YUV422Frame, YUV444Frame, V210Frame, "
+                             f"BayerFrame, MonoFrame or RGBFrame, got {type(frame).__name__}")
+        self.frame, self.code = frame, code
+        shape = tuple(frame.shape)
+        self.shape = (shape[1], shape[0], *shape[2:]) if code & 1 and len(shape) >= 2 else shape
+
+    def __repr__(self) -> str:
+        return f"Oriented({type(self.frame).__name__}, code={self.code})"
+
+
+def stored(frame):
+    """The frame as it is stored: the wrapped frame of an ``Oriented``, any other frame itself."""
+    return frame.frame if isinstance(frame, Oriented) else frame
+
+
+def orient_codes(frames) -> Optional[np.ndarray]:
+    """The (F,) int32 orientation codes of a call's frames (0 for a plain frame), or None when none is ``Oriented``: a
+    call without Oriented frames launches the plain entry points."""
+    if not any(isinstance(f, Oriented) for f in frames):
+        return None
+    return np.array([f.code if isinstance(f, Oriented) else 0 for f in frames], dtype=np.int32)
+
+
 def frame_kind(frame) -> str:
     """"yuv" for a YUV420Frame, YUV422Frame, YUV444Frame or V210Frame, "bayer" for a BayerFrame, "mono" for a
     MonoFrame, "rgb" for an RGBFrame (any channel order and container: BGR, BGRA / ABGR, x2rgb10, rgb48 / rgba64, planar
     RGB; the kernels read its channels where they are), "cuda" for a torch tensor (checked by ``check_device_frame``),
-    "numpy" for anything else.  Host frames are always H x W x 3 RGB."""
+    "numpy" for anything else.  Host frames are always H x W x 3 RGB.  An ``Oriented`` frame has its wrapped frame's
+    kind."""
+    frame = stored(frame)
     if isinstance(frame, RGBFrame):
         return "rgb"
     if isinstance(frame, (_YUVFrame, V210Frame)):
@@ -741,12 +806,13 @@ def check_tensor_frame(i: int, f: torch.Tensor, device) -> None:
 def uses_agc(frames, kind: str) -> bool:
     """Whether any of a call's frames of kind ``kind`` is a MonoFrame with gain control: its table needs
     fear_frame_range_mono before the sums or the crop read it."""
-    return kind == "mono" and any(f.agc is not None for f in frames)
+    return kind == "mono" and any(stored(f).agc is not None for f in frames)
 
 
 def check_device_frame(i: int, f, kind: str, device) -> None:
     """The checks of a frame of kind "cuda", "yuv", "bayer", "mono" or "rgb" (``frame_kind``): ValueError before any
-    device call."""
+    device call.  An ``Oriented`` frame is checked as its wrapped frame."""
+    f = stored(f)
     if kind == "rgb":
         check_device(i, device, *f.tensors)
     elif kind in ("bayer", "mono"):
@@ -761,8 +827,10 @@ def write_records(table: np.ndarray, frames, name: str) -> None:
     """Write the records of device frames into rows of ``table`` (a numpy view of ``TABLE_DTYPES[name]``):
     FearFrameView records of CUDA tensors for "views", FearFrameYUV records for "yuv", FearFrameYCbCr for "ycbcr",
     FearFrameYCbCrV210 for "ycbcr_v210", FearFrameYCbCrHDR for "ycbcr_hdr", FearFrameBayer for "bayer", FearFrameMono
-    for "mono", FearFrameRGB for "rgb" (of RGBFrames and of CUDA tensors, ``tensor_rgb_record``)."""
+    for "mono", FearFrameRGB for "rgb" (of RGBFrames and of CUDA tensors, ``tensor_rgb_record``).  An ``Oriented``
+    frame's record is its stored frame's: its code goes into a table of its own."""
     for i, f in enumerate(frames):
+        f = stored(f)
         if name == "rgb":
             table[i] = f.rgb_record() if isinstance(f, RGBFrame) else tensor_rgb_record(f)
         elif name == "yuv":
@@ -881,7 +949,7 @@ class FEARMultiTracker:
             b = self._buffers(dev)
             num_frames = len(frames)
             table = self._upload_frames(frames, kind, dev)
-            sums_fn, crop_fn, _ = ENTRY_POINTS[table]
+            sums_fn = ENTRY_POINTS[table][0]
             lib = _lib.load()
             stream = torch.cuda.current_stream(dev)
             if uses_agc(frames, kind):
@@ -901,9 +969,8 @@ class FEARMultiTracker:
             b["state"][n0:n0 + n].copy_(torch.from_numpy(recs).pin_memory(), non_blocking=True)
             size = int(cfg["template_size"])
             crops = b["tcrops"][:n]
-            _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b["state"][n0].data_ptr(), n,
-                                             float(cfg["template_bbox_offset"]), size, crops.data_ptr(),
-                                             stream.cuda_stream), crop_fn)
+            self._crop(table, num_frames, orient_codes(frames) is not None, b["state"][n0].data_ptr(), n,
+                       float(cfg["template_bbox_offset"]), size, crops.data_ptr(), stream.cuda_stream)
             b["zf"][n0:n0 + n].copy_(self.net.get_features(crops))
             if keys is not None:  # the rows keep their stream ids, not this call's frame indices
                 b["state"][n0:n0 + n, 0].copy_(torch.from_numpy(streams.astype(np.int32)).pin_memory(),
@@ -957,7 +1024,10 @@ class FEARMultiTracker:
         also be all ``MonoFrame``s (any depths, packings and gain controls), never mixed with other kinds; they give
         exactly what ``image_ops.mono_to_rgb`` of their codes gives as numpy arrays.  ``frames`` may also be
         ``RGBFrame``s (any layouts and depths) mixed freely with CUDA tensors, never with other kinds; they give exactly
-        what ``image_ops.rgb_frame_to_rgb`` of their samples gives as numpy arrays.  Device frames must
+        what ``image_ops.rgb_frame_to_rgb`` of their samples gives as numpy arrays.  Any device frame may be an
+        ``Oriented`` one, with its own code, alongside plain frames of kinds its frame may share a call with; it gives
+        exactly what ``image_ops.orient`` of the frame it wraps gives as a numpy array, with boxes in the turned
+        picture's coordinates.  Device frames must
         be ready on the current CUDA stream (write them on that stream, or make it wait for the stream that did, as for
         any torch op).  ``update`` synchronises that stream before it returns, so they only need to live until the
         call returns."""
@@ -974,7 +1044,8 @@ class FEARMultiTracker:
         with torch.cuda.device(dev):
             b = self._buffers(dev)
             table = self._upload_frames(frames, kind, dev)
-            boxes = self._run_step(n, len(frames), table, dev, uses_agc(frames, kind))
+            boxes = self._run_step(n, len(frames), table, dev, uses_agc(frames, kind),
+                                   orient_codes(frames) is not None)
             b["state_pin"][:n].copy_(b["state"][:n], non_blocking=True)
             b["box_pin"][:n].copy_(boxes, non_blocking=True)
             torch.cuda.current_stream(dev).synchronize()
@@ -999,7 +1070,8 @@ class FEARMultiTracker:
             sel[:m, 0] = rows
             sel[:m, 1] = _positions(keys, self._streams[rows])
             b["select"][:m].copy_(b["select_pin"][:m], non_blocking=True)
-            boxes = self._run_subset_step(m, len(frames), table, dev, uses_agc(frames, kind))
+            boxes = self._run_subset_step(m, len(frames), table, dev, uses_agc(frames, kind),
+                                          orient_codes(frames) is not None)
             b["state_pin"][:m].copy_(b["step_state"][:m], non_blocking=True)
             b["box_pin"][:m].copy_(boxes, non_blocking=True)
             torch.cuda.current_stream(dev).synchronize()
@@ -1044,8 +1116,8 @@ class FEARMultiTracker:
     def _check_frames(self, frames):
         """-> (list of frames, their kind: "numpy", "cuda", "yuv", "bayer", "mono" or "rgb", the last for RGBFrames
         with or without CUDA tensors).  Raises ValueError before any device call."""
-        if isinstance(frames, (_YUVFrame, V210Frame, _RawFrame, RGBFrame)) or (isinstance(frames, (np.ndarray, torch.Tensor))
-                                                          and frames.ndim == 3):
+        if isinstance(frames, _DEVICE_FRAMES + (Oriented,)) or (isinstance(frames, (np.ndarray, torch.Tensor))
+                                                                and frames.ndim == 3):
             frames = [frames]
         frames = list(frames)
         if not frames:
@@ -1120,22 +1192,27 @@ class FEARMultiTracker:
         MonoFrames, "rgb" (FearFrameRGB records) for a call with any RGBFrame, "views" (FearFrameView records)
         otherwise.  Numpy frames are packed into the pinned staging buffer
         first and sent with one host-to-device copy (the packed layout is recomputed only when their shapes change);
-        CUDA tensors, YUV planes, v210 surfaces, Bayer mosaics, mono frames and RGB frames are used where they are."""
+        CUDA tensors, YUV planes, v210 surfaces, Bayer mosaics, mono frames and RGB frames are used where they are.
+        When any frame is ``Oriented``, the F int32 orientation codes follow the F records in the same buffer and the
+        same copy (``_orient_ptr``); otherwise the copy is the records alone, as it always was."""
         b, num_frames = self._buf, len(frames)
+        plain = [stored(f) for f in frames]
         name = "views"
         if kind == "yuv":
-            name = "yuv" if all(isinstance(f, YUV420Frame) for f in frames) else "ycbcr"
-            if any(isinstance(f, V210Frame) for f in frames):
+            name = "yuv" if all(isinstance(f, YUV420Frame) for f in plain) else "ycbcr"
+            if any(isinstance(f, V210Frame) for f in plain):
                 name = "ycbcr_v210"
-            if any(f.transfer is not None for f in frames):
+            if any(f.transfer is not None for f in plain):
                 name = "ycbcr_hdr"
         elif kind in ("bayer", "mono", "rgb"):
             name = kind
         dtype = TABLE_DTYPES[name]
         nbytes = num_frames * dtype.itemsize
-        if b[name] is None or b[name].numel() < nbytes:  # grows only: the step graph keys on it
-            b[name + "_pin"] = torch.empty(nbytes, dtype=torch.uint8).pin_memory()
-            b[name] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        codes = orient_codes(frames)
+        room = nbytes + 4 * num_frames  # every table's record size is a multiple of 8: the codes stay aligned
+        if b[name] is None or b[name].numel() < room:  # grows only: the step graph keys on it
+            b[name + "_pin"] = torch.empty(room, dtype=torch.uint8).pin_memory()
+            b[name] = torch.empty(room, dtype=torch.uint8, device=dev)
         if b["sums"] is None or b["sums"].shape[0] < num_frames:
             # the frame sums entry points write uint64; int64 storage, read back as uint64
             b["sums_pin"] = torch.empty((num_frames, 3), dtype=torch.int64).pin_memory()
@@ -1162,27 +1239,55 @@ class FEARMultiTracker:
                 table[i] = (base + o, 3 * w, 3, 1, h, w)
             nb = b["nbytes"]
             b["frames"][:nb].copy_(b["frames_pin"][:nb], non_blocking=True)
+        if codes is not None:
+            b[name + "_pin"].numpy()[nbytes:nbytes + 4 * num_frames].view(np.int32)[:] = codes
+            nbytes += 4 * num_frames
         b[name][:nbytes].copy_(b[name + "_pin"][:nbytes], non_blocking=True)
         return name
 
+    def _orient_ptr(self, table: str, num_frames: int) -> int:
+        """The device address of the orientation codes ``_upload_frames`` writes after the F records of ``table``."""
+        return self._buf[table].data_ptr() + num_frames * TABLE_DTYPES[table].itemsize
+
+    def _crop(self, table: str, num_frames: int, oriented: bool, state_ptr: int, n: int, offset: float, size: int,
+              crops_ptr: int, s) -> None:
+        """The crop entry point of ``table`` on ``n`` FearTarget rows, or with ``oriented`` the oriented one reading
+        the call's codes."""
+        lib, t = _lib.load(), self._buf[table].data_ptr()
+        if oriented:
+            fn = ORIENTED_ENTRY_POINTS[0]
+            _lib.check(getattr(lib, fn)(_lib.ORIENT_TABLES[table], t, self._orient_ptr(table, num_frames), num_frames,
+                                        state_ptr, n, offset, size, crops_ptr, s), fn)
+        else:
+            fn = ENTRY_POINTS[table][1]
+            _lib.check(getattr(lib, fn)(t, num_frames, state_ptr, n, offset, size, crops_ptr, s), fn)
+
     def _step(self, n: int, num_frames: int, dev: torch.device, table: str = "views",
-              agc: bool = False, state: str = "state", zf: str = "zf") -> torch.Tensor:
+              agc: bool = False, state: str = "state", zf: str = "zf", oriented: bool = False) -> torch.Tensor:
         """crop -> network -> advance on the first ``n`` rows of the FearTarget buffer ``state`` and the templates
-        ``zf`` (the targets' own rows, or the compact step rows of a subset step)."""
+        ``zf`` (the targets' own rows, or the compact step rows of a subset step); with ``oriented`` the oriented crop
+        and advance, the same number of launches."""
         b, cfg, lib = self._buf, self.tracking_config, _lib.load()
-        _, crop_fn, advance_fn = ENTRY_POINTS[table]
         size = int(cfg["instance_size"])
         s = torch.cuda.current_stream(dev).cuda_stream
         if agc:  # the frames' code ranges, written into the table the crop reads
             _lib.check(getattr(lib, RANGE_ENTRY_POINT)(b[table].data_ptr(), num_frames, s), RANGE_ENTRY_POINT)
-        _lib.check(getattr(lib, crop_fn)(b[table].data_ptr(), num_frames, b[state].data_ptr(), n,
-                                         float(cfg["search_context"]), size, b["crops"].data_ptr(), s), crop_fn)
+        self._crop(table, num_frames, oriented, b[state].data_ptr(), n, float(cfg["search_context"]), size,
+                   b["crops"].data_ptr(), s)
         boxes = self.net.track_boxes(b["crops"][:n], b[zf][:n])
-        _lib.check(getattr(lib, advance_fn)(boxes.data_ptr(), b[table].data_ptr(), num_frames, b[state].data_ptr(),
-                                            n, size, s), advance_fn)
+        if oriented:
+            fn = ORIENTED_ENTRY_POINTS[1]
+            _lib.check(getattr(lib, fn)(boxes.data_ptr(), _lib.ORIENT_TABLES[table], b[table].data_ptr(),
+                                        self._orient_ptr(table, num_frames), num_frames, b[state].data_ptr(), n, size,
+                                        s), fn)
+        else:
+            advance_fn = ENTRY_POINTS[table][2]
+            _lib.check(getattr(lib, advance_fn)(boxes.data_ptr(), b[table].data_ptr(), num_frames,
+                                                b[state].data_ptr(), n, size, s), advance_fn)
         return boxes
 
-    def _subset_step(self, m: int, num_frames: int, dev: torch.device, table: str, agc: bool) -> torch.Tensor:
+    def _subset_step(self, m: int, num_frames: int, dev: torch.device, table: str, agc: bool,
+                     oriented: bool = False) -> torch.Tensor:
         """One step of the ``m`` targets named by the selection buffer: gather their rows and templates into the
         compact step buffers, step those, and scatter the new boxes back.  Rows are bounded by ``max_targets`` (the
         buffer's size), not by the target count, so adding or removing targets does not change the captured graph."""
@@ -1191,23 +1296,24 @@ class FEARMultiTracker:
         _lib.check(lib.fear_gather_targets(b["state"].data_ptr(), rows, b["zf"].data_ptr(), b["select"].data_ptr(), m,
                                            b["step_state"].data_ptr(), b["step_zf"].data_ptr(), s),
                    "fear_gather_targets")
-        boxes = self._step(m, num_frames, dev, table, agc, state="step_state", zf="step_zf")
+        boxes = self._step(m, num_frames, dev, table, agc, state="step_state", zf="step_zf", oriented=oriented)
         _lib.check(lib.fear_scatter_targets(b["step_state"].data_ptr(), b["select"].data_ptr(), m,
                                             b["state"].data_ptr(), rows, s), "fear_scatter_targets")
         return boxes
 
-    def _run_subset_step(self, m: int, num_frames: int, table: str, dev: torch.device, agc: bool) -> torch.Tensor:
+    def _run_subset_step(self, m: int, num_frames: int, table: str, dev: torch.device, agc: bool,
+                         oriented: bool = False) -> torch.Tensor:
         """One subset step, replayed from a cache of captured graphs kept apart from the list path's ``_graph``, so
         neither path recaptures the other's graph.  The selection is read from its buffer when the kernels run, so a
         graph is keyed by the step's shape only: the step row count, the frame count, the table and its buffer,
-        ``agc`` and the selection buffer.  A key is captured on its second call, as in ``_run_step``.  The cache holds
+        ``agc``, the selection buffer and whether the step is ``oriented`` (not the codes, read when it runs).  A key is captured on its second call, as in ``_run_step``.  The cache holds
         at most ``SUBSET_GRAPHS`` keys (captured or counting calls) and evicts the least recently used one; a change of
         the net's generation drops every graph."""
         gen = self.net.generation()
         if gen != self._subset_gen:
             self._subset_graphs.clear()
             self._subset_gen = gen
-        key = (m, num_frames, table, self._buf[table].data_ptr(), agc, self._buf["select"].data_ptr())
+        key = (m, num_frames, table, self._buf[table].data_ptr(), agc, self._buf["select"].data_ptr(), oriented)
         entry = self._subset_graphs.pop(key, None) or {"calls": 0, "graph": None, "boxes": None}
         self._subset_graphs[key] = entry  # most recently used last
         while len(self._subset_graphs) > SUBSET_GRAPHS:
@@ -1217,7 +1323,7 @@ class FEARMultiTracker:
             try:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    entry["boxes"] = self._subset_step(m, num_frames, dev, table, agc)
+                    entry["boxes"] = self._subset_step(m, num_frames, dev, table, agc, oriented)
                 entry["graph"] = g
             except RuntimeError as exc:
                 warnings.warn(f"FEARMultiTracker: CUDA-graph capture of the step failed ({exc}); using eager launches")
@@ -1227,16 +1333,19 @@ class FEARMultiTracker:
         if use_graph and entry["graph"] is not None:
             entry["graph"].replay()
             return entry["boxes"]
-        return self._subset_step(m, num_frames, dev, table, agc)
+        return self._subset_step(m, num_frames, dev, table, agc, oriented)
 
-    def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device, agc: bool = False) -> torch.Tensor:
+    def _run_step(self, n: int, num_frames: int, table: str, dev: torch.device, agc: bool = False,
+                  oriented: bool = False) -> torch.Tensor:
         """One step, as a CUDA graph after one eager warm-up call (the pattern of FEARTracker's gpu_crop path).  The
         kernels read the frame table when they run, so frame addresses and shapes are not baked into the graph: it is
         keyed by the target count, the frame count, which table the step reads (RGB views, YUV 4:2:0 records, YCbCr
         records of any subsampling, YCbCr / v210 records, HDR records, Bayer records, mono records or RGB records) and
-        its buffer, whether the step starts with the mono range kernel (``agc``), and the net's generation.
+        its buffer, whether the step starts with the mono range kernel (``agc``), whether it runs the oriented crop
+        and advance (``oriented``; the codes are read when the kernels run, so new codes replay the graph), and the
+        net's generation.
         ``cuda_graph=False`` in the tracking config keeps eager launches."""
-        key = (n, num_frames, table, self._buf[table].data_ptr(), agc)
+        key = (n, num_frames, table, self._buf[table].data_ptr(), agc, oriented)
         if key != self._graph_key or (self._graph is not None and self._graph_gen != self.net.generation()):
             # new target or frame count, another table or a new table buffer, or the net's workspace / weights /
             # options changed: the pointers and sizes baked into the captured graph are stale -> warm up eagerly and
@@ -1247,7 +1356,7 @@ class FEARMultiTracker:
             try:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    self._graph_boxes = self._step(n, num_frames, dev, table, agc)
+                    self._graph_boxes = self._step(n, num_frames, dev, table, agc, oriented=oriented)
                 self._graph, self._graph_gen = g, self.net.generation()
             except RuntimeError as exc:
                 warnings.warn(f"FEARMultiTracker: CUDA-graph capture of the step failed ({exc}); using eager launches")
@@ -1257,4 +1366,4 @@ class FEARMultiTracker:
         if use_graph and self._graph is not None:
             self._graph.replay()
             return self._graph_boxes
-        return self._step(n, num_frames, dev, table, agc)
+        return self._step(n, num_frames, dev, table, agc, oriented=oriented)

@@ -13,7 +13,9 @@ single-channel frames and RGBFrame BGR / BGRA / ABGR, 10-bit, 16-bit and planar 
 the crop, the conversion to RGB (or the demosaic), the network and the decode (plain or smoothed) run on the device, and
 the tracker returns exactly what it returns for the same pixels as a numpy array (``image_ops.yuv_to_rgb`` of a YUV
 frame's planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes, ``image_ops.mono_to_rgb`` of a mono frame's,
-``image_ops.rgb_frame_to_rgb`` of an RGB frame's samples).
+``image_ops.rgb_frame_to_rgb`` of an RGB frame's samples).  Any of them may be wrapped in ``Oriented(frame, rotate,
+mirror)`` (phone video's display rotation, a camera mounted upside down or mirrored): the tracker then sees
+``image_ops.orient`` of that frame, oriented inside the crop.
 """
 from collections import deque
 from typing import Any, Dict, Optional, Tuple, Union
@@ -28,8 +30,10 @@ from .constants import TARGET_CLASSIFICATION_KEY, TARGET_REGRESSION_LABEL_KEY
 
 
 # byte layout of FEARTracker's device-frame inputs: the frame's table record (up to a FearFrameYCbCrHDR; a
-# FearFrameBayer is 40 bytes, a FearFrameMono 48, a FearFrameRGB 72), a FearTarget, then five float64 inputs of fear_decode_smooth
-_TARGET_OFFSET = 104
+# FearFrameBayer is 40 bytes, a FearFrameMono 48, a FearFrameRGB 72), the int32 orientation code of an Oriented frame
+# (8 bytes kept), a FearTarget, then five float64 inputs of fear_decode_smooth, which the window follows on the device
+_ORIENT_OFFSET = 104
+_TARGET_OFFSET = _ORIENT_OFFSET + 8
 _SMOOTH_OFFSET = _TARGET_OFFSET + 64
 _DEVICE_INPUT_BYTES = _SMOOTH_OFFSET + 5 * 8
 
@@ -126,8 +130,10 @@ class FEARTracker(Tracker):
     The results, ``tracking_state`` included, are those of the same tracker fed the same pixels as numpy arrays
     (``image_ops.yuv_to_rgb`` of a YUV frame's planes with its ``CHROMA_SHIFT``, of a v210 frame's
     ``image_ops.v210_unpack`` planes, ``image_ops.bayer_to_rgb`` of a Bayer frame's codes, ``image_ops.mono_to_rgb``
-    of a mono frame's codes with its ``agc``, ``image_ops.rgb_frame_to_rgb`` of an RGB frame's samples).  Device
-    frames must be ready on the current CUDA stream; every call
+    of a mono frame's codes with its ``agc``, ``image_ops.rgb_frame_to_rgb`` of an RGB frame's samples).  An
+    ``Oriented`` device frame takes the table's oriented crop (fear_crop_targets_oriented_u8) with its code staged in
+    the same input copy, and gives what ``image_ops.orient`` of the frame it wraps gives as a numpy array; rects and
+    boxes are in the turned picture's coordinates.  Device frames must be ready on the current CUDA stream; every call
     synchronises it before it returns, so they only need to live for the call.
     ``host_normalize: true`` takes numpy frames only."""
 
@@ -300,8 +306,9 @@ class FEARTracker(Tracker):
         """Buffers of the device-frame step, separate from the gpu_crop path's.  ``inputs`` (pinned) and ``dev_in``
         share one layout, sent with one host-to-device copy per call: the frame's table record (a FearFrameView, a
         FearFrameYCbCr, a FearFrameYCbCrV210, a FearFrameYCbCrHDR, a FearFrameBayer, a FearFrameMono or a FearFrameRGB)
-        at byte 0, the FearTarget at byte 104, fear_decode_smooth's prev_size (w, h), penalty_k, window_influence and lr
-        as float64 at byte 168; then, on the device only, the score_size x score_size window."""
+        at byte 0, an Oriented frame's int32 code at byte 104, the FearTarget at byte 112, fear_decode_smooth's
+        prev_size (w, h), penalty_k, window_influence and lr as float64 at byte 176; then, on the device only, the
+        score_size x score_size window."""
         from . import _lib
 
         dev = self._device()
@@ -332,10 +339,11 @@ class FEARTracker(Tracker):
         "views" for a tensor, "ycbcr_hdr" for a YUV frame with a transfer (PQ, HLG), "ycbcr_v210" for another
         V210Frame, "ycbcr" for every other YUV frame, "bayer" for a BayerFrame, "mono" for a MonoFrame, "rgb" for an
         RGBFrame."""
+        frame = multi_tracker.stored(image)
         table = kind if kind in ("bayer", "mono", "rgb") else "views"
         if kind == "yuv":
-            table = "ycbcr_v210" if isinstance(image, multi_tracker.V210Frame) else "ycbcr"
-            if image.transfer is not None:
+            table = "ycbcr_v210" if isinstance(frame, multi_tracker.V210Frame) else "ycbcr"
+            if frame.transfer is not None:
                 table = "ycbcr_hdr"
         raw, dtype = st["inputs"].numpy(), multi_tracker.TABLE_DTYPES[table]
         multi_tracker.write_records(raw[:dtype.itemsize].view(dtype), [image], table)
@@ -347,6 +355,8 @@ class FEARTracker(Tracker):
             cfg = self.tracking_config
             raw[_SMOOTH_OFFSET:].view(np.float64)[:] = (prev_size[0], prev_size[1], cfg["penalty_k"],
                                                         cfg["window_influence"], cfg["lr"])
+        if isinstance(image, multi_tracker.Oriented):
+            raw[_ORIENT_OFFSET:_ORIENT_OFFSET + 4].view(np.int32)[0] = image.code
         st["dev_in"][:_DEVICE_INPUT_BYTES].copy_(st["inputs"], non_blocking=True)
         return table
 
@@ -359,6 +369,21 @@ class FEARTracker(Tracker):
         if multi_tracker.uses_agc([image], kind):
             fn = multi_tracker.RANGE_ENTRY_POINT
             _lib.check(getattr(_lib.load(), fn)(st["dev_in"].data_ptr(), 1, stream), fn)
+
+    @staticmethod
+    def _device_crop(st: dict, image, table: str, offset: float, size: int, out_ptr: int, stream) -> None:
+        """The crop-targets entry point of ``table`` on the staged record and FearTarget (one frame, one target), or
+        for an ``Oriented`` frame the oriented one reading the staged code."""
+        from . import _lib
+
+        lib, dp = _lib.load(), st["dev_in"].data_ptr()
+        if isinstance(image, multi_tracker.Oriented):
+            fn = multi_tracker.ORIENTED_ENTRY_POINTS[0]
+            _lib.check(getattr(lib, fn)(_lib.ORIENT_TABLES[table], dp, dp + _ORIENT_OFFSET, 1, dp + _TARGET_OFFSET, 1,
+                                        offset, size, out_ptr, stream), fn)
+        else:
+            fn = multi_tracker.ENTRY_POINTS[table][1]
+            _lib.check(getattr(lib, fn)(dp, 1, dp + _TARGET_OFFSET, 1, offset, size, out_ptr, stream), fn)
 
     def _device_mean_color(self, image, kind: str) -> np.ndarray:
         """np.mean(frame, axis=(0, 1)) of the RGB frame, bit for bit: exact per-channel sums on the device over H * W."""
@@ -393,12 +418,9 @@ class FEARTracker(Tracker):
         dev = st["device"]
         with torch.cuda.device(dev):
             table = self._stage_device_inputs(st, image, kind, box.astype(np.int32), image_ops.padding_color(mean_color))
-            crop_fn = multi_tracker.ENTRY_POINTS[table][1]
             stream = torch.cuda.current_stream(dev)
             self._device_frame_range(st, image, kind, stream.cuda_stream)
-            dp = st["dev_in"].data_ptr()
-            _lib.check(getattr(_lib.load(), crop_fn)(dp, 1, dp + _TARGET_OFFSET, 1, offset, size,
-                                                     st["tcrop"].data_ptr(), stream.cuda_stream), crop_fn)
+            self._device_crop(st, image, table, offset, size, st["tcrop"].data_ptr(), stream.cuda_stream)
             features = self.net.get_features(st["tcrop"])
             stream.synchronize()  # the pinned inputs are rewritten by the next call
         return features
@@ -419,8 +441,9 @@ class FEARTracker(Tracker):
         """One update on a device frame: crop-targets (N = 1, search_context, instance_size) -> fear_track_sized_u8 -> the
         plain decode, or with smooth the maps -> fear_decode_smooth_sized; one 48-byte record back.  The crop kernel reads the frame's record
         when it runs, so the graph (captured on the second update) keys on the table kind, smooth, the input buffer,
-        whether it starts with the mono range kernel and
-        net.generation(), not on the frame's address or shape: fresh decoder surfaces and a resolution change replay it."""
+        whether it starts with the mono range kernel, whether the frame is ``Oriented`` and net.generation(), not on the
+        frame's address, shape or orientation code: fresh decoder surfaces, a resolution change and a new rotation
+        replay it."""
         from . import _lib
 
         st = self._device_frame_state()
@@ -434,15 +457,14 @@ class FEARTracker(Tracker):
                 st["zf"].copy_(self._template_features)
                 st["zf_src"] = self._template_features
             lib = _lib.load()
-            crop_fn = multi_tracker.ENTRY_POINTS[table][1]
             agc = multi_tracker.uses_agc([image], kind)
+            oriented = isinstance(image, multi_tracker.Oriented)
 
             def step():
                 stream = torch.cuda.current_stream(dev).cuda_stream
                 self._device_frame_range(st, image, kind, stream)
                 dp = st["dev_in"].data_ptr()
-                _lib.check(getattr(lib, crop_fn)(dp, 1, dp + _TARGET_OFFSET, 1, float(cfg["search_context"]), size,
-                                                 st["crop"].data_ptr(), stream), crop_fn)
+                self._device_crop(st, image, table, float(cfg["search_context"]), size, st["crop"].data_ptr(), stream)
                 if not smooth:
                     return self.net.track_boxes(st["crop"], st["zf"])
                 maps = self.net.track(st["crop"], st["zf"])
@@ -453,7 +475,7 @@ class FEARTracker(Tracker):
                            "fear_decode_smooth_sized")
                 return st["smooth_boxes"]
 
-            key = (table, smooth, st["dev_in"].data_ptr(), self.net.generation(), agc)
+            key = (table, smooth, st["dev_in"].data_ptr(), self.net.generation(), agc, oriented)
             if key != st["key"]:  # another entry point, or stale workspace / weight pointers: warm up and capture again
                 st["graph"], st["key"], st["calls"] = None, key, 0
             use_graph = cfg.get("cuda_graph", True) and st["graph_ok"]

@@ -54,6 +54,9 @@
  *   fear_crop_targets_rgb_u8 / fear_advance_targets_rgb / fear_frame_sums_rgb_u8   the same three on RGB frames in any
  *                         channel order located by FearFrameRGB (BGR / BGRA / ABGR, x2rgb10, rgb48 / rgba64, planar
  *                         gbrp at 8 to 16 bits), each tap's channels read and mapped to 8 bits inside the crop
+ *   fear_crop_targets_oriented_u8 / fear_advance_targets_oriented   the crop and advance of any of the eight tables
+ *                         above on rotated and mirrored frames (90-degree turns, left-right flip), oriented inside
+ *                         the crop
  *   fear_gather_targets / fear_scatter_targets   the selected targets' rows and templates into compact step buffers,
  *                         and their new boxes back, for a step over the targets of some streams only
  *
@@ -576,6 +579,44 @@ int fear_crop_targets_rgb_u8(const FearFrameRGB* d_views, int F, FearTarget* d_t
 int fear_advance_targets_rgb(const FearBox* d_boxes, const FearFrameRGB* d_views, int F, FearTarget* d_targets, int N,
                              int instance_size, void* stream);
 int fear_frame_sums_rgb_u8(const FearFrameRGB* d_views, int F, uint64_t* d_sums, void* stream);
+
+/* Rotated and mirrored frames (phone video's display rotation, cameras mounted upside down or mirrored): the crop and
+ * advance entry points of any of the eight frame tables above, on each frame as it is shown rather than as it is
+ * stored.  `table` names the table d_table holds, one of the *_view_u8, *_yuv_u8, *_ycbcr_u8, *_ycbcr_v210_u8,
+ * *_ycbcr_hdr_u8, *_bayer_u8, *_mono_u8 and *_rgb_u8 families; the packed FearFrame and FearFrameYUV420 tables are not
+ * covered.  d_orient holds F int32 orientation codes in device memory, read when the kernels run (a captured graph sees
+ * each call's codes); a null d_orient means every code is 0, which gives exactly the table's plain entry point.
+ *
+ * A code in [0, 7] turns the stored H x W frame by 90 * (code & 3) degrees clockwise, after a left-right flip when
+ * code & 4 (numpy: np.rot90(rgb[:, ::-1] if code & 4 else rgb, -(code & 3))).  Display pixel (y, x) reads stored pixel
+ *     code & 3 = 0: (y, x)              display H x W
+ *                1: (H - 1 - x, y)      display W x H
+ *                2: (H - 1 - y, W - 1 - x)   display H x W
+ *                3: (x, W - 1 - y)      display W x H
+ * then xs = W - 1 - xs when code & 4.  Targets' boxes are in display coordinates and the advance clamps to the display
+ * size.  The conversion of each table (YUV matrix, v210 unpack, HDR tone map, demosaic, mono gain, RGB container) is
+ * applied at the stored pixel, so the crop equals the table's crop of the oriented converted frame bit for bit.  The
+ * mean colour and the mono code range do not depend on orientation: the table's fear_frame_sums_* and
+ * fear_frame_range_mono run on the stored frames unchanged.  A frame whose code is outside [0, 7] is treated like an
+ * entry the kernels cannot read: a padding-colour crop, and its target keeps its box.  ffmpeg's autorotate convention:
+ * a display-matrix rotation of r degrees (ffprobe's rotation=-90) is code (-r mod 360) / 90 (here 1).
+ * One launch each; handle-free, never allocate, never synchronise.  FEAR_EINVAL: an unknown table, plus the rules of
+ * the plain entry points. */
+enum {
+  FEAR_TABLE_VIEW = 0,
+  FEAR_TABLE_YUV = 1,
+  FEAR_TABLE_YCBCR = 2,
+  FEAR_TABLE_YCBCR_V210 = 3,
+  FEAR_TABLE_YCBCR_HDR = 4,
+  FEAR_TABLE_BAYER = 5,
+  FEAR_TABLE_MONO = 6,
+  FEAR_TABLE_RGB = 7
+};
+int fear_crop_targets_oriented_u8(int table, const void* d_table, const int32_t* d_orient, int F,
+                                  FearTarget* d_targets, int N, double offset, int out_size, uint8_t* d_crops,
+                                  void* stream);
+int fear_advance_targets_oriented(const FearBox* d_boxes, int table, const void* d_table, const int32_t* d_orient,
+                                  int F, FearTarget* d_targets, int N, int instance_size, void* stream);
 
 /* A step over some of the targets (FEARMultiTracker fed the frames of some streams only):
  *   fear_gather_targets -> crop (M) -> fear_track_u8 (B = M, Bz = M) -> advance (M) -> fear_scatter_targets
